@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the Emu2 image->text generate path on B200 (BASELINE.json configs[1]).
+"""bench.py — headline benchmark of the Emu2 image->text generate path on H100 (BASELINE.json configs[1]).
 
 One "step" = one full pass of the hot path over one synthetic request: 1x448x448 image -> EVA-CLIP-4B ViT ->
 project_up -> splice into the ~75-token prompt -> LLaMA-33B prefill -> 128 greedily decoded tokens (EOS suppressed so
@@ -7,6 +7,7 @@ exactly 128 steps run).  bf16 weights/activations, random-init weights of the re
 
   python bench.py --gpus N --steps K --warmup W          # this repo's CUDA engine (tensor parallel for N > 1)
   python bench.py --impl reference ...                   # the reference's CPU path, bounded sample (rank 0 only)
+  python bench.py ... --dump-outputs DIR                 # also write the last timed step's outputs as DIR/<name>.npy
 
 Prints ONE JSON line (see the task contract): value = device-resident tok/s, e2e = through the public API with host
 buffers, roofline = achieved HBM GB/s of the decode step's weight-streaming kernels vs MEASURED_PEAKS.json,
@@ -52,7 +53,7 @@ def kv_bytes_per_ctx_token(lc):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -112,7 +113,7 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -126,8 +127,8 @@ _CPU_KIND = "port"   # "reference" once the LLaMA part of the CPU arm ran throug
 
 
 def ncu_traffic():
-    """dram bytes / algorithmic bytes of the dominant kernel, from the ncu --set full capture committed this round
-    (profiles/r02_ncu_traffic.json, written by tools/ncu_traffic.py from the .ncu-rep of the gate/up GEMV launch)."""
+    """dram bytes / algorithmic bytes of the dominant kernel, from an ncu --set full capture stored as
+    profiles/r02_ncu_traffic.json (tools/ncu_traffic.py); None when there is none."""
     for name in ("r02_ncu_traffic.json",):
         p = os.path.join(ROOT, "profiles", name)
         if os.path.exists(p):
@@ -622,6 +623,8 @@ def run_cuda(args):
     clocks = sampler.stop() if rank == 0 else {}
     assert toks.shape[1] == NEW_TOKENS, toks.shape
     value = args.steps * NEW_TOKENS / (ms / 1000.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"tokens": toks})
 
     # end to end through the public API with host buffers
     one_step(False)
@@ -706,7 +709,7 @@ def run_cuda(args):
         try:
             del model
             torch.cuda.empty_cache()
-            bf16_peak = 1739.4
+            bf16_peak = 989.0  # H100 SXM data sheet, dense bf16 (not measured)
             try:
                 bf16_peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops_sustained"])
             except Exception:
@@ -750,7 +753,7 @@ def run_cuda(args):
                        "latents_sha1_per_pair": r.get("latents_sha1_per_pair"),
                        "roofline": {"bound": "tensor", "achieved": ach, "peak": bf16_peak * world, "unit": "TFLOP/s",
                                     "frac": ach / (bf16_peak * world), "flops_per_step": images * 2 * UNET_FLOP_PER_SAMPLE_STEP,
-                                    "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained x n_gpus"}}
+                                    "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (else the H100 SXM data sheet) x n_gpus"}}
         except Exception as ex:
             denoise = {"metric": "emu2gen_denoise_steps_per_s", "value": None, "error": repr(ex)}
 
@@ -779,8 +782,6 @@ def run_cuda(args):
         "roofline": {"bound": "hbm", "kernel": "gemv_tma_kernel (the weight-streaming launches of one decode step; "
                      ">95% of the CUDA-graphed step)", "achieved": achieved, "peak": peak, "unit": "GB/s",
                      "frac": achieved / peak, "peak_source": peak_src,
-                     # ncu --set full on the gate/up launch (profiles/r01_ncu_full_gemv_tma_gateup.txt): dram read
-                     # 477.3 MB + write 6.5 MB for 477.1 MB of weights -> x1.014 of the algorithmic bytes, per step here
                      "traffic": (alg_bytes * traffic_ratio) if traffic_ratio else None,
                      "traffic_source": ("ncu dram__bytes_read+write / algorithmic bytes of the gate_up launch (x%.3f, %s), "
                                         "scaled to the step" % (traffic_ratio, traffic_src)) if traffic_ratio else None,
@@ -905,7 +906,7 @@ def run_c4(args):
     kv_bytes = kv_bytes_per_ctx_token(lc) * (prompt_len + new_tokens / 2.0) * batch * beams
     alg_bytes = (llm_bytes_per_token(lc, vocab) + kv_bytes) / world
     peak, peak_src = measured_peaks()
-    bf16_peak = 1480.4
+    bf16_peak = 989.0  # H100 SXM data sheet, dense bf16 (not measured)
     try:
         bf16_peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops_sustained"])
     except Exception:
@@ -926,7 +927,7 @@ def run_c4(args):
             "gpu_launches": int(launches),
             "vit_ms": vit_ms, "prefill_ms": prefill_ms, "decode_ms": decode_ms, "decode_step_ms": step_ms,
             "tokens_sha1": hashlib.sha1(toks.to(torch.int64).numpy().tobytes()).hexdigest()[:16],
-            "roofline": {"bound": "hbm", "kernel": "wide decode step: gemm_skinny_kernel (tcgen05, weights as the 128-row operand, %d cache rows as N) + split-KV attn_decode_kernel through the beam row table" % (batch * beams),
+            "roofline": {"bound": "hbm", "kernel": "wide decode step: gemm_skinny_kernel (wgmma, weights as the 128-row operand, %d cache rows as N) + split-KV attn_decode_kernel through the beam row table" % (batch * beams),
                          "achieved": alg_bytes / (step_ms / 1000.0) / 1e9, "peak": peak, "unit": "GB/s",
                          "frac": alg_bytes / (step_ms / 1000.0) / 1e9 / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_step_per_gpu": alg_bytes, "traffic": None},
@@ -967,7 +968,7 @@ def run_c5(args):
         t = torch.tensor([ms_loop], device="cuda")
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms_loop = float(t.item())
-    bf16_peak = 1480.4
+    bf16_peak = 989.0  # H100 SXM data sheet, dense bf16 (not measured)
     try:
         bf16_peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops_sustained"])
     except Exception:
@@ -1009,6 +1010,14 @@ def emit(line):
     out.flush()
 
 
+def dump_outputs(d, arrays):
+    """What the timed path returned in its last step, as float64 .npy files (token ids are exact in float64)."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), t.detach().to(torch.float64).cpu().numpy())
+
+
 def main():
     quiet_stdout()
     ap = argparse.ArgumentParser()
@@ -1020,6 +1029,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-denoise", action="store_true", help="skip the Emu2-Gen denoise-loop measurement")
     ap.add_argument("--no-beam", action="store_true", help="skip the secondary 5-beam measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the generated token ids of the last one to DIR/tokens.npy (float64)")
     ap.add_argument("--config", default="c2", choices=["c2", "c4", "c5"],
                     help="c2 = BASELINE configs[1] (the headline, default); c4 = configs[3]: 8-shot interleaved prompts "
                          "(seq ~4k), batch 4, 5 beams, LLaMA-33B tensor parallel over --gpus (needs >= 2 GPUs for the KV cache); "

@@ -1,4 +1,4 @@
-"""emu_b200 — B200-native (sm_100a) engine for baaivision/Emu's multimodal generate path.
+"""emu_b200 — H100-native (sm_90a) engine for baaivision/Emu's multimodal generate path.
 
 Python host code mirrors the reference's public API — emu2.emu.EmuModel (generate / generate_image / encode_image),
 emu2.chat.EmuChatGeneration, emu2.diffusion.EmuVisualGeneration, emu1.modeling_emu.Emu, emu1.pipeline.EmuGenerationPipeline —

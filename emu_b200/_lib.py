@@ -114,7 +114,7 @@ def check(rc, engine=None):
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise EmuError("emu_b200 needs a CUDA device (B200 / sm_100a); there is no CPU fallback")
+        raise EmuError("emu_b200 needs a CUDA device (H100 / sm_90a); there is no CPU fallback")
 
 
 _DT = {torch.float32: DTYPE_F32, torch.bfloat16: DTYPE_BF16, torch.float16: DTYPE_F16}

@@ -1,4 +1,4 @@
-"""In-tree build of libemu_b200.so (nvcc, sm_100a only).
+"""In-tree build of libemu_b200.so (nvcc, sm_90a only).
 
 The shared library is the product: a C-ABI (include/emu_b200.h) over hand-written CUDA.  It is built next to
 the sources (emu_b200/libemu_b200.so) so that it travels to the GPU box with the repo snapshot.
@@ -14,7 +14,7 @@ LIB = os.path.join(HERE, "libemu_b200.so")
 STAMP = os.path.join(HERE, ".build_stamp")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--use_fast_math=false" if False else "-DEMU_B200",
 ]
 
@@ -61,7 +61,7 @@ def build(force=False, verbose=False):
             print(out.decode())
     if failed:
         raise RuntimeError("libemu_b200.so build failed")
-    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-lcudart", "-ldl", "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-lcudart", "-ldl", "-gencode", "arch=compute_90a,code=sm_90a"]
     subprocess.check_call(cmd)
     with open(STAMP, "w") as f:
         f.write(dig)

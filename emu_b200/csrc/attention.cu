@@ -460,7 +460,7 @@ int attn_prefill(const AttnArgs& a, cudaStream_t st) {
   if ((a.q_ts % 8) || (a.k_ts % 8) || (a.v_ts % 8) || (a.q_hs % 8) || (a.k_hs % 8) || (a.v_hs % 8) ||
       (a.q_bs % 8) || (a.k_bs % 8) || (a.v_bs % 8) || (a.o_ts % 2) || (a.o_hs % 2) || (a.o_bs % 2))
     return EMU_ERR_INVALID;
-  // dense problems go to the tcgen05 kernel (attention_tc.cu); EMU_ATTN=legacy forces this file's mma.sync kernel
+  // dense problems go to the wgmma kernel (attention_tc.cu); EMU_ATTN=legacy forces this file's mma.sync kernel
   static int legacy = -1;
   if (legacy < 0) {
     const char* v = getenv("EMU_ATTN");

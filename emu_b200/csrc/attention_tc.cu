@@ -1,26 +1,15 @@
-// emu_b200 — flash attention on the 5th-gen tensor cores (tcgen05 + TMEM), the dense-attention path of
+// emu_b200 — flash attention on the Hopper tensor cores (wgmma + TMA), the dense-attention path of
 //   * the EVA-CLIP ViT blocks            (reference: Emu2/emu/eva_vit.py:228-283 `Attention.forward`, non-causal, D=112)
 //   * the SD-XL UNet self-attention      (diffusers 0.24 `Attention` via Emu2/emu/diffusion.py:136-141, D=64, 4096/1024 tokens)
 //   * LLaMA prefill / `generate_image`   (transformers `LlamaAttention`, Emu2/emu/lm.py:37-41, causal + left padding, D=128)
 // softmax(scale * Q K^T [+ mask]) V with fp32 scores / statistics and bf16 probabilities — the same rounding points as
 // the mma.sync kernel in attention.cu, which stays the path for additive-bias (T5) and tiny problems.
 //
-// One CTA = 256 query rows (two 128-row tiles) of one (batch, head); K/V blocks stream through a 3-stage TMA ring and
-// are shared by both tiles (halves L2->SMEM traffic per flop).  Warp roles (384 threads = 3 warpgroups):
-//   warp 0      TMA producer: Q once, then K_j / V_j tiles (4-D tensor maps over the strided [B, N, H, D] views, 128B
-//               swizzle, out-of-bounds rows / head-dim padding arrive as zeros)
-//   warp 1      single-thread tcgen05.mma issuer: S_t = Q_t K_j^T (both operands K-major) and O_t += P_t V_j (V is used
-//               in place as an MN-major B operand — no transpose pass), accumulators in TMEM
-//   warps 2-3   idle (they complete warpgroup 0 so that it can hand its registers over with setmaxnreg)
-//   warps 4-7   softmax for tile 0, warps 8-11 for tile 1: thread == query row (TMEM lane); S row -> registers, online
-//               max/sum, P (bf16) written to swizzled SMEM as the A operand of the second MMA.
-// Warpgroup 0 shrinks to 72 registers per thread and the two softmax warpgroups grow to 216 (setmaxnreg; 128 x 72 + 256 x 216 = the 384 x 168 registers the CTA was launched with — asking for more would block forever), so the 128
-// scores of a row live in registers without spills.  The softmax inner loop is written for issue slots, the scarce
-// resource of a lone warp per scheduler: packed f32x2 FMA / ADD (one instruction per two scores), 3-input max, one
-// 16-byte st.shared per 8 probabilities (conflict-free under the 128B swizzle).
-// O accumulates in TMEM across KV blocks.  The running max used for the exponent is only advanced when it grew by more
-// than 2^8 (exact: the final 1/l normalisation uses the same stale max), so the O rescale (TMEM ld/st) is rare.
-// While tile 0's softmax runs, the tensor core works on tile 1 and vice versa.
+// One CTA = 128 query rows of one (batch, head); K/V blocks stream through a 3-stage TMA ring (4-D tensor maps over the
+// strided [B, N, H, D] views, 128B swizzle, out-of-bounds rows / head-dim padding arrive as zeros) and are shared by the
+// two consumer warpgroups (64 query rows each).  Per KV block a consumer runs S = Q K^T as wgmma from shared memory,
+// the online softmax on the S fragment in registers, and O += P V as wgmma with P as the register A operand and V used in
+// place as an MN-major B operand (no transpose pass); O accumulates in registers.
 #include <cstdlib>
 
 #include <cuda.h>
@@ -28,6 +17,7 @@
 
 #include "common.cuh"
 #include "ops.h"
+#include "wgmma.cuh"
 
 namespace emu {
 
@@ -40,22 +30,15 @@ constexpr int kAtStages = 3;
 
 template <int DT, int BN>
 struct AtCfg {
-  static constexpr int kThreads = 384;             // warpgroup 0 = {TMA, MMA, 2 idle}, warpgroups 1/2 = softmax of tile 0/1
+  static constexpr int kThreads = 384;             // warpgroup 0 = TMA producer, warpgroups 1/2 = query rows 0..63 / 64..127
   static constexpr int kDC = DT / 64;              // 64-wide head-dim chunks (one 128 B swizzle row each)
-  static constexpr int kKC = BN / 64;              // 64-wide key chunks of P
-  static constexpr int kQBytes = 128 * DT * 2;     // one Q tile
+  static constexpr int kQBytes = 128 * DT * 2;     // the Q tile
   static constexpr int kKVBytes = BN * DT * 2;     // one K (or V) block
-  static constexpr int kPBytes = 128 * BN * 2;     // one P tile
-  static constexpr int kOffK = 2 * kQBytes;
+  static constexpr int kOffK = kQBytes;
   static constexpr int kOffV = kOffK + kAtStages * kKVBytes;
-  static constexpr int kOffP = kOffV + kAtStages * kKVBytes;
-  static constexpr int kOffBar = kOffP + 2 * kPBytes;
+  static constexpr int kOffBar = kOffV + kAtStages * kKVBytes;
   static constexpr int kSmem = kOffBar + 32 * 8 + 1024;  // + 1024 B alignment slack
-  static constexpr int kTmemS = 0;                 // S_t at t*BN
-  static constexpr int kTmemO = 2 * BN;            // O_t at 2*BN + t*DT
-  static constexpr int kTmemCols = 512;
-  static_assert(BN % 32 == 0 && DT % 32 == 0, "rows are moved in 32-column TMEM chunks");
-  static_assert(2 * BN + 2 * DT <= 512, "TMEM budget");
+  static_assert(BN % 16 == 0 && DT % 64 == 0, "tile shapes");
   static_assert(kSmem <= 227 * 1024, "SMEM budget");
 };
 
@@ -76,78 +59,6 @@ __device__ __forceinline__ void load_rows(void* dst, const CUtensorMap* m, uint6
   else tma_load_4d(dst, m, bar, d0, tok, head, batch);
 }
 
-__device__ __forceinline__ uint64_t umma_desc_sw128_ex(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-// (Tried and removed: FlashAttention-4's trick of evaluating a share of the exponentials with a polynomial on the FMA
-//  pipe — slower at every share in round 1, when the softmax warps were instruction-issue bound (729 issue slots per
-//  128-key block and row: 32-bit generic P stores, scalar FMA / ADD, spills under the 168-register cap).  Also removed:
-//  splitting each row over two softmax warps (330 vs 478 TFLOP/s).)
-
-// packed fp32 pairs: one issue slot for two scores (Blackwell FFMA2 / FADD2)
-__device__ __forceinline__ uint64_t pack2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t fadd2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ void sts128(uint32_t saddr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_s(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_s(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-
 template <int DT, int BN>
 __global__ void __launch_bounds__(AtCfg<DT, BN>::kThreads, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -161,25 +72,13 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   uint64_t* k_empty = k_full + kAtStages;  // [3]
   uint64_t* v_full = k_empty + kAtStages;
   uint64_t* v_empty = v_full + kAtStages;
-  uint64_t* s_full = v_empty + kAtStages;  // [2]
-  uint64_t* s_free = s_full + 2;
-  uint64_t* p_ready = s_free + 2;
-  uint64_t* o_done = p_ready + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 256, head = blockIdx.y, batch = blockIdx.z;
+  const int q0 = blockIdx.x * 128, head = blockIdx.y, batch = blockIdx.z;
   const int off = p.Nk - p.Nq;
-
-  // KV blocks needed per 128-row tile (0 when the tile lies entirely past Nq)
-  auto blocks_for = [&](int qlo) -> int {
-    if (qlo >= p.Nq) return 0;
-    int kmax = p.Nk - 1;
-    if (p.causal) kmax = min(kmax, min(qlo + 127, p.Nq - 1) + off);
-    return kmax < 0 ? 0 : kmax / BN + 1;
-  };
-  const int nb0 = blocks_for(q0), nb1 = blocks_for(q0 + 128);
-  const int nbmax = max(nb0, nb1);
+  int kmax = p.Nk - 1;  // last key any query row of this CTA may see
+  if (p.causal) kmax = min(kmax, min(q0 + 127, p.Nq - 1) + off);
+  const int nb = kmax < 0 ? 0 : kmax / BN + 1;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -188,254 +87,136 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     mbar_init(q_full, 1);
     for (int i = 0; i < kAtStages; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
+      mbar_init(&k_empty[i], 8);  // lane 0 of every consumer warp
       mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
-    }
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&s_full[t], 1);
-      mbar_init(&s_free[t], 4);
-      mbar_init(&p_ready[t], 4);
-      mbar_init(&o_done[t], 1);
+      mbar_init(&v_empty[i], 8);
     }
     mbar_fence_init();
   }
   if (p.pdl) pdl_launch_dependents();
-  if (warp == 1) tmem_alloc(tmem_slot, C::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-    if (warp == 0) {
-      // ===================== TMA producer =====================
-      if (lane == 0 && nbmax > 0) {
-        if (p.pdl) pdl_wait();  // Q/K/V are the predecessor's output; all stores of this kernel happen after these loads
-        mbar_expect_tx(q_full, 2 * C::kQBytes);
-        for (int t = 0; t < 2; ++t)
-          for (int c = 0; c < C::kDC; ++c)
-            load_rows(smem + t * C::kQBytes + c * (128 * 128), &tmQ, q_full, c * 64, q0 + t * 128, head, batch, p.q_hf);
-        for (int j = 0; j < nbmax; ++j) {
-          const int s = j % kAtStages;
-          const uint32_t ph = (uint32_t)(j / kAtStages) & 1u;
-          mbar_wait(&k_empty[s], ph ^ 1);
-          mbar_expect_tx(&k_full[s], C::kKVBytes);
-          for (int c = 0; c < C::kDC; ++c)
-            load_rows(smem + C::kOffK + s * C::kKVBytes + c * (BN * 128), &tmK, &k_full[s], c * 64, j * BN, head, batch, p.k_hf);
-          mbar_wait(&v_empty[s], ph ^ 1);
-          mbar_expect_tx(&v_full[s], C::kKVBytes);
-          for (int c = 0; c < C::kDC; ++c)
-            load_rows(smem + C::kOffV + s * C::kKVBytes + c * (BN * 128), &tmV, &v_full[s], c * 64, j * BN, head, batch, p.v_hf);
-        }
-      }
-    } else if (warp == 1) {
-      // ===================== MMA issuer =====================
-      if (lane == 0 && nbmax > 0) {
-        constexpr uint32_t idesc_s = umma_idesc_bf16(128, BN);
-        constexpr uint32_t idesc_o = umma_idesc_bf16(128, DT) | (1u << 16);  // B (= V) is MN-major
-        const uint32_t sQ = smem_u32(smem), sK = smem_u32(smem + C::kOffK), sV = smem_u32(smem + C::kOffV),
-                       sP = smem_u32(smem + C::kOffP);
-        auto issue_S = [&](int t, int stage) {
-          const uint32_t d = tmem_base + C::kTmemS + t * BN;
-#pragma unroll
-          for (int c = 0; c < C::kDC; ++c) {
-            const uint64_t da = umma_desc_sw128(sQ + t * C::kQBytes + c * (128 * 128));
-            const uint64_t db = umma_desc_sw128(sK + stage * C::kKVBytes + c * (BN * 128));
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_bf16(d, da + 2 * k, db + 2 * k, idesc_s, (c | k) != 0);
-          }
-        };
-        auto issue_PV = [&](int t, int stage, bool acc) {
-          const uint32_t d = tmem_base + C::kTmemO + t * DT;
-#pragma unroll
-          for (int kk = 0; kk < BN / 16; ++kk) {
-            const uint64_t da = umma_desc_sw128(sP + t * C::kPBytes + (kk >> 2) * (128 * 128)) + 2 * (kk & 3);
-            // V block in place: rows = keys (the MMA K dim), 64-wide d chunks BN*128 B apart (LBO), 8-key groups 1024 B (SBO)
-            const uint64_t db = umma_desc_sw128_ex(sV + stage * C::kKVBytes + kk * 2048, BN * 128, 1024);
-            umma_bf16(d, da, db, idesc_o, (acc || kk > 0) ? 1u : 0u);
-          }
-        };
-        mbar_wait(q_full, 0);
-        mbar_wait(&k_full[0], 0);
-        tc_fence_after();
-        if (nb0 > 0) { issue_S(0, 0); umma_commit(&s_full[0]); }
-        if (nb1 > 0) { issue_S(1, 0); umma_commit(&s_full[1]); }
-        umma_commit(&k_empty[0]);
-        for (int j = 0; j < nbmax; ++j) {
-          const int sv = j % kAtStages;
-          const uint32_t phv = (uint32_t)(j / kAtStages) & 1u;
-          const bool has_next = j + 1 < nbmax;
-          const int sk = (j + 1) % kAtStages;
-          const uint32_t phk = (uint32_t)((j + 1) / kAtStages) & 1u;
-          if (has_next) mbar_wait(&k_full[sk], phk);
-          mbar_wait(&v_full[sv], phv);
-          tc_fence_after();
-#pragma unroll
-          for (int t = 0; t < 2; ++t) {
-            const int nbt = t ? nb1 : nb0;
-            if (j + 1 < nbt) {
-              mbar_wait(&s_free[t], (uint32_t)j & 1u);
-              tc_fence_after();
-              issue_S(t, sk);
-              umma_commit(&s_full[t]);
-            }
-            if (j < nbt) {
-              mbar_wait(&p_ready[t], (uint32_t)j & 1u);
-              tc_fence_after();
-              issue_PV(t, sv, j > 0);
-              umma_commit(&o_done[t]);
-            }
-          }
-          if (has_next) umma_commit(&k_empty[sk]);
-          umma_commit(&v_empty[sv]);
-        }
+    // ===================== TMA producer =====================
+    if (warp == 0 && lane == 0 && nb > 0) {
+      if (p.pdl) pdl_wait();  // Q/K/V are the predecessor's output; all stores of this kernel happen after these loads
+      mbar_expect_tx(q_full, C::kQBytes);
+      for (int c = 0; c < C::kDC; ++c) load_rows(smem + c * (128 * 128), &tmQ, q_full, c * 64, q0, head, batch, p.q_hf);
+      for (int j = 0; j < nb; ++j) {
+        const int s = j % kAtStages;
+        const uint32_t ph = (uint32_t)(j / kAtStages) & 1u;
+        mbar_wait(&k_empty[s], ph ^ 1);
+        mbar_expect_tx(&k_full[s], C::kKVBytes);
+        for (int c = 0; c < C::kDC; ++c)
+          load_rows(smem + C::kOffK + s * C::kKVBytes + c * (BN * 128), &tmK, &k_full[s], c * 64, j * BN, head, batch, p.k_hf);
+        mbar_wait(&v_empty[s], ph ^ 1);
+        mbar_expect_tx(&v_full[s], C::kKVBytes);
+        for (int c = 0; c < C::kDC; ++c)
+          load_rows(smem + C::kOffV + s * C::kKVBytes + c * (BN * 128), &tmV, &v_full[s], c * 64, j * BN, head, batch, p.v_hf);
       }
     }
   } else {
-    // ===================== softmax / correction / epilogue warpgroups =====================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-    const int t = (warp - 4) >> 2;  // query tile of this warpgroup
-    const int quad = warp & 3;      // TMEM lane quarter this warp may access
-    const int r = quad * 32 + lane;
-    const int qi = q0 + t * 128 + r;
-    const uint32_t lane_base = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const uint32_t tS = lane_base + C::kTmemS + t * BN;
-    const uint32_t tO = lane_base + C::kTmemO + t * DT;
-    // this row inside the swizzled P tile: 8-row groups 1024 B apart, 128 B per row, 16 B chunk index ^ (row & 7)
-    const uint32_t Pt = smem_u32(smem + C::kOffP) + t * C::kPBytes + (r >> 3) * 1024 + (r & 7) * 128;
-    const uint32_t swz = (uint32_t)(r & 7) << 4;
-    const uint32_t b_s_full = smem_u32(&s_full[t]), b_s_free = smem_u32(&s_free[t]), b_p_ready = smem_u32(&p_ready[t]),
-                   b_o_done = smem_u32(&o_done[t]);
-    const int n = t ? nb1 : nb0;
+    // ===================== consumers: 64 query rows each =====================
+    // S / O fragments (wgmma accumulator layout): rows qi[h] = q0 + 64 wg + 16 (warp % 4) + lane / 4 + 8 h, columns
+    // 8 jj + 2 (lane % 4) + e at index 4 jj + 2 h + e.  P is re-packed from the S fragment into the register A operand.
+    const int wg = (warp >> 2) - 1;
+    const int t = lane & 3;
+    int qi[2];
+    qi[0] = q0 + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    qi[1] = qi[0] + 8;
+    const uint32_t sQ = smem_u32(smem) + wg * (64 * 128), sK = smem_u32(smem + C::kOffK), sV = smem_u32(smem + C::kOffV);
     const float c = p.scale_log2;
-    const uint64_t c2 = pack2(c, c);
     const int lo = p.kv_start ? p.kv_start[batch] : 0;
-    const int hi = p.causal ? min(p.Nk - 1, qi + off) : p.Nk - 1;
-    float m_run = -INFINITY, m_used = -INFINITY;
-    uint64_t l2[4];  // 8 independent row-sum chains, packed in pairs
+    int hi[2];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) l2[i] = 0ull;
-    for (int j = 0; j < n; ++j) {
-      mbar_wait_s(b_s_full, (uint32_t)j & 1u);
-      tc_fence_after();
-      float s[BN];
+    for (int h = 0; h < 2; ++h) hi[h] = p.causal ? min(p.Nk - 1, qi[h] + off) : p.Nk - 1;
+    float o[DT / 2];
 #pragma unroll
-      for (int cc = 0; cc < BN / 32; ++cc) tmem_ld_32x32(tS + cc * 32, reinterpret_cast<uint32_t*>(s) + cc * 32);
-      tmem_ld_wait();
-      tc_fence_before();
+    for (int i = 0; i < DT / 2; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    if (nb > 0) mbar_wait(q_full, 0);
+    for (int j = 0; j < nb; ++j) {
+      const int s = j % kAtStages;
+      const uint32_t ph = (uint32_t)(j / kAtStages) & 1u;
+      // ---- S = Q K_j^T ----
+      float sc[BN / 2];
+      mbar_wait(&k_full[s], ph);
+      wgmma_fence();
+#pragma unroll
+      for (int cc = 0; cc < C::kDC; ++cc) {
+        const uint64_t da = wgmma_desc_sw128(sQ + cc * (128 * 128));
+        const uint64_t db = wgmma_desc_sw128(sK + s * C::kKVBytes + cc * (BN * 128));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) WgmmaSS<BN>::run(sc, da + 2 * k, db + 2 * k, (cc | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive_s(b_s_free);
+      if (lane == 0) mbar_arrive(&k_empty[s]);
+      // ---- mask, online softmax (log2 domain) ----
       const int k0 = j * BN;
-      if (k0 < lo || k0 + BN - 1 > hi) {
+      float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-        for (int i = 0; i < BN; ++i) s[i] = (k0 + i < lo || k0 + i > hi) ? -INFINITY : s[i];
+      for (int i = 0; i < BN / 2; ++i) {
+        const int h = (i >> 1) & 1;
+        const int kj = k0 + 8 * (i >> 2) + 2 * t + (i & 1);
+        const float x = (kj >= lo && kj <= hi[h]) ? sc[i] * c : -INFINITY;
+        sc[i] = x;
+        mx[h] = fmaxf(mx[h], x);
       }
-      // 8 independent max chains (a single long dependent chain is pure latency for a lone warp per sub-partition);
-      // fmaxf(fmaxf(a, b), c) folds into one 3-input FMNMX3
-      float mx8[8];
+      float m_use[2], corr[2];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) mx8[i] = fmaxf(s[i], s[i + 8]);
-#pragma unroll
-      for (int i = 16; i + 8 < BN; i += 16) {
-#pragma unroll
-        for (int u = 0; u < 8; ++u) mx8[u] = fmaxf(fmaxf(mx8[u], s[i + u]), s[i + 8 + u]);
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        const float m_new = fmaxf(m_run[h], mx[h]);
+        m_use[h] = (m_new == -INFINITY) ? 0.f : m_new;  // fully masked row so far
+        corr[h] = (m_run[h] == -INFINITY) ? 0.f : ex2_approx_ftz(m_run[h] - m_use[h]);
+        m_run[h] = m_new;
       }
-      if ((BN / 8) & 1) {
+      float rs[2] = {0.f, 0.f};
+      uint32_t pa[BN / 16][4];
 #pragma unroll
-        for (int u = 0; u < 8; ++u) mx8[u] = fmaxf(mx8[u], s[BN - 8 + u]);
+      for (int jj = 0; jj < BN / 8; ++jj) {
+        const float p0 = ex2_approx_ftz(sc[4 * jj] - m_use[0]), p1 = ex2_approx_ftz(sc[4 * jj + 1] - m_use[0]);
+        const float p2 = ex2_approx_ftz(sc[4 * jj + 2] - m_use[1]), p3 = ex2_approx_ftz(sc[4 * jj + 3] - m_use[1]);
+        rs[0] += p0 + p1;
+        rs[1] += p2 + p3;
+        pa[jj >> 1][(jj & 1) * 2] = pack_bf16(p0, p1);
+        pa[jj >> 1][(jj & 1) * 2 + 1] = pack_bf16(p2, p3);
       }
-      const float mx = fmaxf(fmaxf(fmaxf(mx8[0], mx8[1]), fmaxf(mx8[2], mx8[3])), fmaxf(fmaxf(mx8[4], mx8[5]), fmaxf(mx8[6], mx8[7])));
-      const float m_new = fmaxf(m_run, mx);
-      m_run = m_new;
-      if (j > 0) {
-        mbar_wait_s(b_o_done, (uint32_t)(j - 1) & 1u);  // PV_{j-1} retired: O is quiescent and P may be overwritten
-        tc_fence_after();
-      }
-      const bool need = (m_new - m_used) * c > 8.f;
-      if (__any_sync(0xffffffffu, need)) {
-        float f = 1.f;
-        if (m_new != -INFINITY) {
-          f = (m_used == -INFINITY) ? 0.f : ex2_approx((m_used - m_new) * c);
-          m_used = m_new;
-        }
-        const uint64_t f2 = pack2(f, f);
-        const uint64_t z2 = 0ull;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) l2[i] = ffma2(l2[i], f2, z2);
-        if (j > 0) {
-#pragma unroll 1
-          for (int cc = 0; cc < DT / 32; ++cc) {
-            uint32_t v[32];
-            tmem_ld_32x32(tO + cc * 32, v);
-            tmem_ld_wait();
+      for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * corr[h] + rs[h];
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * f);
-            tmem_st_32x32(tO + cc * 32, v);
-          }
-          tmem_st_wait();
-        }
-      }
-      const float mu = (m_used == -INFINITY) ? 0.f : m_used * c;
-      const uint64_t nmu2 = pack2(-mu, -mu);
+      for (int i = 0; i < DT / 2; ++i) o[i] *= corr[(i >> 1) & 1];
+      // ---- O += P V_j : V is used in place as an MN-major B operand (64-wide d chunks BN*128 B apart, 8-key groups 1 KB) ----
+      mbar_wait(&v_full[s], ph);
+      wgmma_fence();
 #pragma unroll
-      for (int g = 0; g < BN / 8; ++g) {
-        float e[8];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          float x0, x1;
-          unpack2(ffma2(pack2(s[g * 8 + 2 * i], s[g * 8 + 2 * i + 1]), c2, nmu2), x0, x1);
-          e[2 * i] = ex2_approx(x0);
-          e[2 * i + 1] = ex2_approx(x1);
-          l2[i] = fadd2(l2[i], pack2(e[2 * i], e[2 * i + 1]));
-        }
-        // keys g*8 .. g*8+7 of this row: 64-key chunk g >> 3 (16 KB apart), 16-byte slot (g & 7) ^ (row & 7)
-        sts128(Pt + (g >> 3) * (128 * 128) + ((((uint32_t)g & 7u) << 4) ^ swz), pack_bf16(e[0], e[1]), pack_bf16(e[2], e[3]),
-               pack_bf16(e[4], e[5]), pack_bf16(e[6], e[7]));
-      }
-      fence_proxy_async_smem();  // generic-proxy P stores -> visible to the tensor core's async-proxy reads
-      tc_fence_before();
+      for (int kk = 0; kk < BN / 16; ++kk)
+        WgmmaRS<DT, 1>::run(o, pa[kk], wgmma_desc_sw128(sV + s * C::kKVBytes + kk * 2048, BN * 128, 1024), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive_s(b_p_ready);
+      if (lane == 0) mbar_arrive(&v_empty[s]);
     }
-    if (n > 0) {
-      float la[8];
+    // ---- normalise and store ----
 #pragma unroll
-      for (int i = 0; i < 4; ++i) unpack2(l2[i], la[2 * i], la[2 * i + 1]);
-      const float l = ((la[0] + la[1]) + (la[2] + la[3])) + ((la[4] + la[5]) + (la[6] + la[7]));
-      mbar_wait_s(b_o_done, (uint32_t)(n - 1) & 1u);
-      tc_fence_after();
-      const float inv = l > 0.f ? 1.f / l : 0.f;
-      bf16* dst = p.out + (long)batch * p.o_bs + (long)qi * p.o_ts + (long)head * p.o_hs;
-#pragma unroll 1
-      for (int cc = 0; cc < DT / 32; ++cc) {
-        uint32_t v[32];
-        tmem_ld_32x32(tO + cc * 32, v);
-        tmem_ld_wait();
-        if (qi < p.Nq) {
+    for (int h = 0; h < 2; ++h) {
+      l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+      l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+    }
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            const int col = cc * 32 + g * 8;
-            if (col < p.D) {  // D % 8 == 0
-              uint4 w;
-              w.x = pack_bf16(__uint_as_float(v[g * 8 + 0]) * inv, __uint_as_float(v[g * 8 + 1]) * inv);
-              w.y = pack_bf16(__uint_as_float(v[g * 8 + 2]) * inv, __uint_as_float(v[g * 8 + 3]) * inv);
-              w.z = pack_bf16(__uint_as_float(v[g * 8 + 4]) * inv, __uint_as_float(v[g * 8 + 5]) * inv);
-              w.w = pack_bf16(__uint_as_float(v[g * 8 + 6]) * inv, __uint_as_float(v[g * 8 + 7]) * inv);
-              *reinterpret_cast<uint4*>(dst + col) = w;
-            }
-          }
-        }
+    for (int h = 0; h < 2; ++h) {
+      if (qi[h] >= p.Nq) continue;
+      const float inv = l_run[h] > 0.f ? 1.f / l_run[h] : 0.f;
+      bf16* dst = p.out + (long)batch * p.o_bs + (long)qi[h] * p.o_ts + (long)head * p.o_hs;
+#pragma unroll
+      for (int jj = 0; jj < DT / 8; ++jj) {
+        const int d = 8 * jj + 2 * t;
+        if (d < p.D) *reinterpret_cast<uint32_t*>(dst + d) = pack_bf16(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::kTmemCols);
   }
 }
 
@@ -457,7 +238,7 @@ int launch_attn_tc(const AttnArgs& a, cudaStream_t st) {
   p.kv_start = a.kv_start; p.Nq = a.Nq; p.Nk = a.Nk; p.D = a.D; p.causal = a.causal;
   p.scale_log2 = a.scale * 1.4426950408889634f;
   p.pdl = g_pdl_chain;
-  dim3 grid((a.Nq + 255) / 256, a.H, a.B);
+  dim3 grid((a.Nq + 127) / 128, a.H, a.B);
   return launch_kernel(attn_tc_kernel<DT, BN>, grid, dim3(C::kThreads), C::kSmem, st, p.pdl, tq, tk, tv, p);
 }
 

@@ -35,7 +35,7 @@ extern "C" int emu_op_gemm_skinny(const void* X, int ldx, const void* W, int ldw
 
 extern "C" int emu_debug_gemm_phases(const void* A, int lda, const void* W, int ldw, int M, int N, int K, const void* bias,
                                      const void* residual, int ldr, int epi_mode, void* C, int ldc, int force_bn,
-                                     unsigned long long* stamps /*[148][8] device*/, emu_stream_t s) {
+                                     unsigned long long* stamps /*[grid][8] device*/, emu_stream_t s) {
   if (!A || !W || !C || !stamps) return EMU_ERR_INVALID;
   GemmEpilogue e;
   e.C = C; e.ldc = ldc; e.bias = (const bf16*)bias; e.residual = (const bf16*)residual; e.ldr = ldr;
@@ -68,7 +68,7 @@ extern "C" int emu_op_gemv(const void* W, int N, int K, const void* x, int ldx, 
 
 extern "C" int emu_debug_gemv_phases(const void* W, int N, int K, const void* x, int ldx, int B, const void* norm_w, float eps,
                                      int mode, const void* residual, int ldr, void* y, int ldy, int pdl,
-                                     unsigned long long* stamps /*[148][8] device*/, emu_stream_t s) {
+                                     unsigned long long* stamps /*[grid][8] device*/, emu_stream_t s) {
   if (!W || !x || !y || !stamps) return EMU_ERR_INVALID;
   GemvArgs a;
   a.W = (const bf16*)W; a.N = N; a.K = K; a.x = (const bf16*)x; a.ldx = ldx; a.B = B;

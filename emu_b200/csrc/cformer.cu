@@ -7,7 +7,7 @@
 // :422-424), T5LayerFF / T5DenseActDense :352-365 (ReLU), T5Block :766-905, T5Stack.forward :1100-1366 (causal mask
 // for the decoder self-attention, final_layer_norm).
 //
-// All contractions are tiny (32 queries): they go through the same tcgen05 GEMM and flash-attention kernels as the
+// All contractions are tiny (32 queries): they go through the same wgmma GEMM and flash-attention kernels as the
 // rest of the engine (additive bias + causal mask for self-attention, plain cross-attention over the 257 ViT tokens).
 #include <math.h>
 

@@ -1,8 +1,8 @@
-// emu_b200 — shared device helpers (sm_100a only).
+// emu_b200 — shared device helpers (sm_90a only).
 //
-// PTX wrappers for mbarrier / TMA / tcgen05 / TMEM, plus small numeric helpers
+// PTX wrappers for mbarrier / TMA / clusters, plus small numeric helpers
 // used by every kernel in csrc/.  Nothing here is generic across architectures:
-// the library is compiled with -gencode arch=compute_100a,code=sm_100a only.
+// the library is compiled with -gencode arch=compute_90a,code=sm_90a only.
 #pragma once
 
 #include <cuda.h>
@@ -15,7 +15,7 @@ namespace emu {
 typedef __nv_bfloat16 bf16;
 typedef __nv_bfloat162 bf162;
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // ----------------------------------------------------------------------------------------------
 // error plumbing: the C ABI never throws/aborts; kernels are launched through EMU_CUDA_OK
@@ -39,7 +39,7 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 }
 __device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 // two values at once: one F2FP pack + two bit moves on the ALU pipe instead of two F2F conversions on the quarter-rate
-// XU pipe (the GEMM epilogues round 2-3 times per output: this was their bottleneck, profiles/r02_gemm_phases_*.txt)
+// XU pipe (the GEMM epilogues round 2-3 times per output)
 __device__ __forceinline__ void round_bf16x2(float& a, float& b) {
   const uint32_t p = pack_bf16(a, b);
   a = bf16_lo(p);
@@ -185,6 +185,14 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster (may be this CTA)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n.reg .b32 ra;\nmapa.shared::cluster.u32 ra, %0, %1;\nmbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n}\n" ::"r"(
+          smem_u32(bar)),
+      "r"(cta)
+      : "memory");
+}
 // all threads of all CTAs in the cluster
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
@@ -197,81 +205,6 @@ __device__ __forceinline__ void bulk_load_1d(void* smem, const void* gmem, uint3
                "l"(gmem), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-
-// ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// whole-warp: allocate `ncols` (power of two >= 32) TMEM columns, base address written to *smem_out
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_out, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_out)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-
-// K-major, 128-byte-swizzled operand tile: rows of 64 bf16 (128 B); 8-row groups are 1024 B apart.
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48),
-//  layout_type [61,64) with SWIZZLE_128B = 2.)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
-  d |= (uint64_t)1 << 16;             // LBO: unused for swizzled K-major, canonical value 1
-  d |= (uint64_t)(1024 >> 4) << 32;   // SBO: 8 rows x 128 B
-  d |= (uint64_t)1 << 46;             // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;             // SWIZZLE_128B
-  return d;
-}
-
-// instruction descriptor, kind::f16: D=f32, A=B=bf16, both K-major, dense, no negate
-__device__ __host__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// same, but the arrive lands on the barrier at this offset in every CTA of cta_mask
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes (lane quarter = warp_id % 4), 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
 // legacy warp MMA (used only where the contraction is tiny or bandwidth-bound: GEMV, attention)

@@ -384,7 +384,7 @@ extern "C" void emu_engine_destroy(EmuEngine* e) {
 
 extern "C" const char* emu_last_error(EmuEngine* e) { return e ? e->err.c_str() : "null engine"; }
 extern "C" uint64_t emu_launch_count(void) { return g_launches; }
-extern "C" const char* emu_version(void) { return "emu_b200 0.1 (sm_100a)"; }
+extern "C" const char* emu_version(void) { return "emu_b200 0.1 (sm_90a)"; }
 
 // ================================================================================================
 // weight ingestion
@@ -881,7 +881,7 @@ extern "C" int emu_llm_prefill(EmuEngine* e, const void* inputs_embeds, const in
     count_launch();
   }
   if (logits_last && B > 8) {
-    // more rows than the skinny GEMV takes: final norm of the last position of every sequence, then the tcgen05 GEMM
+    // more rows than the skinny GEMV takes: final norm of the last position of every sequence, then the wgmma GEMM
     EMU_TRY(e->ensure(e->pf_last, (size_t)B * Hd * 2));
     bf16* last = (bf16*)e->pf_last.p;
     if (cudaMemcpy2DAsync(last, (size_t)Hd * 2, h + (size_t)(N - 1) * Hd, (size_t)N * Hd * 2, (size_t)Hd * 2, B,
@@ -960,7 +960,7 @@ static int row_parallel_tail(EmuEngine* e, GemvArgs& g, bf16* h, int B, int Hd, 
 }
 
 // One decode step for MORE than 8 cache rows (BASELINE config 4: 4 prompts x 5 beams = 20 rows): the skinny GEMV takes at most
-// 8 activation rows, so the projections run on the tcgen05 GEMM with M = B (one 128-row tile, weights streamed once — still
+// 8 activation rows, so the projections run on the wgmma GEMM with M = B (one 128-row tile, weights streamed once — still
 // HBM-bound), RoPE + cache append as in prefill but at the device-side slot, the split-KV decode attention over the cache,
 // NCCL all-reduce on the row-parallel outputs under tensor parallelism.  Same arithmetic / rounding points as the narrow
 // path; captured into the same CUDA-graph cache.

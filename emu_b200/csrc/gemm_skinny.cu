@@ -1,24 +1,21 @@
-// emu_b200 — tcgen05 skinny GEMM for the wide decode step:  C[B,N] = epilogue( X[B,K] · W[N,K]^T ),  B <= 32.
+// emu_b200 — wgmma skinny GEMM for the wide decode step:  C[B,N] = epilogue( X[B,K] · W[N,K]^T ),  B <= 32.
 //
 // The decode step of more than 8 cache rows (BASELINE config 4: 4 prompts x 5 beams = 20 rows; reference call site
 // Emu2/emu/emu.py:213-229 -> HF beam search) streams every weight once per token: HBM-bound, so what matters is how many
-// weight bytes each SM keeps in flight.  gemm_tc.cu treats the activations as the 128-row MMA operand: at 20 rows, 16 KB of
-// every 24 KB pipeline stage is zero padding, 8 stages hold 64 KB of weights per SM, and the N = 6656 projections fill
-// 104 of 148 SMs (profiles/r02_wide_decode_launches.txt: o_proj + down_proj at 0.40 of the HBM rate).  Here the operands
-// are swapped:
-//   A operand (M = 128)  : a tile of 128 WEIGHT rows x 64 k      (16 KB per stage)
-//   B operand (N = 32)   : the activations, 32 rows (zero-filled past B) x 64 k   (4 KB per stage)
-//   accumulator in TMEM  : [128 weight rows (lanes)] x [32 batch columns] fp32, double buffered (64 columns)
+// weight bytes each SM keeps in flight.  gemm_tc.cu treats the activations as the 128-row MMA operand: at 20 rows most of
+// every pipeline stage is zero padding.  Here the operands are swapped:
+//   A operand (2 x M = 64) : a tile of 128 WEIGHT rows x 64 k      (16 KB per stage)
+//   B operand (N = 32)     : the activations, 32 rows (zero-filled past B) x 64 k   (4 KB per stage)
+//   accumulators           : [128 weight rows] x [32 batch columns] fp32 in the registers of one warpgroup
 // -> 10 stages x 16 KB = 160 KB of weights in flight per SM.  Work units are (weight-row tile, K split): projections with
 // few tiles are split along K so that every SM streams; the partial sums go through an fp32 workspace and the CTA that
 // arrives last at a tile adds them in split order (deterministic) and runs the epilogue.
-//   warp 0 : TMA producer (weight tiles are requested before griddepcontrol.wait — they do not depend on the predecessor)
-//   warp 1 : TMEM allocation + tcgen05.mma issue (one thread)
-//   warps 2..5 : epilogue — tcgen05.ld, lane = weight row: for a fixed batch row the 32 lanes of a warp hold 32 consecutive
-//                output columns, so stores / residual loads are 64-byte coalesced.  plain / +residual / SwiGLU (gate and up
-//                rows interleaved: one shuffle), bf16 or fp32 output.
+//   warp 4     : TMA producer (weight tiles are requested before griddepcontrol.wait — they do not depend on the predecessor)
+//   warps 0..3 : wgmma m64n32k16 (two per 16-deep k step) and the epilogue: plain / +residual / SwiGLU (gate and up rows
+//                interleaved: one shuffle), bf16 or fp32 output.
 #include "common.cuh"
 #include "ops.h"
+#include "wgmma.cuh"
 
 namespace emu {
 
@@ -31,9 +28,8 @@ constexpr int SKN = 32;   // activation rows (MMA N)
 constexpr int SKK = 64;   // k per stage: 64 bf16 = one 128-byte swizzle row
 constexpr int kSkStageBytes = (SKM + SKN) * SKK * 2;  // 20480
 constexpr int kSkStages = 10;
-constexpr int kSkThreads = 192;
+constexpr int kSkThreads = 160;  // warps 0..3 = the consumer warpgroup, warp 4 = TMA producer
 constexpr int kSkSmem = kSkStages * kSkStageBytes + 1024 /*align*/ + 256 /*barriers*/;
-constexpr uint32_t kSkTmemCols = 64;
 
 struct SkinnyParams {
   int B, N, K;
@@ -57,9 +53,6 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kSkStages * kSkStageBytes);
   uint64_t* empty_bar = full_bar + kSkStages;
-  uint64_t* tmem_full = empty_bar + kSkStages;  // [2]
-  uint64_t* tmem_empty = tmem_full + 2;         // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   __shared__ int s_last;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -71,22 +64,13 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   }
   if (threadIdx.x < kSkStages) {
     mbar_init(&full_bar[threadIdx.x], 1);
-    mbar_init(&empty_bar[threadIdx.x], 1);
-    mbar_fence_init();
-  } else if (threadIdx.x >= 32 && threadIdx.x < 34) {
-    const int i = threadIdx.x - 32;
-    mbar_init(&tmem_full[i], 1);
-    mbar_init(&tmem_empty[i], 4);
+    mbar_init(&empty_bar[threadIdx.x], 4);  // lane 0 of every consumer warp
     mbar_fence_init();
   }
   if (p.pdl) pdl_launch_dependents();
-  if (warp == 1) tmem_alloc(tmem_slot, kSkTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
@@ -125,128 +109,118 @@ gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
         first = false;
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(SKM, SKN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const int s = u % p.splits;
-        const int kb0 = s * p.kb_per_split, kb1 = min(p.num_kb, kb0 + p.kb_per_split);
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * SKN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * kSkStageBytes);
-          const uint64_t da = umma_desc_sw128(sa);
-          const uint64_t db = umma_desc_sw128(sa + SKM * SKK * 2);
-#pragma unroll
-          for (int k = 0; k < SKK / 16; ++k) umma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb != kb0 || k != 0) ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (++stage == kSkStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // ===================== epilogue (warps 2..5: TMEM lane quarter = warp & 3) =====================
-    const int q = warp & 3;
-    const int r = q * 32 + lane;  // weight row inside the tile
-    if (p.pdl) pdl_wait();        // residual is a predecessor output and C may alias a buffer it still reads
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ===================== consumer warpgroup: wgmma + epilogue =====================
+    // v[16 m + 4 j + 2 h + e] = weight row 64 m + 16 warp + lane / 4 + 8 h of the tile, batch row 8 j + 2 (lane % 4) + e
+    if (p.pdl) pdl_wait();  // residual is a predecessor output and C may alias a buffer it still reads
     const int B = p.B;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int u = blockIdx.x; u < units; u += gridDim.x) {
       const int tile = u / p.splits, s = u % p.splits;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * SKN), v);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      float f[32];
+      const int kb0 = s * p.kb_per_split, kb1 = min(p.num_kb, kb0 + p.kb_per_split);
+      float v[32];
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * kSkStageBytes);
+        const uint64_t da0 = wgmma_desc_sw128(sa), da1 = wgmma_desc_sw128(sa + 64 * SKK * 2);
+        const uint64_t db = wgmma_desc_sw128(sa + SKM * SKK * 2);
+        wgmma_fence();
 #pragma unroll
-      for (int b = 0; b < 32; ++b) f[b] = __uint_as_float(v[b]);
+        for (int k = 0; k < SKK / 16; ++k) {
+          const int acc = (kb != kb0 || k != 0) ? 1 : 0;
+          WgmmaSS<SKN>::run(v, da0 + 2 * k, db + 2 * k, acc);
+          WgmmaSS<SKN>::run(v + 16, da1 + 2 * k, db + 2 * k, acc);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == kSkStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      const int rbase = 16 * warp + (lane >> 2), bbase = 2 * (lane & 3);
       bool fin = true;
       if (p.splits > 1) {
-        float* wt = p.ws + ((long)(tile * p.splits + s) * 32) * SKM + r;
+        float* wt = p.ws + ((long)(tile * p.splits + s) * 32) * SKM;
 #pragma unroll
-        for (int b = 0; b < 32; ++b)
-          if (b < B) wt[b * SKM] = f[b];
+        for (int i = 0; i < 32; ++i) {
+          const int r = 64 * (i >> 4) + rbase + 8 * ((i >> 1) & 1), b = 8 * ((i >> 2) & 3) + bbase + (i & 1);
+          if (b < B) wt[b * SKM + r] = v[i];
+        }
         __threadfence();
         sk_named_bar(1, 128);
-        if (threadIdx.x == 64) {
-          const int prev = atomicAdd(&p.counters[tile], 1);
-          s_last = prev == p.splits - 1;
-          if (prev == p.splits - 1) p.counters[tile] = 0;  // self-reset for the next launch / graph replay
+        if (threadIdx.x == 0) {
+          const int prev_cnt = atomicAdd(&p.counters[tile], 1);
+          s_last = prev_cnt == p.splits - 1;
+          if (prev_cnt == p.splits - 1) p.counters[tile] = 0;  // self-reset for the next launch / graph replay
         }
         sk_named_bar(1, 128);
         fin = s_last != 0;
         if (fin) {
           __threadfence();
-          const float* base = p.ws + ((long)tile * p.splits * 32) * SKM + r;
+          const float* base = p.ws + ((long)tile * p.splits * 32) * SKM;
 #pragma unroll
-          for (int b = 0; b < 32; ++b) f[b] = 0.f;
-          for (int s2 = 0; s2 < p.splits; ++s2) {  // split order: deterministic.  All rows of one split are loaded before any
-            const float* src = base + (long)s2 * 32 * SKM;  // is added: one L2 round trip per split, not per value
+          for (int i = 0; i < 32; ++i) v[i] = 0.f;
+          for (int s2 = 0; s2 < p.splits; ++s2) {  // split order: deterministic.  All values of one split are loaded before
+            const float* src = base + (long)s2 * 32 * SKM;  // any is added: one L2 round trip per split, not per value
             float t[32];
 #pragma unroll
-            for (int b = 0; b < 32; ++b) t[b] = b < B ? __ldcg(src + b * SKM) : 0.f;
+            for (int i = 0; i < 32; ++i) {
+              const int r = 64 * (i >> 4) + rbase + 8 * ((i >> 1) & 1), b = 8 * ((i >> 2) & 3) + bbase + (i & 1);
+              t[i] = b < B ? __ldcg(src + b * SKM + r) : 0.f;
+            }
 #pragma unroll
-            for (int b = 0; b < 32; ++b) f[b] += t[b];
+            for (int i = 0; i < 32; ++i) v[i] += t[i];
           }
         }
         sk_named_bar(1, 128);  // s_last is rewritten by the next unit
       }
       if (!fin) continue;
-      const long n = (long)tile * SKM + r;
       if (p.mode == EPI_SWIGLU) {
-        // rows 2j / 2j+1 of W are gate_j / up_j: silu(gate) * up with HF's bf16 rounding points
+        // rows 2j / 2j+1 of W are gate_j / up_j (lanes l and l ^ 4): silu(gate) * up with HF's bf16 rounding points
         bf16* out = reinterpret_cast<bf16*>(p.C);
 #pragma unroll
-        for (int b = 0; b < 32; ++b) {
-          if (b < B) {
-            const float other = __shfl_xor_sync(0xffffffffu, f[b], 1);
-            if (!(lane & 1) && n < p.N) {
-              const float gate = round_bf16(f[b]), up = round_bf16(other);
-              out[(long)b * p.ldc + (n >> 1)] = __float2bfloat16_rn(round_bf16(silu(gate)) * up);
-            }
+        for (int i = 0; i < 32; ++i) {
+          const float other = __shfl_xor_sync(0xffffffffu, v[i], 4);
+          const long n = (long)tile * SKM + 64 * (i >> 4) + rbase + 8 * ((i >> 1) & 1);
+          const int b = 8 * ((i >> 2) & 3) + bbase + (i & 1);
+          if (!((lane >> 2) & 1) && n < p.N && b < B) {
+            const float gate = round_bf16(v[i]), up = round_bf16(other);
+            out[(long)b * p.ldc + (n >> 1)] = __float2bfloat16_rn(round_bf16(silu(gate)) * up);
           }
         }
-      } else if (n < p.N) {
-        if (p.residual != nullptr) {  // all residual rows in flight before the first is consumed
-          float rs[32];
+      } else {
+        float rs[32];
+        if (p.residual != nullptr) {  // all residual values in flight before the first is consumed
 #pragma unroll
-          for (int b = 0; b < 32; ++b)
-            rs[b] = b < B ? __uint_as_float((uint32_t)__ldcg(reinterpret_cast<const unsigned short*>(p.residual) + (long)b * p.ldr + n) << 16)
-                          : 0.f;
+          for (int i = 0; i < 32; ++i) {
+            const long n = (long)tile * SKM + 64 * (i >> 4) + rbase + 8 * ((i >> 1) & 1);
+            const int b = 8 * ((i >> 2) & 3) + bbase + (i & 1);
+            rs[i] = (b < B && n < p.N)
+                        ? __uint_as_float((uint32_t)__ldcg(reinterpret_cast<const unsigned short*>(p.residual) + (long)b * p.ldr + n) << 16)
+                        : 0.f;
+          }
 #pragma unroll
-          for (int b = 0; b < 32; ++b) f[b] = round_bf16(f[b]) + rs[b];
+          for (int i = 0; i < 32; ++i) v[i] = round_bf16(v[i]) + rs[i];
         }
 #pragma unroll
-        for (int b = 0; b < 32; ++b) {
-          if (b < B) {
-            if (p.out_fp32) reinterpret_cast<float*>(p.C)[(long)b * p.ldc + n] = f[b];
-            else reinterpret_cast<bf16*>(p.C)[(long)b * p.ldc + n] = __float2bfloat16_rn(f[b]);
+        for (int i = 0; i < 32; ++i) {
+          const long n = (long)tile * SKM + 64 * (i >> 4) + rbase + 8 * ((i >> 1) & 1);
+          const int b = 8 * ((i >> 2) & 3) + bbase + (i & 1);
+          if (b < B && n < p.N) {
+            if (p.out_fp32) reinterpret_cast<float*>(p.C)[(long)b * p.ldc + n] = v[i];
+            else reinterpret_cast<bf16*>(p.C)[(long)b * p.ldc + n] = __float2bfloat16_rn(v[i]);
           }
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kSkTmemCols);
   }
 }
 
@@ -284,8 +258,8 @@ int gemm_skinny_bf16(const bf16* X, int ldx, const bf16* W, int ldw, int B, int 
   int best_s = 1;
   double best_cost = 1e30;
   const int max_s = (ws && counters) ? 16 : 1;
-  // every weight byte crosses HBM once: no split can beat tiles x k-blocks x 16 KB at ~3370 B/clk
-  const double hbm_floor = (double)p.tiles * p.num_kb * (SKM * SKK * 2) / 3370.0;
+  // every weight byte crosses HBM once: no split can beat tiles x k-blocks x 16 KB at ~1800 B/clk
+  const double hbm_floor = (double)p.tiles * p.num_kb * (SKM * SKK * 2) / 1800.0;
   for (int S = 1; S <= max_s; ++S) {
     const int kbs = (p.num_kb + S - 1) / S;
     if (S > 1 && (kbs < 4 || (long)p.tiles * S > kSkinnyMaxUnits || p.tiles > kSkinnyMaxTiles)) break;

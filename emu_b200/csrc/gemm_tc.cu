@@ -1,23 +1,15 @@
-// emu_b200 — tcgen05 GEMM:  C[M,N] = epilogue( A[M,K] · W[N,K]^T )
+// emu_b200 — wgmma GEMM:  C[M,N] = epilogue( A[M,K] · W[N,K]^T )
 //
 // The dense-contraction workhorse of the generate path: ViT QKV/proj/MLP (Emu2/emu/eva_vit.py:194-200,
 // 105-114), LLaMA prefill q/k/v/o/gate/up/down (HF LlamaDecoderLayer, called from Emu2/emu/emu.py:133-138,
 // 213-229), project_up/project_down (emu.py:53-55), UNet linears and — through the 4-D TMA "conv" A-loader —
 // the UNet/VAE 3x3 convolutions (diffusers UNet2DConditionModel, called from Emu2/emu/diffusion.py:136-141).
 //
-// Design (one CTA per SM, persistent over output tiles):
-//   warp 0      : TMA producer — cp.async.bulk.tensor loads of 128x64 (A) and BNx64 (W) bf16 tiles into a
-//                 kStages-deep ring of 128B-swizzled shared-memory stages, completion on mbarriers
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (kind::f16, M=128, N=BN, K=16),
-//                 fp32 accumulators double-buffered in TMEM so the epilogue of tile i overlaps tile i+1
-//   warps 2..9  : epilogue — tcgen05.ld accumulator rows to registers (two warps per TMEM lane quarter, alternating
-//                 32-column slabs), fused bias / GELU / residual / SwiGLU / GEGLU.  bf16 outputs are STAGED: the tile is
-//                 assembled in shared memory as 64B-swizzled [128 rows x 32 columns] slabs (one conflict-free 16-byte
-//                 st.shared per 8 outputs) and leaves with TMA stores; a residual tile arrives the same way (TMA load issued
-//                 while the MMAs still run).  Round 1 stored / loaded rows straight from registers — one row per lane, so
-//                 every 16-byte access of a warp touched 32 different cache lines: 3.3 k cycles (plain) to 7.6 k (residual)
-//                 to 13.8 k (GEGLU) per 128 x 160..224 tile against a 9.7 k-cycle main loop (profiles/r02_gemm_phases_*.txt).
-//                 fp32 outputs, unaligned or very wide (> 192 columns) tiles keep the direct path.
+// 128 x BN output tiles, persistent CTAs (one per SM), a TMA producer feeding a ring of 128B-swizzled stages and two
+// consumer warpgroups that run wgmma (fp32 accumulators in registers) and the fused epilogue — bias / GELU / residual /
+// SwiGLU / GEGLU.  bf16 outputs are STAGED: the tile is assembled in shared memory as 64B-swizzled [rows x 32 columns]
+// slabs and leaves with TMA stores; a residual tile arrives the same way (TMA load issued before the tile's main loop
+// ends).  fp32 outputs, unaligned or very wide (> 192 columns) tiles store straight from registers.
 // A and W are both K-major, so neither operand needs a transpose anywhere in the model.
 #include <cstdlib>
 #include <cstring>
@@ -25,12 +17,13 @@
 
 #include "common.cuh"
 #include "ops.h"
+#include "wgmma.cuh"
 
 namespace emu {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle row
-constexpr int kGemmThreads = 320;  // TMA warp + MMA warp + 8 epilogue warps
+constexpr int kGemmThreads = 384;  // producer warpgroup + two consumer warpgroups
 
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(m), "r"(smem_u32(smem)),
@@ -53,7 +46,7 @@ __device__ __forceinline__ uint4 lds128(uint32_t saddr) {
 
 template <int BN>
 struct GemmSmem {
-  static_assert(BN % 32 == 0 && BN >= 64 && BN <= 256, "BN: multiple of 32 (epilogue chunks) within the tcgen05 N range");
+  static_assert(BN % 32 == 0 && BN >= 64 && BN <= 256, "BN: multiple of 32 (epilogue slabs) within the wgmma N range");
   static constexpr int kStageBytes = (BM + BN) * BK * 2;
   // staging for the TMA-store epilogue: [slabs of 32 output columns][128 rows][64 B].  Tiles wider than 192 columns are
   // only staged by the pair epilogues (SwiGLU / GEGLU), which emit BN / 2 columns.
@@ -62,8 +55,6 @@ struct GemmSmem {
   static constexpr int kStages = kFit > 8 ? 8 : kFit;  // 8 / 7 / 6 / 5 / 4 / 4 / 4 for BN = 64 .. 256
   static constexpr int kBytes = kStages * kStageBytes + kStagingBytes + 1024 /*align slack*/ + 512 /*barriers*/;
   static_assert(kStages >= 3, "pipeline too shallow");
-  // two accumulator stages; tcgen05.alloc wants a power of two
-  static constexpr uint32_t kTmemCols = 2 * BN <= 128 ? 128 : (2 * BN <= 256 ? 256 : 512);
 };
 
 struct GemmParams {
@@ -86,7 +77,7 @@ struct GemmParams {
   int staged;    // bf16 output through shared memory + TMA store (tmC)
   int res_smem;  // residual tile through TMA load into the staging buffer (tmR); else direct global loads
   // diagnostics (emu_debug_gemm_phases): when non-null, every CTA writes 8 x u64 = {globaltimer at entry, clock64 at entry,
-  // after set-up, first TMA issued, first stage landed (MMA side), last MMA committed, epilogue released by the MMAs,
+  // after set-up, first TMA issued, first stage landed (MMA side), last MMA of the tile retired, epilogue started,
   // epilogue done} for its FIRST tile
   unsigned long long* dbg;
 };
@@ -101,26 +92,47 @@ __device__ __forceinline__ unsigned long long gtimer() {
   return t;
 }
 
+// two consecutive bf16 at p (the second only if `two`) as floats; 4-byte load when aligned
+__device__ __forceinline__ float2 ld_bf16x2(const bf16* p, bool two) {
+  if (two && !(reinterpret_cast<uintptr_t>(p) & 3)) {
+    const uint32_t v = *reinterpret_cast<const uint32_t*>(p);
+    return make_float2(bf16_lo(v), bf16_hi(v));
+  }
+  return make_float2(__bfloat162float(p[0]), two ? __bfloat162float(p[1]) : 0.f);
+}
+__device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void sts32(uint32_t saddr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory"); }
+__device__ __forceinline__ void sts16(uint32_t saddr, uint16_t v) { asm volatile("st.shared.b16 [%0], %1;" ::"r"(saddr), "h"(v) : "memory"); }
+// byte offset of (row, column c < 32) inside a 64B-swizzled [rows][32 bf16] slab (the TMA SWIZZLE_64B pattern)
+__device__ __forceinline__ uint32_t slab_off(int row, int c) {
+  return (uint32_t)row * 64u + ((((uint32_t)c >> 3) ^ (((uint32_t)row >> 1) & 3u)) << 4) + ((uint32_t)c & 7u) * 2u;
+}
+
+// Warp roles (384 threads = 3 warpgroups, one CTA per SM, persistent over output tiles):
+//   warpgroup 0 : TMA producer (one thread) — 128x64 (A) and BNx64 (W) bf16 tiles into a kStages-deep ring of
+//                 128B-swizzled shared-memory stages, completion on mbarriers; the other warps give their registers away
+//   warpgroups 1/2 : consumers of tile rows 0..63 / 64..127 — wgmma m64nBNk16 from shared memory into fp32 registers,
+//                 then the fused epilogue of their 64 rows.
 // CL = thread-block cluster size along M (1 or 2).  With CL == 2 the two CTAs of a cluster work on vertically adjacent
 // output tiles (same weight columns): each loads HALF of the W tile and TMA-multicasts it into both CTAs' shared memory,
-// so W crosses the L2->SM fabric once per pair — the fabric, not the tensor pipe, bounds the BN <= 160 tiles.
+// so W crosses the L2->SM fabric once per pair; a stage is released in both CTAs once both have consumed it.
 template <int BN, int CL>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
   constexpr int kStages = GemmSmem<BN>::kStages;
   constexpr int kStageBytes = GemmSmem<BN>::kStageBytes;
-  constexpr uint32_t kTmemCols = GemmSmem<BN>::kTmemCols;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* staging = smem + kStages * kStageBytes;  // 1024-aligned: kStageBytes is a multiple of 4096
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + GemmSmem<BN>::kStagingBytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;        // [2]
-  uint64_t* res_full = tmem_empty + 2;         // [2] residual slabs of epilogue group 0 / 1 have landed
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(res_full + 2);
+  uint64_t* res_full = empty_bar + kStages;  // [2] residual slabs of consumer 0 / 1 have landed
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -144,29 +156,23 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (p.staged) tma_prefetch_desc(&tmC);
     if (p.res_smem) tma_prefetch_desc(&tmR);
   }
-  if (threadIdx.x < kStages) {  // barrier inits spread over threads (one thread walking ~22 of them costs ~0.3 us per launch)
+  if (threadIdx.x < kStages) {
     mbar_init(&full_bar[threadIdx.x], 1);
-    mbar_init(&empty_bar[threadIdx.x], CL);  // one tcgen05.commit arrival from every CTA that reads the multicast stage
+    mbar_init(&empty_bar[threadIdx.x], 8 * CL);  // lane 0 of every consumer warp, in every CTA that reads the stage
     mbar_fence_init();
   } else if (threadIdx.x >= 32 && threadIdx.x < 34) {
-    const int i = threadIdx.x - 32;
-    mbar_init(&tmem_full[i], 1);
-    mbar_init(&tmem_empty[i], 8);
-    mbar_init(&res_full[i], 1);
+    mbar_init(&res_full[threadIdx.x - 32], 1);
     mbar_fence_init();
   }
   if (p.pdl) pdl_launch_dependents();  // the next kernel of the chain may start its own prologue now
-  if (warp == 1) tmem_alloc(tmem_base_slot, kTmemCols);
-  tc_fence_before();
   if (CL > 1) cluster_sync_all();  // the peer's barriers must be initialised before anything is multicast at them
   else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
   if (dbg && threadIdx.x == 0) dbg[2] = clk64();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
       if (p.pdl) pdl_wait();  // activations (A) come from the predecessor; everything above overlapped its tail
       if (dbg) dbg[3] = clk64();
       int stage = 0;
@@ -207,460 +213,199 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = unit0; tile < num_tiles; tile += unit_step) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (dbg && kb == 0 && tile == unit0) dbg[4] = clk64();
-          const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-          const uint32_t sb = sa + BM * BK * 2;
-          const uint64_t da = umma_desc_sw128(sa);
-          const uint64_t db = umma_desc_sw128(sb);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // advance 16 elements (32 B) along K inside the 128 B swizzle row: +2 in the (addr>>4) field
-            umma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-          }
-          // frees the smem stage when these MMAs retire — in every CTA of the cluster (the peer's producer overwrites
-          // half of OUR stage, so it must see our consumption too)
-          if (CL > 1) umma_commit_mc(&empty_bar[stage], (uint16_t)((1u << CL) - 1));
-          else umma_commit(&empty_bar[stage]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator ready for the epilogue
-        if (dbg && tile == unit0) dbg[5] = clk64();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // ===================== epilogue warps (2..9) =====================
-    // warp w owns TMEM lane quarter (w & 3) — the hardware restriction — and every second 32-column chunk
-    // (chunk parity = (w - 2) >> 2), so two warps per SM sub-partition share a tile's epilogue.
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
+    // ===================== consumers: wgmma main loop + epilogue of 64 rows =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int wg = (warp >> 2) - 1;                   // 0 / 1: tile rows 64 wg ..
+    const int rl = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // tile rows rl and rl + 8 of this thread
+    const int cq = 2 * (lane & 3);                    // column pair offset inside every 8-column group
+    const bool pair = (p.epi == EPI_SWIGLU || p.epi == EPI_GEGLU);
+    const int n_out = pair ? (p.N >> 1) : p.N;        // output columns of the whole matrix
+    const int bn_out = pair ? BN / 2 : BN;            // ... of one tile
+    const int n_units = bn_out / 32;
+    const uint32_t stg = smem_u32(staging);
+    const bool issuer = (threadIdx.x & 127) == 0;
+    const int bar_id = 1 + wg;
     if (p.pdl) pdl_wait();  // residual / bias2 are predecessor outputs and C may alias a buffer it still reads
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    if (p.staged) {
-      // ---------- staged epilogue: registers -> 64B-swizzled shared-memory slabs -> TMA store ----------
-      // The two warp groups (half = 0 / 1, four warps = the four TMEM lane quarters each) own the even / odd 32-column
-      // output slabs of the tile and run independently: own named barrier, own elected issuer thread (TMA stores, the
-      // residual loads of the next tile), own residual mbarrier.
-      const bool pair = (p.epi == EPI_SWIGLU || p.epi == EPI_GEGLU);
-      const int n_out = pair ? (p.N >> 1) : p.N;            // output columns of the whole matrix
-      const int bn_out = pair ? BN / 2 : BN;                // ... of one tile
-      const int n_units = bn_out / 32;
-      const int r_in_tile = q * 32 + lane;
-      const uint32_t stg = smem_u32(staging);
-      const uint32_t my_row = (uint32_t)r_in_tile * 64u;
-      const uint32_t swz = (uint32_t)((r_in_tile >> 1) & 3);
-      const bool issuer = (q == 0 && lane == 0);
-      const int bar_id = 1 + half;
-      const bool vec_bias = p.bias != nullptr && ((reinterpret_cast<uintptr_t>(p.bias) & 15) == 0);
-      const bool vec_b2 = p.bias2 != nullptr && (p.N % 8 == 0) && ((reinterpret_cast<uintptr_t>(p.bias2) & 15) == 0);
-      const bool vec_res = p.residual != nullptr && (p.ldr % 8 == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0);
-      auto tile_row0 = [&](int tm) -> long {
-        if (!p.conv) return (long)tm * BM;
-        const int tiles_w = p.W / p.tw, tiles_h = p.H / p.th;
-        const int w0 = (tm % tiles_w) * p.tw, h0 = ((tm / tiles_w) % tiles_h) * p.th, img = tm / (tiles_w * tiles_h);
-        return ((long)img * p.H + h0) * p.W + w0;  // a tile is th full-width rows or one 128-pixel run: 128 consecutive rows
-      };
-      auto load_residual = [&](int tile) {  // issuer only: this group's residual slabs of `tile` -> staging
-        const int tm = (tile % units_m) * CL + crank, tn = tile / units_m;
-        int cnt = 0;
-        for (int u = half; u < n_units; u += 2)
-          if (tn * bn_out + u * 32 < n_out) ++cnt;
-        if (tm >= tiles_m) cnt = 0;
-        mbar_expect_tx(&res_full[half], (uint32_t)cnt * 8192u);  // arrive + expect: with 0 bytes the phase completes at once
-        if (cnt == 0) return;
-        const int row0 = (int)tile_row0(tm);
-        for (int u = half; u < n_units; u += 2)
-          if (tn * bn_out + u * 32 < n_out) tma_load_2d(staging + u * 8192, &tmR, &res_full[half], tn * bn_out + u * 32, row0);
-      };
-      if (p.res_smem && issuer && unit0 < num_tiles) load_residual(unit0);
-      uint32_t res_phase = 0;
-      for (int tile = unit0; tile < num_tiles; tile += unit_step) {
-        const int tm = (tile % units_m) * CL + crank, tn = tile / units_m;
-        const long row0 = tile_row0(tm);
-        const long row = row0 + r_in_tile;
-        const bool row_ok = row < p.M && tm < tiles_m;
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-        if (dbg && tile == unit0 && threadIdx.x == 64) dbg[6] = clk64();
-        if (p.res_smem) mbar_wait(&res_full[half], res_phase);
-#pragma unroll 1
-        for (int u = half; u < n_units; u += 2) {
-          const int oc0 = tn * bn_out + u * 32;  // first output column of this slab
-          if (oc0 >= n_out) break;
-          const uint32_t slab = stg + (uint32_t)u * 8192u + my_row;
-          if (!pair) {
-            uint32_t v[32];
-            tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + u * 32), v);
-            tmem_ld_wait();
-            float f[32];
+    auto tile_row0 = [&](int tm) -> long {
+      if (!p.conv) return (long)tm * BM;
+      const int tiles_w = p.W / p.tw, tiles_h = p.H / p.th;
+      const int w0 = (tm % tiles_w) * p.tw, h0 = ((tm / tiles_w) % tiles_h) * p.th, img = tm / (tiles_w * tiles_h);
+      return ((long)img * p.H + h0) * p.W + w0;  // a tile is th full-width rows or one 128-pixel run: 128 consecutive rows
+    };
+    auto load_residual = [&](int tile) {  // issuer only: this consumer's 64 residual rows of every slab of `tile` -> staging
+      const int tm = (tile % units_m) * CL + crank, tn = tile / units_m;
+      int cnt = 0;
+      for (int u = 0; u < n_units; ++u)
+        if (tn * bn_out + u * 32 < n_out) ++cnt;
+      if (tm >= tiles_m) cnt = 0;
+      mbar_expect_tx(&res_full[wg], (uint32_t)cnt * 4096u);  // arrive + expect: with 0 bytes the phase completes at once
+      if (cnt == 0) return;
+      const int row0 = (int)tile_row0(tm) + 64 * wg;
+      for (int u = 0; u < n_units; ++u)
+        if (tn * bn_out + u * 32 < n_out)
+          tma_load_2d(staging + u * 8192 + wg * 4096, &tmR, &res_full[wg], tn * bn_out + u * 32, row0);
+    };
+    if (p.staged && p.res_smem && issuer && unit0 < num_tiles) load_residual(unit0);
+    uint32_t res_phase = 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    float d[BN / 2];
+    for (int tile = unit0; tile < num_tiles; tile += unit_step) {
+      const int tm = (tile % units_m) * CL + crank, tn = tile / units_m;
+      // ---------- main loop: one k block = 4 x wgmma k16; the stage of k block kb - 1 is released once kb's are issued ----------
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        if (dbg && kb == 0 && tile == unit0 && threadIdx.x == 128) dbg[4] = clk64();
+        const uint32_t sa = smem_u32(smem + stage * kStageBytes) + wg * (64 * BK * 2);
+        const uint32_t sb = smem_u32(smem + stage * kStageBytes) + BM * BK * 2;
+        const uint64_t da = wgmma_desc_sw128(sa), db = wgmma_desc_sw128(sb);
+        wgmma_fence();
 #pragma unroll
-            for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-            const bool full = oc0 + 32 <= p.N;
-            if (p.bias != nullptr) {
-              if (full && vec_bias) {
-                const uint4* bsrc = reinterpret_cast<const uint4*>(p.bias + oc0);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const uint4 b = __ldg(bsrc + i);
-                  const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) { f[8 * i + 2 * j] += bf16_lo(bw[j]); f[8 * i + 2 * j + 1] += bf16_hi(bw[j]); }
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                  if (oc0 + i < p.N) f[i] += __bfloat162float(p.bias[oc0 + i]);
-              }
-            }
-            if (p.bias2 != nullptr && row_ok) {
-              const bf16* b2 = p.bias2 + (row / p.bias2_rows) * p.N + oc0;
-              if (full && vec_b2) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const uint4 b = __ldg(reinterpret_cast<const uint4*>(b2) + i);
-                  const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-                    round_bf16x2(f[8 * i + 2 * j], f[8 * i + 2 * j + 1]);
-                    f[8 * i + 2 * j] += bf16_lo(bw[j]);
-                    f[8 * i + 2 * j + 1] += bf16_hi(bw[j]);
-                  }
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                  if (oc0 + i < p.N) f[i] = round_bf16(f[i]) + __bfloat162float(b2[i]);
-              }
-            }
-            if (p.epi == EPI_GELU) {
-#pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                round_bf16x2(f[i], f[i + 1]);
-                f[i] = gelu_erf_fast(f[i]);
-                f[i + 1] = gelu_erf_fast(f[i + 1]);
-              }
-            } else if (p.epi == EPI_RELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) f[i] = fmaxf(f[i], 0.f);
-            }
-            if (p.res_smem) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const uint4 r = lds128(slab + (((uint32_t)i ^ swz) << 4));
-                const uint32_t rw[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  round_bf16x2(f[8 * i + 2 * j], f[8 * i + 2 * j + 1]);
-                  f[8 * i + 2 * j] += bf16_lo(rw[j]);
-                  f[8 * i + 2 * j + 1] += bf16_hi(rw[j]);
-                }
-              }
-            } else if (p.residual != nullptr && row_ok) {
-              const bf16* rsd = p.residual + row * p.ldr + oc0;
-              if (full && vec_res) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const uint4 r = __ldg(reinterpret_cast<const uint4*>(rsd) + i);
-                  const uint32_t rw[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-                    round_bf16x2(f[8 * i + 2 * j], f[8 * i + 2 * j + 1]);
-                    f[8 * i + 2 * j] += bf16_lo(rw[j]);
-                    f[8 * i + 2 * j + 1] += bf16_hi(rw[j]);
-                  }
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                  if (oc0 + i < p.N) f[i] = round_bf16(f[i]) + __bfloat162float(rsd[i]);
-              }
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              uint4 w;
-              w.x = pack_bf16(f[8 * i], f[8 * i + 1]);
-              w.y = pack_bf16(f[8 * i + 2], f[8 * i + 3]);
-              w.z = pack_bf16(f[8 * i + 4], f[8 * i + 5]);
-              w.w = pack_bf16(f[8 * i + 6], f[8 * i + 7]);
-              sts128(slab + (((uint32_t)i ^ swz) << 4), w);
-            }
-          } else {
-            // interleaved (a_j, b_j) accumulator column pairs -> one output column: slab u <- accumulator chunks 2u, 2u+1
-#pragma unroll
-            for (int hc = 0; hc < 2; ++hc) {
-              const int ac0 = tn * BN + (2 * u + hc) * 32;  // first accumulator column of this chunk
-              uint32_t v[32];
-              tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + (2 * u + hc) * 32), v);
-              tmem_ld_wait();
-              float f[32];
-#pragma unroll
-              for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-              if (p.bias != nullptr) {
-                if (ac0 + 32 <= p.N && vec_bias) {
-                  const uint4* bsrc = reinterpret_cast<const uint4*>(p.bias + ac0);
-#pragma unroll
-                  for (int i = 0; i < 4; ++i) {
-                    const uint4 b = __ldg(bsrc + i);
-                    const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) { f[8 * i + 2 * j] += bf16_lo(bw[j]); f[8 * i + 2 * j + 1] += bf16_hi(bw[j]); }
-                  }
-                } else {
-#pragma unroll
-                  for (int i = 0; i < 32; ++i)
-                    if (ac0 + i < p.N) f[i] += __bfloat162float(p.bias[ac0 + i]);
-                }
-              }
-              // rounding points of the reference (Linear -> bf16, activation -> bf16, product -> bf16), two values per
-              // conversion: (a_i, b_i) together, then the activations of two neighbouring outputs together
-              float o[16];
-#pragma unroll
-              for (int i = 0; i < 16; i += 2) {
-                round_bf16x2(f[2 * i], f[2 * i + 1]);
-                round_bf16x2(f[2 * i + 2], f[2 * i + 3]);
-                float g0, g1;
-                if (p.epi == EPI_SWIGLU) { g0 = silu(f[2 * i]); g1 = silu(f[2 * i + 2]); }
-                else { g0 = gelu_erf_fast(f[2 * i + 1]); g1 = gelu_erf_fast(f[2 * i + 3]); }
-                round_bf16x2(g0, g1);
-                if (p.epi == EPI_SWIGLU) { o[i] = g0 * f[2 * i + 1]; o[i + 1] = g1 * f[2 * i + 3]; }
-                else { o[i] = f[2 * i] * g0; o[i + 1] = f[2 * i + 2] * g1; }
-              }
-#pragma unroll
-              for (int i = 0; i < 2; ++i) {
-                uint4 w;
-                w.x = pack_bf16(o[8 * i], o[8 * i + 1]);
-                w.y = pack_bf16(o[8 * i + 2], o[8 * i + 3]);
-                w.z = pack_bf16(o[8 * i + 4], o[8 * i + 5]);
-                w.w = pack_bf16(o[8 * i + 6], o[8 * i + 7]);
-                sts128(slab + (((uint32_t)(hc * 2 + i) ^ swz) << 4), w);
-              }
+        for (int k = 0; k < BK / 16; ++k)  // 16 elements (32 B) along K inside the 128 B swizzle row: +2 in the (addr>>4) field
+          WgmmaSS<BN>::run(d, da + 2 * k, db + 2 * k, (kb | k) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) {
+            if (CL > 1) {
+              for (int c = 0; c < CL; ++c) mbar_arrive_cluster(&empty_bar[prev], (uint32_t)c);
+            } else {
+              mbar_arrive(&empty_bar[prev]);
             }
           }
         }
-        // the accumulator is drained: hand the TMEM stage back before the stores leave
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        fence_async_smem();        // generic-proxy slab writes -> visible to the TMA engine
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) {
+        if (CL > 1) {
+          for (int c = 0; c < CL; ++c) mbar_arrive_cluster(&empty_bar[prev], (uint32_t)c);
+        } else {
+          mbar_arrive(&empty_bar[prev]);
+        }
+      }
+      if (dbg && tile == unit0 && threadIdx.x == 128) dbg[5] = dbg[6] = clk64();
+
+      // ---------- epilogue ----------
+      const long row0 = tile_row0(tm);
+      const bool tile_ok = tm < tiles_m;
+      long rows[2];
+      bool row_ok[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = rl + 8 * h;
+        if (p.conv && !p.staged) {
+          const int tiles_w = p.W / p.tw, tiles_h = p.H / p.th;
+          const int w0 = (tm % tiles_w) * p.tw, h0 = ((tm / tiles_w) % tiles_h) * p.th, img = tm / (tiles_w * tiles_h);
+          rows[h] = ((long)img * p.H + h0 + r / p.tw) * p.W + w0 + r % p.tw;
+        } else {
+          rows[h] = row0 + r;
+        }
+        row_ok[h] = tile_ok && rows[h] < p.M;
+      }
+      if (p.staged && p.res_smem) mbar_wait(&res_full[wg], res_phase);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int ct = 8 * j + cq;      // accumulator column inside the tile (even)
+        const int col = tn * BN + ct;   // ... of the matrix
+        if (col >= p.N) continue;
+        const bool two = col + 1 < p.N;
+        float2 b = make_float2(0.f, 0.f);
+        if (p.bias != nullptr) b = ld_bf16x2(p.bias + col, two);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float f0 = d[4 * j + 2 * h] + b.x, f1 = d[4 * j + 2 * h + 1] + b.y;
+          const int r = rl + 8 * h;
+          if (p.bias2 != nullptr && row_ok[h]) {
+            const float2 b2 = ld_bf16x2(p.bias2 + (rows[h] / p.bias2_rows) * p.N + col, two);
+            round_bf16x2(f0, f1);
+            f0 += b2.x;
+            f1 += b2.y;
+          }
+          if (pair) {
+            // interleaved (a_j, b_j) accumulator columns -> output column j; rounding points of the reference
+            // (Linear -> bf16, activation -> bf16, product -> bf16).  SwiGLU: silu(gate) * up; GEGLU: hidden * gelu(gate)
+            round_bf16x2(f0, f1);
+            const float o = (p.epi == EPI_SWIGLU) ? round_bf16(silu(f0)) * f1 : f0 * round_bf16(gelu_erf_fast(f1));
+            const int oct = ct >> 1;  // output column inside the tile
+            if (p.staged) {
+              sts16(stg + (uint32_t)(oct >> 5) * 8192u + slab_off(r, oct & 31), __bfloat16_as_ushort(__float2bfloat16_rn(o)));
+            } else if (row_ok[h]) {
+              reinterpret_cast<bf16*>(p.C)[rows[h] * p.ldc + (col >> 1)] = __float2bfloat16_rn(o);
+            }
+            continue;
+          }
+          if (p.epi == EPI_GELU) {
+            round_bf16x2(f0, f1);
+            f0 = gelu_erf_fast(f0);
+            f1 = gelu_erf_fast(f1);
+          } else if (p.epi == EPI_RELU) {
+            f0 = fmaxf(f0, 0.f);
+            f1 = fmaxf(f1, 0.f);
+          }
+          if (p.staged) {
+            const uint32_t a = stg + (uint32_t)(ct >> 5) * 8192u + slab_off(r, ct & 31);
+            if (p.res_smem) {
+              const uint32_t rv = lds32(a);
+              round_bf16x2(f0, f1);
+              f0 += bf16_lo(rv);
+              f1 += bf16_hi(rv);
+            } else if (p.residual != nullptr && row_ok[h]) {
+              const float2 rv = ld_bf16x2(p.residual + rows[h] * p.ldr + col, two);
+              round_bf16x2(f0, f1);
+              f0 += rv.x;
+              f1 += rv.y;
+            }
+            sts32(a, pack_bf16(f0, f1));
+            continue;
+          }
+          if (!row_ok[h]) continue;
+          if (p.residual != nullptr) {
+            const float2 rv = ld_bf16x2(p.residual + rows[h] * p.ldr + col, two);
+            round_bf16x2(f0, f1);
+            f0 += rv.x;
+            f1 += rv.y;
+          }
+          if (p.out_fp32) {
+            float* dst = reinterpret_cast<float*>(p.C) + rows[h] * p.ldc + col;
+            if (two && !(reinterpret_cast<uintptr_t>(dst) & 7)) *reinterpret_cast<float2*>(dst) = make_float2(f0, f1);
+            else { dst[0] = f0; if (two) dst[1] = f1; }
+          } else {
+            bf16* dst = reinterpret_cast<bf16*>(p.C) + rows[h] * p.ldc + col;
+            if (two && !(reinterpret_cast<uintptr_t>(dst) & 3)) *reinterpret_cast<uint32_t*>(dst) = pack_bf16(f0, f1);
+            else { dst[0] = __float2bfloat16_rn(f0); if (two) dst[1] = __float2bfloat16_rn(f1); }
+          }
+        }
+      }
+      if (p.staged) {
+        // this consumer's 64 rows of every slab leave with TMA stores (rows / columns past the matrix are clipped)
+        fence_async_smem();  // generic-proxy slab writes -> visible to the TMA engine
         named_bar(bar_id, 128);
         if (issuer) {
-          if (tm < tiles_m) {
-            for (int u = half; u < n_units; u += 2) {
+          if (tile_ok) {
+            for (int u = 0; u < n_units; ++u) {
               const int oc0 = tn * bn_out + u * 32;
-              if (oc0 < n_out) tma_store_2d(&tmC, staging + u * 8192, oc0, (int)row0);
+              if (oc0 < n_out) tma_store_2d(&tmC, staging + u * 8192 + wg * 4096, oc0, (int)row0 + 64 * wg);
             }
           }
           bulk_commit();
-          bulk_wait_read0();       // the slabs may be overwritten once the stores have READ them
+          bulk_wait_read0();  // the slabs may be overwritten once the stores have READ them
           if (p.res_smem && tile + unit_step < num_tiles) load_residual(tile + unit_step);
         }
-        named_bar(bar_id, 128);    // nobody of the group touches the slabs before the issuer got here
-        if (dbg && tile == unit0 && threadIdx.x == 64) dbg[7] = clk64();
+        named_bar(bar_id, 128);  // nobody of the group touches the slabs before the issuer got here
         res_phase ^= 1;
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
       }
-      if (issuer) bulk_wait0();    // all stores complete (global writes performed) before the CTA retires
-    } else
-    for (int tile = unit0; tile < num_tiles; tile += unit_step) {
-      const int tm = (tile % units_m) * CL + crank, tn = tile / units_m;
-      // output row owned by this thread
-      long row;
-      const int r_in_tile = q * 32 + lane;
-      if (p.conv) {
-        const int tiles_w = p.W / p.tw, tiles_h = p.H / p.th;
-        const int w0 = (tm % tiles_w) * p.tw;
-        const int h0 = ((tm / tiles_w) % tiles_h) * p.th;
-        const int img = tm / (tiles_w * tiles_h);
-        const int hh = h0 + r_in_tile / p.tw, ww = w0 + r_in_tile % p.tw;
-        row = ((long)img * p.H + hh) * p.W + ww;
-      } else {
-        row = (long)tm * BM + r_in_tile;
-      }
-      const bool row_ok = row < p.M && tm < tiles_m;
-      const bool pair = (p.epi == EPI_SWIGLU || p.epi == EPI_GEGLU);
-      // 16-byte paths need aligned rows; everything in the models is, ragged shapes take the scalar path
-      const bool vec_res = p.residual != nullptr && (p.ldr % 8 == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0);
-      const bool vec_b2 = p.bias2 != nullptr && (p.N % 8 == 0) && ((reinterpret_cast<uintptr_t>(p.bias2) & 15) == 0);
-      const bool vec_bias = p.bias != nullptr && ((reinterpret_cast<uintptr_t>(p.bias) & 15) == 0);
-      // operands that do not depend on the accumulator are fetched BEFORE waiting for the MMAs of this tile
-      uint4 rsd_v[4] = {}, b2_v[4] = {};
-      auto prefetch = [&](int c) {
-        const int col0 = tn * BN + c * 32;
-        if (!row_ok || col0 + 32 > p.N) return;
-        if (vec_res) {
-          const uint4* src = reinterpret_cast<const uint4*>(p.residual + row * p.ldr + col0);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) rsd_v[i] = __ldg(src + i);
-        }
-        if (vec_b2) {
-          const uint4* src = reinterpret_cast<const uint4*>(p.bias2 + (row / p.bias2_rows) * p.N + col0);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) b2_v[i] = __ldg(src + i);
-        }
-      };
-      prefetch(half);
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      if (dbg && tile == unit0 && threadIdx.x == 64) dbg[6] = clk64();
-#pragma unroll 1
-      for (int c = half; c < BN / 32; c += 2) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + c * 32);
-        tmem_ld_32x32(taddr, v);
-        tmem_ld_wait();
-        const int col0 = tn * BN + c * 32;
-        uint4 rsd_c[4], b2_c[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { rsd_c[i] = rsd_v[i]; b2_c[i] = b2_v[i]; }
-        if (c + 2 < BN / 32) prefetch(c + 2);  // next chunk's operands fly while this one is processed
-        if (row_ok && col0 < p.N) {
-          const bool full = col0 + 32 <= p.N;
-          float f[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-          if (p.bias != nullptr) {
-            if (full && vec_bias) {
-              const uint4* bsrc = reinterpret_cast<const uint4*>(p.bias + col0);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const uint4 b = __ldg(bsrc + i);
-                const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-                for (int j = 0; j < 4; ++j) { f[8 * i + 2 * j] += bf16_lo(bw[j]); f[8 * i + 2 * j + 1] += bf16_hi(bw[j]); }
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (col0 + i < p.N) f[i] += __bfloat162float(p.bias[col0 + i]);
-            }
-          }
-          if (p.bias2 != nullptr) {
-            if (full && vec_b2) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const uint32_t bw[4] = {b2_c[i].x, b2_c[i].y, b2_c[i].z, b2_c[i].w};
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  f[8 * i + 2 * j] = round_bf16(f[8 * i + 2 * j]) + bf16_lo(bw[j]);
-                  f[8 * i + 2 * j + 1] = round_bf16(f[8 * i + 2 * j + 1]) + bf16_hi(bw[j]);
-                }
-              }
-            } else {
-              const bf16* b2 = p.bias2 + (row / p.bias2_rows) * p.N + col0;
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (col0 + i < p.N) f[i] = round_bf16(f[i]) + __bfloat162float(b2[i]);
-            }
-          }
-          if (pair) {
-            // interleaved (a_j, b_j) column pairs -> one output column j
-            // SwiGLU: silu(gate)*up with HF's bf16 rounding points; GEGLU: hidden * gelu(gate)
-            float o[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float a = round_bf16(f[2 * i]), b = round_bf16(f[2 * i + 1]);
-              if (p.epi == EPI_SWIGLU) o[i] = round_bf16(silu(a)) * b;
-              else o[i] = a * round_bf16(gelu_erf_fast(b));
-            }
-            const int oc0 = col0 >> 1;
-            bf16* dst = reinterpret_cast<bf16*>(p.C) + row * p.ldc + oc0;
-            if (oc0 + 16 <= (p.N >> 1) && (p.ldc % 8 == 0)) {
-              uint4 w0, w1;
-              w0.x = pack_bf16(o[0], o[1]); w0.y = pack_bf16(o[2], o[3]); w0.z = pack_bf16(o[4], o[5]); w0.w = pack_bf16(o[6], o[7]);
-              w1.x = pack_bf16(o[8], o[9]); w1.y = pack_bf16(o[10], o[11]); w1.z = pack_bf16(o[12], o[13]); w1.w = pack_bf16(o[14], o[15]);
-              reinterpret_cast<uint4*>(dst)[0] = w0;
-              reinterpret_cast<uint4*>(dst)[1] = w1;
-            } else {
-              for (int i = 0; i < 16; ++i)
-                if (oc0 + i < (p.N >> 1)) dst[i] = __float2bfloat16_rn(o[i]);
-            }
-          } else {
-            if (p.epi == EPI_GELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) f[i] = gelu_erf_fast(round_bf16(f[i]));
-            } else if (p.epi == EPI_RELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) f[i] = fmaxf(f[i], 0.f);
-            }
-            if (p.residual != nullptr) {
-              if (full && vec_res) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const uint32_t rw[4] = {rsd_c[i].x, rsd_c[i].y, rsd_c[i].z, rsd_c[i].w};
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-                    f[8 * i + 2 * j] = round_bf16(f[8 * i + 2 * j]) + bf16_lo(rw[j]);
-                    f[8 * i + 2 * j + 1] = round_bf16(f[8 * i + 2 * j + 1]) + bf16_hi(rw[j]);
-                  }
-                }
-              } else {
-                const bf16* rsd = p.residual + row * p.ldr + col0;
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                  if (col0 + i < p.N) f[i] = round_bf16(f[i]) + __bfloat162float(rsd[i]);
-              }
-            }
-            if (p.out_fp32) {
-              float* dst = reinterpret_cast<float*>(p.C) + row * p.ldc + col0;
-              if (full && (p.ldc % 4 == 0)) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                  reinterpret_cast<float4*>(dst)[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-              } else {
-                for (int i = 0; i < 32; ++i)
-                  if (col0 + i < p.N) dst[i] = f[i];
-              }
-            } else {
-              bf16* dst = reinterpret_cast<bf16*>(p.C) + row * p.ldc + col0;
-              if (full && (p.ldc % 8 == 0)) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  uint4 w;
-                  w.x = pack_bf16(f[8 * i], f[8 * i + 1]);
-                  w.y = pack_bf16(f[8 * i + 2], f[8 * i + 3]);
-                  w.z = pack_bf16(f[8 * i + 4], f[8 * i + 5]);
-                  w.w = pack_bf16(f[8 * i + 6], f[8 * i + 7]);
-                  reinterpret_cast<uint4*>(dst)[i] = w;
-                }
-              } else {
-                for (int i = 0; i < 32; ++i)
-                  if (col0 + i < p.N) dst[i] = __float2bfloat16_rn(f[i]);
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (dbg && tile == unit0 && threadIdx.x == 64) dbg[7] = clk64();
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      if (dbg && tile == unit0 && threadIdx.x == 128) dbg[7] = clk64();
     }
+    if (p.staged && issuer) bulk_wait0();  // all stores complete (global writes performed) before the CTA retires
   }
 
-  tc_fence_before();
   if (CL > 1) cluster_sync_all();  // nobody leaves while the peer can still multicast into / arrive on its shared memory
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -696,14 +441,15 @@ int make_tmap_2d(CUtensorMap* out, const void* base, long rows, long cols, long 
   return r == CUDA_SUCCESS ? EMU_OK : EMU_ERR_CUDA;
 }
 
-// bf16 [rows, cols] output / residual matrix for the staged epilogue: box = 128 rows x 32 columns (64 B), 64B swizzle.
+// bf16 [rows, cols] output / residual matrix for the staged epilogue: box = 64 rows (one consumer warpgroup) x 32 columns
+// (64 B), 64B swizzle.
 // TMA clips the rows / columns of a box that fall outside the matrix on a store and zero-fills them on a load.
 int make_tmap_out(CUtensorMap* out, const void* base, long rows, long cols, long ld) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return EMU_ERR_CUDA;
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {32, (cuuint32_t)BM};
+  cuuint32_t box[2] = {32, 64};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -810,10 +556,9 @@ static int launch_gemm_cl(const CUtensorMap& tmA, const CUtensorMap& tmB, const 
   return cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL>, tmA, tmB, tmC, tmR, p) == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
-// Cluster mode (W tile TMA-multicast over a 2-CTA cluster).  Measured on B200 (profiles/r01_gemm_bench_cluster.txt):
-// +8..15 % on the K >= 5760 implicit-GEMM convolutions, -2..8 % on the one-wave linear layers (cluster start-up and
-// lock step cost more than the halved W traffic saves).  Default: convolutions only.  EMU_GEMM_CLUSTER = 0 (never),
-// 1 (always), unset (convs); force bits: 1024 = off, 2048 = on (tests / A-B runs).
+// Cluster mode (W tile TMA-multicast over a 2-CTA cluster): halves the W traffic into shared memory at the price of
+// cluster start-up and lock step.  Default: convolutions only (K >= 5760 for most UNet convs).  EMU_GEMM_CLUSTER = 0
+// (never), 1 (always), unset (convs); force bits: 1024 = off, 2048 = on (tests / A-B runs).
 static bool use_cluster(int M, int force, bool is_conv) {
   static int env = -2;
   if (env == -2) {
@@ -846,11 +591,11 @@ static bool env_no_stage() {
 }
 
 // Tile width: minimise the modelled time of one CTA's tile stream over the instantiated widths.  Per tile the main loop
-// costs kblocks x max(tensor pipe: 2 x bn cycles per 64-deep k block, L2 -> shared-memory operand traffic: (128 + bn) x 128 B at
-// ~75 B/cycle/SM) and the epilogue, which overlaps the NEXT tile's main loop (double-buffered TMEM), costs per output
-// column ~6 cycles staged and 21 (plain) / 47 (residual) / 60 (GELU, GEGLU) direct — all measured with
-// emu_debug_gemm_phases (profiles/r02_gemm_phases_*.txt).  Odd widths such as 160 exist because e.g. M=2048, N=1280 is 160
-// tiles at BN=128 (two waves on 148 SMs, the second 8 % full) but 128 tiles at BN=160 (one wave).
+// costs kblocks x max(tensor pipe: 4 x bn cycles per 128-row, 64-deep k block at H100's 1024 bf16 FMA / clk / SM, L2 ->
+// shared-memory operand traffic: (128 + bn) x 128 B at ~64 B/cycle/SM); the epilogue runs after the main loop in the same
+// warps and costs a few cycles per output column (more with activations or a residual).  Odd widths such as 160 exist
+// because e.g. M=2048, N=1280 is 160 tiles at BN=128 (two waves on 132 SMs, the second 21 % full) but 128 tiles at BN=160
+// (one wave).
 static int pick_bn(int M, int N, int K, const GemmEpilogue& e) {
   static const int cand[] = {256, 224, 192, 160, 128, 96, 64};
   const long tm = (M + BM - 1) / BM;
@@ -862,18 +607,18 @@ static int pick_bn(int M, int N, int K, const GemmEpilogue& e) {
     const long tiles = tm * ((N + bn - 1) / bn);
     const long waves = (tiles + kNumSMs - 1) / kNumSMs;
     const double a_rows = M < 128 ? (double)M : 128.0;  // rows past M are zero-filled by TMA, not fetched
-    const double mma = 2.0 * bn, l2 = (a_rows + bn) * 128.0 / 75.0;
+    const double mma = 4.0 * bn, l2 = (a_rows + bn) * 128.0 / 64.0;
     double per_kb = mma > l2 ? mma : l2;
-    if (tm == 1) {  // one row of tiles: every weight byte comes from HBM exactly once, shared by the busy SMs (~3370 B/clk)
+    if (tm == 1) {  // one row of tiles: every weight byte comes from HBM exactly once, shared by the busy SMs (~1800 B/clk)
       const double active = tiles < kNumSMs ? (double)tiles : (double)kNumSMs;
-      const double hbm = bn * 128.0 * active / 3370.0;
+      const double hbm = bn * 128.0 * active / 1800.0;
       if (hbm > per_kb) per_kb = hbm;
     }
     const double ml = (double)kb * per_kb + 1500.0;  // + pipeline fill
     const bool staged = !env_no_stage() && can_stage(e, N, bn);
-    double per_col = staged ? (act ? 20.0 : 6.0) : (act ? 60.0 : (e.residual ? 47.0 : 21.0));
+    double per_col = staged ? (act ? 20.0 : 8.0) : (act ? 40.0 : (e.residual ? 30.0 : 16.0));
     const double epi = per_col * bn + 400.0;
-    const double cost = (double)(waves - 1) * (ml > epi ? ml : epi) + ml + epi;
+    const double cost = (double)waves * (ml + epi);
     if (cost < best_cost - 1e-9) {
       best_cost = cost;
       best = bn;

@@ -150,8 +150,7 @@ static __device__ __forceinline__ void tma_produce(const CUtensorMap* tm, int cp
 
 // ---- consumers: stage x (optionally RMS-normalised, zero padded to kpad) into shared memory ----
 // Staging sits on the critical path of every GEMV (the weight ring is full long before it ends), so it is written for
-// latency: loads are issued four deep per thread before anything is consumed (round 1 walked one 16-byte load at a time:
-// 4.2 k cycles without and 8.9 k with the RMSNorm for K = 6656, profiles/r02_gemv_phases_*.txt), and the norm weights —
+// latency: loads are issued four deep per thread before anything is consumed, and the norm weights —
 // which do not depend on the predecessor kernel — are fetched by the caller before griddepcontrol.wait (XPre).
 // LlamaRMSNorm on two packed bf16: w * bf16(x * rstd).  cvt.rn.bf16x2.f32 rounds both products in one instruction and
 // mul.rn.bf16x2 rounds the exact bf16 x bf16 product once — bit-identical to round_bf16(round_bf16(x * rstd) * w) in fp32.

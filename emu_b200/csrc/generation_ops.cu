@@ -241,7 +241,7 @@ __global__ void __launch_bounds__(256) beam_step_kernel(BeamStepArgs a) {
 // the whole group `keep` times with one CTA: 10 dependent passes over 5 x 32k floats, ~0.4 ms of every beam step.)
 constexpr int kTopkThreads = 256;
 constexpr int kTopkMaxKeep = 32;
-constexpr int kTopkMaxParts = 2 * 148;
+constexpr int kTopkMaxParts = 2 * kNumSMs;
 constexpr int kTopkSlice = 4096;  // values per slice (shared-memory items: 32 KB)
 
 __device__ __forceinline__ uint32_t topk_key(float x) {  // monotone map; 0 is reserved for "nothing" (NaN, taken, padding)

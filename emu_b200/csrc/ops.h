@@ -31,13 +31,13 @@ struct GemmEpilogue {
   unsigned long long* dbg = nullptr;  // diagnostics: per-CTA phase time stamps (emu_debug_gemm_phases)
 };
 
-// ---- gemm_tc.cu : tcgen05 GEMM / implicit-GEMM conv ----
+// ---- gemm_tc.cu : wgmma GEMM / implicit-GEMM conv ----
 int gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K, const GemmEpilogue& e,
               cudaStream_t st);
 int conv3x3_bf16(const bf16* X_nhwc, int NB, int H, int W, int Cin, const bf16* Wk, int Cout, const GemmEpilogue& e,
                  cudaStream_t st);
 
-// ---- gemm_skinny.cu : tcgen05 GEMM with the WEIGHTS as the 128-row operand, activations B <= 32 rows (wide decode) ----
+// ---- gemm_skinny.cu : wgmma GEMM with the WEIGHTS as the 128-row operand, activations B <= 32 rows (wide decode) ----
 // plain / +residual / EPI_SWIGLU epilogues, bf16 or fp32 output; K-split partial sums through `ws` (gemm_skinny_workspace_bytes())
 // and `counters` (kSkinnyMaxTiles ints, zeroed once).  EMU_ERR_UNSUPPORTED: shape / epilogue outside this kernel -> gemm_bf16.
 constexpr int kSkinnyMaxUnits = 1024;
@@ -118,9 +118,9 @@ int attn_prefill(const AttnArgs& a, cudaStream_t st);
 int attn_prefill_tc(const AttnArgs& a, cudaStream_t st);  // attention_tc.cu; EMU_ERR_UNSUPPORTED -> use attn_prefill's own kernel
 
 // ---- programmatic dependent launch for kernel chains (UNet / ViT / prefill) ----
-// While a PdlScope is alive on this thread, the PDL-aware launchers (GEMM / conv, tcgen05 attention, LayerNorm,
+// While a PdlScope is alive on this thread, the PDL-aware launchers (GEMM / conv, wgmma attention, LayerNorm,
 // GroupNorm, copy_cols) launch with cudaLaunchAttributeProgrammaticStreamSerialization: the kernel's prologue (CTA launch,
-// barrier init, TMEM allocation, tensor-map prefetch) overlaps the predecessor's tail, and the kernel executes
+// barrier init, tensor-map prefetch) overlaps the predecessor's tail, and the kernel executes
 // griddepcontrol.wait before it touches anything a predecessor wrote.  EMU_NO_PDL=1 disables.
 extern thread_local int g_pdl_chain;
 struct PdlScope {

@@ -5,7 +5,7 @@
 // The module arithmetic itself is diffusers==0.24.0 (third party, not vendored): restated from the published
 // algorithm, see oracle/diffusion_oracle.py ("parity unpinned").
 //
-// B200 mapping: activations live in HBM as NHWC bf16, so every 3x3 convolution is an implicit GEMM on tcgen05
+// H100 mapping: activations live in HBM as NHWC bf16, so every 3x3 convolution is an implicit GEMM on wgmma
 // (4-D TMA tile loads, halo = TMA out-of-bounds zero fill — csrc/gemm_tc.cu) and every Linear is the same kernel
 // with a 2-D A tile; GroupNorm+SiLU is a 2-kernel bandwidth pass; time-embedding add, bias, residual and GEGLU are
 // GEMM epilogues; attention is the flash kernel (head_dim 64).  The whole denoise step (≈1.5 k launches) is

@@ -5,8 +5,8 @@
 // arithmetic is diffusers==0.24.0 (third party, not vendored) restated in oracle/diffusion_oracle.py
 // ("parity unpinned").  The pipeline runs the VAE in bf16 (force_upcast is not honoured by the reference pipeline).
 //
-// Same building blocks as the UNet: NHWC bf16, tcgen05 implicit-GEMM 3x3 convs, 2-kernel GroupNorm+SiLU.  The
-// mid-block attention is single-head with head_dim = 512 (> the flash tile), so it is three GEMMs on tcgen05
+// Same building blocks as the UNet: NHWC bf16, wgmma implicit-GEMM 3x3 convs, 2-kernel GroupNorm+SiLU.  The
+// mid-block attention is single-head with head_dim = 512 (> the flash tile), so it is three GEMMs on wgmma
 // (S = Q K^T, O = P V with V transposed once) around a row-softmax kernel; it runs once per image.
 #include <math.h>
 

@@ -1,4 +1,4 @@
-"""The Emu1 image-generation example on the B200 engine (Emu1/image_inference.py): image blending, text-to-image and in-context
+"""The Emu1 image-generation example on the H100 engine (Emu1/image_inference.py): image blending, text-to-image and in-context
 generation through `EmuGenerationPipeline`, 512 x 512, the reference's guidance scales and output file names."""
 import argparse
 

@@ -1,4 +1,4 @@
-"""The Emu1 example entry point on the B200 engine — what `python inference.py [--instruct] --ckpt-path ...` is in the reference
+"""The Emu1 example entry point on the H100 engine — what `python inference.py [--instruct] --ckpt-path ...` is in the reference
 (Emu1/inference.py; BASELINE configs[0] is its captioning call on CPU).  Same command line, same helper names
 (`prepare_model`, `Emu_inference`, `Emu_instruct_caption`, `pretrain_example`, `instruct_example`), same prompts and example files;
 the model behind them is `emu_b200.emu1.modeling_emu.Emu` and the checkpoint — DeepSpeed `module` wrapper and the `--instruct`

@@ -1,7 +1,7 @@
 """Drop-in for the reference's Emu1 model ``models.modeling_emu.Emu`` (Emu1/models/modeling_emu.py:22-249).
 
 Same public methods and argument meaning: ``generate(samples={"image","prompt"}, ...)`` (:100-185) and
-``generate_image(text, image, placeholder)`` (:187-249).  Arithmetic on the B200 engine: EVA-CLIP-g ViT (pre-norm,
+``generate_image(text, image, placeholder)`` (:187-249).  Arithmetic on the H100 engine: EVA-CLIP-g ViT (pre-norm,
 head_dim 88) + ``ln_visual`` -> Causal-Former (T5 decoder stack, 32 causal queries) -> LLaMA-13B prefill/decode;
 the regression head is ``stu_regress_head`` and regressed embeddings are fed back directly (no project_up).
 """

@@ -6,7 +6,7 @@ Same public surface: ``EmuGenerationPipeline.from_pretrained(path, args=...)`` o
 the optional post-filter), and ``forward(inputs, height=512, width=512, num_inference_steps=50, guidance_scale=7.5)`` returning
 ``(PIL.Image, nsfw flag | None)``.  ``inputs`` is the reference's interleaved list of strings and PIL images.
 
-Arithmetic on the B200 engine: prompt -> ``Emu.generate_image`` (EVA-CLIP-g + Causal-Former + LLaMA-13B regression of 32 visual
+Arithmetic on the H100 engine: prompt -> ``Emu.generate_image`` (EVA-CLIP-g + Causal-Former + LLaMA-13B regression of 32 visual
 embeddings, cached form) for [prompt, ""] -> Stable-Diffusion-1.5-topology UNet (1x1-conv projections, 8 heads per level = head
 widths 40 / 80 / 160, no added conditioning) under classifier-free guidance with the PNDM / PLMS scheduler, one CUDA-graphed
 fused iteration per timestep (emu_denoise_step_multistep) -> VAE decode -> uint8 on the device.

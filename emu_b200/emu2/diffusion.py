@@ -2,7 +2,7 @@
 
 Same public surface — ``from_pretrained`` / ``from_config`` / ``forward(inputs, height, width,
 num_inference_steps, guidance_scale, crop_info, original_size)`` returning an
-``EmuVisualGenerationPipelineOutput(image, nsfw_content_detected)`` — with the arithmetic on the B200 engine:
+``EmuVisualGenerationPipelineOutput(image, nsfw_content_detected)`` — with the arithmetic on the H100 engine:
 prompt encoding through ``EmuModel.generate_image`` / ``encode_image``, the denoise loop as one CUDA-graphed
 ``emu_denoise_step`` per iteration (cat + scale_model_input + UNet + CFG + Euler fused), VAE decode on device.
 

@@ -1,4 +1,4 @@
-"""Drop-in for the reference's ``emu.emu.EmuModel`` (Emu2/emu/emu.py:19-235) on the B200 engine.
+"""Drop-in for the reference's ``emu.emu.EmuModel`` (Emu2/emu/emu.py:19-235) on the H100 engine.
 
 Same constructor signature (vision_cfg, text_decoder_cfg), same public methods and argument meaning:
 ``encode_image``, ``generate``, ``generate_image``; weights enter through ``load_state_dict`` with the reference's

@@ -363,7 +363,7 @@ def release_followers(group=None):
 
 def main(argv=None):
     ap = argparse.ArgumentParser(description="Emu2 demo back end (HTTP contract of Emu2/demo/backend/pytorch_model/backend.py) "
-                                             "on the B200 engine")
+                                             "on the H100 engine")
     ap.add_argument("--port", type=int, default=9000)
     ap.add_argument("--host", type=str, default="0.0.0.0")
     ap.add_argument("--start-card", type=int, default=0)

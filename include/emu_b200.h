@@ -1,4 +1,4 @@
-/* emu_b200 — C ABI of the B200-native engine for baaivision/Emu's multimodal generate path.
+/* emu_b200 — C ABI of the H100-native engine for baaivision/Emu's multimodal generate path.
  *
  * The reference has no FFI: the path sits behind Python methods (SURVEY.md §8b).  These entry points are what a
  * reference-side binding (ctypes, see INTEGRATION.md) calls in place of the library calls the reference makes:
@@ -235,17 +235,16 @@ int emu_beam_step(const float* topk_lp, const int32_t* topk_idx, int batch, int 
 int emu_sample_tokens(const float* logits, int rows, int vocab, float temperature, int top_k, float top_p, int ban_id,
                       uint64_t seed, uint64_t offset, int32_t* out_ids, emu_stream_t s);
 
-/* Diagnostics: emu_op_gemm (bf16 output) with per-CTA phase time stamps.  stamps: DEVICE [148][8] uint64, per CTA
- * {globaltimer ns at entry, then SM clock64 at: entry, set-up done, first TMA issued, first stage landed, last MMA committed,
- * epilogue released, epilogue done} of the CTA's first tile.  tools/gemm_phases.py turns them into the phase table under
- * profiles/. */
+/* Diagnostics: emu_op_gemm (bf16 output) with per-CTA phase time stamps.  stamps: DEVICE [number of SMs][8] uint64, per CTA
+ * {globaltimer ns at entry, then SM clock64 at: entry, set-up done, first TMA issued, first stage landed, last MMA retired,
+ * epilogue started, epilogue done} of the CTA's first tile.  tools/gemm_phases.py turns them into a phase table. */
 int emu_debug_gemm_phases(const void* A, int lda, const void* W, int ldw, int M, int N, int K, const void* bias,
                           const void* residual, int ldr, int epi_mode, void* C, int ldc, int force_bn,
                           unsigned long long* stamps, emu_stream_t s);
 
-/* Diagnostics: emu_op_gemv (bf16 output) with per-CTA phase time stamps.  stamps: DEVICE [148][8] uint64, per CTA {globaltimer
+/* Diagnostics: emu_op_gemv (bf16 output) with per-CTA phase time stamps.  stamps: DEVICE [number of SMs][8] uint64, per CTA {globaltimer
  * ns at entry, then SM clock64 at: entry, barriers ready, dependency resolved (griddepcontrol.wait), x staged, first weight
- * chunk landed, own chunks consumed and rows flushed, exit}.  tools/gemv_phases.py prints the table under profiles/. */
+ * chunk landed, own chunks consumed and rows flushed, exit}.  tools/gemv_phases.py prints the table. */
 int emu_debug_gemv_phases(const void* W, int N, int K, const void* x, int ldx, int B, const void* norm_w, float eps, int mode,
                           const void* residual, int ldr, void* y, int ldy, int pdl, unsigned long long* stamps,
                           emu_stream_t s);

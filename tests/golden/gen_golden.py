@@ -69,7 +69,7 @@ def main():
                   return_tensors="pt")
         out["genimg_mm_input_ids"], out["genimg_mm_attention_mask"] = gi2.input_ids, gi2.attention_mask
     path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu2_tiny.pt")
-    torch.save(out, path)
+    torch.save({k: v.clone() if torch.is_tensor(v) else v for k, v in out.items()}, path)  # no view keeps a larger storage
     print("wrote", path, {k: (tuple(v.shape) if hasattr(v, "shape") else v) for k, v in out.items()})
 
 

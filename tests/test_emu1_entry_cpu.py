@@ -9,7 +9,6 @@ import pytest
 import torch
 from PIL import Image
 
-from oracle import ref_shim
 
 
 def _picture(seed, size=(93, 61)):
@@ -28,21 +27,18 @@ def test_process_img_formula():
     assert torch.equal(x[0], torch.tensor(ref).to(torch.float).permute(2, 0, 1))
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="/root/reference only exists in the authoring container")
-def test_process_img_and_get_index_vs_live_reference():
-    import importlib.util
-    if "decord" not in sys.modules:
-        sys.modules["decord"] = types.ModuleType("decord")
-        sys.modules["decord"].VideoReader = object          # imported at module level by the reference, unused here
-    spec = importlib.util.spec_from_file_location("emu1_ref_utils", "/root/reference/Emu1/utils.py")
-    ref = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(ref)
+def test_process_img_and_get_index_vs_reference():
+    """bit-identical to the reference's own utils.process_img / get_index (tests/golden/live_reference.pt: the tensors
+    as SHA-256 digests of their bytes)"""
+    import os
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+    from gen_golden_live import FRAMES, PICTURES, digest, picture
+    gold = torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live_reference.pt"))
     from emu_b200.emu1 import utils as mine
-    for seed, size in ((1, (640, 480)), (2, (100, 333)), (3, (224, 224))):
-        img = _picture(seed, size)
-        assert torch.equal(mine.process_img(img=img, device=torch.device("cpu")), ref.process_img(img=img, device=torch.device("cpu")))
-    for frames, segs in ((300, 8), (9, 8), (17, 4), (1000, 8)):
-        assert np.array_equal(mine.get_index(frames, segs), ref.get_index(frames, segs))
+    for (seed, size), want in zip(PICTURES, gold["process_img"]):
+        assert digest(mine.process_img(img=picture(seed, size), device=torch.device("cpu"))) == want
+    for (frames, segs), want in zip(FRAMES, gold["get_index"]):
+        assert np.array_equal(mine.get_index(frames, segs), want.numpy())
 
 
 class _FakeEmu:

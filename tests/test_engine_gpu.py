@@ -222,7 +222,7 @@ def wide_model(cuda, sd):
 
 
 def test_wide_decode_more_than_8_rows(wide_model, sd):
-    """More than 8 cache rows (BASELINE config 4: 4 prompts x 5 beams = 20) decode on the tcgen05 GEMM path with the same
+    """More than 8 cache rows (BASELINE config 4: 4 prompts x 5 beams = 20) decode on the wgmma GEMM path with the same
     rounding points: prefill + 3 teacher-forced steps of 11 left-padded sequences against the fp32 and bf16-policy oracles."""
     m = wide_model
     g = torch.Generator().manual_seed(91)

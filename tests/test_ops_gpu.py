@@ -226,8 +226,8 @@ def test_attn_prefill(cuda, B, Nq, Nk, H, D, causal):
     (1, 1025, 1025, 2, 112, False, 6.0, True), (2, 256, 64, 2, 64, False, 1.0, False),
 ])
 def test_attn_prefill_tc(cuda, B, Nq, Nk, H, D, causal, qscale, fused):
-    """tcgen05 flash attention (attention_tc.cu): multi-tile, ragged, causal with Nk > Nq and left padding, large score
-    ranges (exercises the lazy max / TMEM rescale path), and head-interleaved fused-QKV strides."""
+    """wgmma flash attention (attention_tc.cu): multi-tile, ragged, causal with Nk > Nq and left padding, large score
+    ranges (exercises the online max / O rescale), and head-interleaved fused-QKV strides."""
     from emu_b200 import _lib
     if fused and Nq == Nk:
         qkv = _rand((B, Nq, 3, H, D), 27)

@@ -1,6 +1,6 @@
 """CPU: the oracle restatement (oracle/emu_oracle.py) against the golden outputs of the UNMODIFIED reference
-(tests/golden/emu2_tiny.pt, made by tests/golden/gen_golden.py) and — when /root/reference is present — against the
-reference imported live."""
+(tests/golden/emu2_tiny.pt, made by tests/golden/gen_golden.py, and tests/golden/live_reference.pt, made by
+tests/golden/gen_golden_live.py)."""
 import os
 
 import numpy as np
@@ -9,9 +9,10 @@ import torch
 import torch.nn.functional as F
 
 from helpers import TINY_LLAMA, TINY_VISION, make_emu2_state_dict
-from oracle import emu_oracle as O, ref_shim
+from oracle import emu_oracle as O
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "emu2_tiny.pt")
+LIVE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live_reference.pt")
 L, NH = TINY_LLAMA["num_hidden_layers"], TINY_LLAMA["num_attention_heads"]
 
 
@@ -64,24 +65,15 @@ def test_generate_image_literal_and_cached(gold, sd):
     assert O.rel_err(out2, gold["genimg_mm"]) < 1e-4
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="reference tree not present (GPU box)")
-def test_oracle_vs_live_reference(sd):
-    d = ref_shim.make_llama_config_dir(TINY_LLAMA["hidden_size"], L, NH, TINY_LLAMA["intermediate_size"])
-    vk = dict(TINY_VISION)
-    model = ref_shim.build_emu2_model(vk, d)
-    model.load_state_dict(sd, strict=True)
+def test_oracle_vs_reference_encode_and_generate_image(sd):
+    """encode_image and generate_image of the reference's EmuModel on the tiny model; generate_image's tokenizer ids
+    of every iteration come with the golden"""
+    ref = torch.load(LIVE)["emu2"]
     img = torch.randn(1, 3, 56, 56, generator=torch.Generator().manual_seed(5))
-    with torch.no_grad():
-        ref = model.encode_image(img)
-        gi = model.generate_image(text=["two dogs"])
-    assert O.rel_err(O.encode_image(sd, img, patch=14, num_heads=4, layers=2, n_query=4), ref) < 1e-5
-    tok = model.decoder.tokenizer
-
-    def ids_fn(k):
-        i = tok(["two dogs[IMG]" + "<image>" * k], padding="longest", return_tensors="pt")
-        return i.input_ids, i.attention_mask
-    lit = O.generate_image_regress(sd, ids_fn, 4, layers=L, heads=NH, image_token_id=32003, boi_token_id=32001)
-    assert O.rel_err(lit, gi) < 1e-5
+    assert O.rel_err(O.encode_image(sd, img, patch=14, num_heads=4, layers=2, n_query=4), ref["encode_image"]) < 1e-5
+    lit = O.generate_image_regress(sd, lambda k: ref["ids"][k], 4, layers=L, heads=NH, image_token_id=32003,
+                                   boi_token_id=32001)
+    assert O.rel_err(lit, ref["generate_image"]) < 1e-5
 
 
 @pytest.mark.parametrize("H,W,S", [(37, 53, 16), (500, 333, 448), (448, 448, 448), (1024, 768, 448), (100, 100, 224),
@@ -124,20 +116,19 @@ def test_t5_oracle_vs_reference_golden():
     assert torch.equal(out16, g["out_bf16"])
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="/root/reference only exists in the authoring container")
-def test_t5_oracle_vs_live_reference_t5_base():
-    """Same, against the live reference at the real t5-base dimensions (12 layers, d_model 768) with its own default
-    initialisation — bit-exact."""
-    from oracle import t5_oracle as T
-    CF = ref_shim.import_emu1_causal_former()
-    torch.manual_seed(0)
-    m = CF(None, n_causal=32, vision_width=1408, output_dim=512).eval()
-    x = torch.randn(1, 257, 1408)
-    for dt in (torch.float32, torch.bfloat16):  # the module is created half bf16 / half fp32: make it uniform first
-        m = m.to(dt)
-        sd = {"cformer." + k: v.detach().clone() for k, v in m.state_dict().items()}
-        with torch.no_grad():
-            assert torch.equal(m(x.to(dt)), T.causal_former(sd, x.to(dt)))
+def test_t5_oracle_vs_reference_t5_base():
+    """Same, against the reference at the real t5-base dimensions (12 layers, d_model 768; seeded weights, fp32 and
+    bf16) — bit-exact."""
+    from oracle import diffusion_oracle as D, t5_oracle as T
+    ref = torch.load(LIVE)["t5_base"]
+    sd = D.random_state_dict(T.param_shapes(T.T5_BASE, 1408, 512, n_causal=32), seed=ref["seed"])
+    for k in sd:
+        if k.endswith("Attention.q.weight"):
+            sd[k] = sd[k] * 0.125
+    x = torch.randn(1, 257, 1408, generator=torch.Generator().manual_seed(ref["seed"] + 1))
+    for name, dt in (("fp32", torch.float32), ("bf16", torch.bfloat16)):
+        sdt = {k: v.to(dt) for k, v in sd.items()}
+        assert torch.equal(T.causal_former(sdt, x.to(dt)), ref["out_" + name])
 
 
 def test_emu1_oracle_vs_reference_golden():
@@ -156,15 +147,13 @@ def test_emu1_oracle_vs_reference_golden():
         assert torch.equal(T.causal_former(sd, feats, emu1_t5_cfg()), g["cformer_out"])
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="/root/reference only exists in the authoring container")
-def test_emu1_vit_oracle_vs_live_reference():
-    from helpers import EMU1_VIS88
-    vit = ref_shim.build_emu1_vit(EMU1_VIS88)
-    sd = {"visual." + k: v.detach().clone() for k, v in vit.state_dict().items()}
+def test_emu1_vit_oracle_vs_reference():
+    """forward_features of the reference's Emu1 EVA ViT (head width 88, seeded weights) — bit-exact"""
+    from oracle import diffusion_oracle as D
+    ref = torch.load(LIVE)["emu1_vit"]
+    sd = {"visual." + k: v for k, v in D.random_state_dict(ref["shapes"], seed=ref["seed"]).items()}
     img = torch.randn(2, 3, 56, 56, generator=torch.Generator().manual_seed(9))
-    with torch.no_grad():
-        ref = vit.forward_features(img)
-    assert torch.equal(ref, O.vit_forward_features(sd, img, patch=14, num_heads=2, layers=2, postnorm=False))
+    assert torch.equal(ref["features"], O.vit_forward_features(sd, img, patch=14, num_heads=2, layers=2, postnorm=False))
 
 
 def _emu1_generate_image_oracle(sd, ids, image, vis):

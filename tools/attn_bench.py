@@ -1,4 +1,4 @@
-"""Micro-benchmark of emu_op_attn_prefill on the hot-path shapes (run twice: default = tcgen05 kernel, EMU_ATTN=legacy =
+"""Micro-benchmark of emu_op_attn_prefill on the hot-path shapes (run twice: default = wgmma kernel, EMU_ATTN=legacy =
 mma.sync kernel).  CUDA events, 3 warm-ups, inputs re-used (they fit L2 for the small shapes; stated in the output)."""
 import os
 import sys
@@ -63,7 +63,7 @@ def main():
         out = torch.empty(B, N, H, D, dtype=torch.bfloat16, device="cuda")
         us = graph_us(lambda: _lib.op_attn_prefill(q, k, v, D ** -0.5, causal=causal))
         print("%-34s %8.3f ms  %7.1f TFLOP/s | in-graph %8.1f us %7.1f TFLOP/s  [%s]"
-              % (name, ms, flops / ms / 1e9, us, flops / us / 1e6, os.environ.get("EMU_ATTN", "tcgen05")), flush=True)
+              % (name, ms, flops / ms / 1e9, us, flops / us / 1e6, os.environ.get("EMU_ATTN", "wgmma")), flush=True)
     for name, B, Nq, Nk, H, D in CROSS:
         q = (torch.randn(B, Nq, H, D, generator=g) * 0.5).to(torch.bfloat16).cuda()
         kv = (torch.randn(B, Nk, 2, H, D, generator=g) * 0.5).to(torch.bfloat16).cuda()

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM / implicit-GEMM conv on the hot-path shapes (UNet levels, ViT, LLaMA prefill).
+"""Micro-benchmark of the wgmma GEMM / implicit-GEMM conv on the hot-path shapes (UNet levels, ViT, LLaMA prefill).
 CUDA events, 3 warm-ups, 20 timed launches back to back (weights + activations of one launch fit L2 for the small shapes)."""
 import os
 import sys

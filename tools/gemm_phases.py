@@ -1,4 +1,4 @@
-"""Where the time of a tcgen05 GEMM launch goes: per-CTA phase stamps (emu_debug_gemm_phases) on the UNet / ViT shapes, plus
+"""Where the time of a wgmma GEMM launch goes: per-CTA phase stamps (emu_debug_gemm_phases) on the UNet / ViT shapes, plus
 the launch-to-launch time of the same GEMM replayed inside a CUDA graph (no host launch overhead, L2-warm like the model)."""
 import os
 import sys

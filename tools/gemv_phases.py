@@ -28,7 +28,7 @@ def main():
         nw = torch.ones(H, device="cuda", dtype=torch.bfloat16)
         outs = {n: torch.empty(B, n, device="cuda", dtype=torch.bfloat16) for _, n, _, _, _ in shapes}
         outs[Fl] = torch.empty(B, Fl, device="cuda", dtype=torch.bfloat16)
-        stamps = [[torch.zeros(148, 8, dtype=torch.int64, device="cuda") for _ in shapes] for _ in range(layers)]
+        stamps = [[torch.zeros(2 * 132, 8, dtype=torch.int64, device="cuda") for _ in shapes] for _ in range(layers)]
 
         def run():
             for l in range(layers):

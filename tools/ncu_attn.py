@@ -1,4 +1,4 @@
-"""Tiny driver for `ncu --set full` on the tcgen05 attention kernel: python tools/ncu_attn.py B N H D [causal]"""
+"""Tiny driver for `ncu --set full` on the wgmma attention kernel: python tools/ncu_attn.py B N H D [causal]"""
 import os
 import sys
 

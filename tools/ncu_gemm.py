@@ -1,4 +1,4 @@
-"""Tiny driver for `ncu --set full` on one tcgen05 GEMM shape: python tools/ncu_gemm.py M N K [force_bn] [epi]"""
+"""Tiny driver for `ncu --set full` on one wgmma GEMM shape: python tools/ncu_gemm.py M N K [force_bn] [epi]"""
 import os
 import sys
 

@@ -77,7 +77,7 @@ def main():
 
     errs, ratios = [], []
     # B = 2: the skinny-GEMV decode path (exchange fused into the GEMV epilogue); B = 11: the wide path (> 8 cache rows:
-    # tcgen05 skinny GEMM + peer-memory reduce kernel), both with left padding
+    # wgmma skinny GEMM + peer-memory reduce kernel), both with left padding
     for B in (2, 11):
         g = torch.Generator().manual_seed(5 + B)
         ids = torch.randint(100, 30000, (B, 9), generator=g)
