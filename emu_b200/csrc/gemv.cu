@@ -6,68 +6,76 @@
 // 64.6 GB of bf16 weights (HF LlamaDecoderLayer q/k/v/o/gate/up/down + lm_head, driven from
 // Emu2/emu/emu.py:213-229 and :133-138), so the kernel is judged on HBM GB/s, not FLOPs.
 //
-// Work decomposition ("stream-K"): the weight matrix is cut into chunks of (16*RT rows) x 256 columns.  A
-// persistent grid of 2 CTAs per SM gives every CTA the SAME number of consecutive chunks (+-1), so all SMs stream
-// the same number of bytes and finish together — no wave quantisation whatever N and K are.  A row group whose chunks straddle
-// CTAs is finished by whichever CTA arrives last (per-group counter; partial sums are added in a fixed order, so
-// results are run-to-run deterministic).
-//
-// Inside a CTA the 8 warps each own one 32-column block of the current chunk; every lane streams 16-byte pieces
-// of 2*RT rows with ld.global.nc.L1::no_allocate (each request = 64 B contiguous per row, 8 rows) through a
-// register ring holding 16 loads in flight per lane (128 KB per SM), with plain pointer increments in the steady
-// state (~11 SASS instructions per KB; a first stream-K cut with 16-row chunks and per-chunk address math was
-// instruction-issue bound at 3 TB/s).  The tiny x operand (<= 8 rows) is staged once per CTA in shared memory —
-// optionally through a fused RMSNorm prologue (HF LlamaRMSNorm rounding) — and fed as the 8-wide N operand of
-// mma.sync.m16n8k16, so batch 1..8 (greedy .. 5-beam search) all run at the same bandwidth-bound speed.
-// Epilogues: bias / residual / SwiGLU / RoPE + KV-cache append.  Launched with programmatic dependent launch: the
-// ring is filled before griddepcontrol.wait, so HBM keeps streaming while the previous kernel drains.
-#include <stdlib.h>
+// The bytes in flight live in shared memory:
+//   * one producer thread issues cp.async.bulk.tensor (TMA) loads of [32 rows x 64 cols] 128B-swizzled tiles into an
+//     8-stage x 16 KB ring signalled by mbarriers — 128 KB in flight per SM with zero registers and zero address math
+//     (a deep prefetch rather than a shallower ring that would let the PDL successor co-reside);
+//   * 8 consumer warps pull A fragments with ldmatrix (conflict-free through the swizzle) and run mma.sync.m16n8k16 with
+//     the staged x rows as the 8-wide N operand, then release the stage — batch 1..8 (greedy .. 5-beam search) all run
+//     at the same bandwidth-bound speed;
+//   * ONE persistent CTA per SM (grid = kNumSMs), stream-K over (row group, k chunk) units: every CTA gets the same
+//     number of consecutive chunks (+-1), so all SMs stream the same number of bytes whatever N and K are.  A row group
+//     whose chunks straddle CTAs is finished by whichever CTA arrives last (per-group counter; partial sums are added in a
+//     fixed order, so results are run-to-run deterministic).  With PDL the producer starts streaming weights before
+//     griddepcontrol.wait resolves.
+// x (batch <= 8 rows) reaches shared memory by one cp.async.bulk per row, optionally through a fused RMSNorm (HF
+// LlamaRMSNorm rounding) applied in place.  When batch x K does not fit next to the ring (5 beams x 17920) x is staged in
+// K segments that are re-staged as the chunk stream crosses them (GemvTmaParams::xsc).
+// Ragged N and K tails cost nothing (TMA zero-fills out-of-bounds rows/columns).
+// Epilogues: bias / residual / SwiGLU / RoPE + KV-cache append / tensor-parallel {value, flag} push.
+#include <stdio.h>
 
 #include "common.cuh"
 #include "ops.h"
 
 namespace emu {
 
-int gemv_tma_bf16(const GemvArgs& a, cudaStream_t st);  // gemv_tma.cu
-int gemv_tma_init();
-int gemv_reg_bf16(const GemvArgs& a, cudaStream_t st);
+int make_tmap_2d(CUtensorMap* out, const void* base, long rows, long cols, long ld, int box_rows);  // gemm_tc.cu
 
-constexpr int kGemvWarps = 8;
-constexpr int kGemvThreads = kGemvWarps * 32;
-constexpr int kMaxParts = 8;    // CTAs that may share one row group
-constexpr int kWsTiles = 8192;  // workspace capacity in 16-row tiles (N <= 131072)
+constexpr int kTW = 8;                  // consumer warps
+constexpr int kTThreads = (kTW + 1) * 32;  // + 1 producer warp
+constexpr int kTRT = 2;                 // 16-row tiles per chunk
+constexpr int kTRows = 16 * kTRT;       // 32 rows
+constexpr int kTCols = 256;             // columns per chunk (4 TMA tiles of 64)
+constexpr int kTStageBytes = kTRows * kTCols * 2;  // 16 KB
+constexpr int kTStages = 10;  // ring slots carved; p.nstages of them are used
+constexpr int kTMaxParts = 8;
+constexpr int kTWsGroups = 8192;
 
-struct GemvParams {
+struct GemvTmaParams {
   GemvArgs a;
-  int ldxs;       // smem row stride of staged x (elements)
-  int red_off;    // byte offset of the reduction buffers
-  int cpt;        // chunks per row group (= ceil(K / 256))
-  int rt;         // 16-row tiles per group
-  long total;     // total chunks
-  float* ws;      // [groups][kMaxParts][rt*128]
-  int* counters;  // [groups], self-resetting
+  int ldxs;      // smem row stride of staged x (elements), = xsc * 256 + 8
+  int kpad;      // K rounded up to 256
+  int cpt;       // chunks per row group
+  int xsc;       // chunks of x staged in shared memory at a time (== cpt: the whole row; smaller: K segments that are
+                 //   re-staged as the chunk stream crosses them — batch x K too large for shared memory, e.g. 5 x 17920)
+  int nstages;   // ring depth actually used (<= kTStages)
+  int geff;      // number of CTAs that share this matrix's chunks (<= gridDim.x); CTAs >= geff get none
+  long total;    // total chunks
+  float* ws;     // [groups][kTMaxParts][kTRT*128]
+  int* counters;
 };
 
-// Finish the k-segment [kc_lo, kc_hi] of row group `grp`; per-warp partial sums are already in `red`.
-// Called uniformly by all threads of the CTA.  Kept out of line: it runs once per row group, and inlining it into
-// the unrolled streaming loop blew the instruction cache.
-__device__ __noinline__ void gemv_flush(const GemvParams* sp, float* red, float* fin, int* s_last_p, int grp, int kc_lo,
-                                        int kc_hi) {
-  const GemvParams& p = *sp;
+static __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// finish k-segment [kc_lo, kc_hi] of row group grp (consumer threads only; `red` already holds per-warp partials).
+// Kept out of line: it runs once per row group, and inlining it into the chunk loop bloats the instruction stream.
+static __device__ __noinline__ void gemv_tma_flush(const GemvTmaParams* sp, float* red, float* fin, int* s_last_p, int grp,
+                                            int kc_lo, int kc_hi) {
+  const GemvTmaParams& p = *sp;
   const GemvArgs& a = p.a;
-  const int N = a.N, B = a.B, CPT = p.cpt, RT = p.rt;
-  const int nval = RT * 128;
-  const long G = gridDim.x;
-  __syncthreads();
+  const int N = a.N, B = a.B, CPT = p.cpt;
+  constexpr int nval = kTRT * 128;
+  const long G = p.geff;
+  const int tid = threadIdx.x;  // < 256
+  consumer_bar();
   const bool whole = (kc_lo == 0 && kc_hi == CPT - 1);
   bool do_epilogue = whole;
-  if (whole) {
-    for (int idx = threadIdx.x; idx < nval; idx += kGemvThreads) {
-      float v = 0.f;
+  float v = 0.f;
 #pragma unroll
-      for (int w = 0; w < kGemvWarps; ++w) v += red[w * nval + idx];
-      fin[idx] = v;
-    }
+  for (int w = 0; w < kTW; ++w) v += red[w * nval + tid];
+  if (whole) {
+    fin[tid] = v;
   } else {
     // owner(x) = largest c with floor(c*total/G) <= x  =  floor(((x+1)*G - 1) / total)
     const long first_chunk = (long)grp * CPT;
@@ -75,347 +83,525 @@ __device__ __noinline__ void gemv_flush(const GemvParams* sp, float* red, float*
     const int last_owner = (int)(((first_chunk + CPT) * G - 1) / p.total);
     const int nparts = last_owner - first_owner + 1;
     const int my = (int)blockIdx.x - first_owner;
-    float* wt = p.ws + ((long)grp * kMaxParts) * nval;
-    for (int idx = threadIdx.x; idx < nval; idx += kGemvThreads) {
-      float v = 0.f;
-#pragma unroll
-      for (int w = 0; w < kGemvWarps; ++w) v += red[w * nval + idx];
-      wt[my * nval + idx] = v;
-    }
+    float* wt = p.ws + ((long)grp * kTMaxParts) * nval;
+    wt[my * nval + tid] = v;
     __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
+    consumer_bar();
+    if (tid == 0) {
       const int prev = atomicAdd(&p.counters[grp], 1);
       *s_last_p = (prev == nparts - 1);
       if (prev == nparts - 1) p.counters[grp] = 0;  // self-reset for the next launch / graph replay
     }
-    __syncthreads();
+    consumer_bar();
     do_epilogue = *s_last_p != 0;
     if (do_epilogue) {
       __threadfence();
-      for (int idx = threadIdx.x; idx < nval; idx += kGemvThreads) {
-        float s = 0.f;
-        for (int q = 0; q < nparts; ++q) s += __ldcg(&wt[q * nval + idx]);  // fixed order: deterministic
-        fin[idx] = s;
-      }
+      float s = 0.f;
+      for (int q = 0; q < nparts; ++q) s += __ldcg(&wt[q * nval + tid]);  // fixed order: deterministic
+      fin[tid] = s;
     }
   }
-  if (do_epilogue) {  // uniform across the CTA
-    __syncthreads();
-    // fin[rt*128 + r*8 + b] holds the full dot product of row (grp*RT + rt)*16 + r with x[b]
-    for (int idx = threadIdx.x; idx < nval; idx += kGemvThreads) {
-      const int rt = idx >> 7, r = idx & 15, b = (idx >> 4) & 7;
-      const float* f = fin + rt * 128;
-      const int nrow = (grp * RT + rt) * 16 + r;
-      if (b >= B || nrow >= N) continue;
-      if (a.mode == EPI_NONE) {
-        float v = f[r * 8 + b];
-        if (a.bias) v += __bfloat162float(a.bias[nrow]);
-        if (a.residual) v = round_bf16(v) + __bfloat162float(a.residual[(long)b * a.ldr + nrow]);
-        if (a.out_fp32) reinterpret_cast<float*>(a.y)[(long)b * a.ldy + nrow] = v;
-        else reinterpret_cast<bf16*>(a.y)[(long)b * a.ldy + nrow] = __float2bfloat16_rn(v);
+  if (do_epilogue) {
+    consumer_bar();
+    // fin[rt*128 + r*8 + b] holds the full dot product of row (grp*kTRT + rt)*16 + r with x[b]
+    const int rt = tid >> 7, r = tid & 15, b = (tid >> 4) & 7;
+    const float* f = fin + rt * 128;
+    const int nrow = (grp * kTRT + rt) * 16 + r;
+    if (b < B && nrow < N) {
+      if (a.mode == EPI_NONE && a.ll_n > 0) {
+        // fused tensor-parallel push: {value, flag} words are self-validating, so no fence / separate flag round trip
+        const unsigned flag = __ldcg(a.ll_step) * 256u + (unsigned)a.ll_idx + 1u;
+        const unsigned bits = __float_as_uint(f[r * 8 + b]);
+        const size_t off = ((size_t)(a.ll_idx & 1) * a.ll_n + a.ll_rank) * a.ll_slot_elems + (size_t)b * a.ldy + nrow;
+        for (int pr = 0; pr < a.ll_n; ++pr)
+          asm volatile("st.global.v2.b32 [%0], {%1, %2};" ::"l"(reinterpret_cast<uint2*>(a.ll_peer[pr]) + off), "r"(bits),
+                       "r"(flag)
+                       : "memory");
+      } else if (a.mode == EPI_NONE) {
+        float o = f[r * 8 + b];
+        if (a.bias) o += __bfloat162float(a.bias[nrow]);
+        if (a.residual)
+          o = round_bf16(o) + __uint_as_float((uint32_t)__ldcg(reinterpret_cast<const unsigned short*>(a.residual) + (long)b * a.ldr + nrow) << 16);
+        if (a.out_fp32) reinterpret_cast<float*>(a.y)[(long)b * a.ldy + nrow] = o;
+        else reinterpret_cast<bf16*>(a.y)[(long)b * a.ldy + nrow] = __float2bfloat16_rn(o);
       } else if (a.mode == EPI_SWIGLU) {
-        if (r & 1) continue;
-        const float gate = round_bf16(f[r * 8 + b]), up = round_bf16(f[(r + 1) * 8 + b]);
-        const float v = round_bf16(silu(gate)) * up;
-        reinterpret_cast<bf16*>(a.y)[(long)b * a.ldy + (nrow >> 1)] = __float2bfloat16_rn(v);
+        if (!(r & 1)) {
+          const float gate = round_bf16(f[r * 8 + b]), up = round_bf16(f[(r + 1) * 8 + b]);
+          reinterpret_cast<bf16*>(a.y)[(long)b * a.ldy + (nrow >> 1)] = __float2bfloat16_rn(round_bf16(silu(gate)) * up);
+        }
       } else {  // GEMV_ROPE_QKV
         const int D = a.head_dim, H = a.n_heads;
         const int hh = nrow / D, i = nrow - hh * D;
         const int slot = a.pos[b];
         if (hh < 2 * H) {
-          if (r & 1) continue;
-          const float x1 = round_bf16(f[r * 8 + b]), x2 = round_bf16(f[(r + 1) * 8 + b]);
-          const int rp = slot - (a.pos_off ? a.pos_off[b] : 0);
-          const float c = __bfloat162float(a.rope_cos[(long)rp * (D / 2) + (i >> 1)]);
-          const float s = __bfloat162float(a.rope_sin[(long)rp * (D / 2) + (i >> 1)]);
-          // HF apply_rotary_pos_emb in bf16: (q*cos) + (rotate_half(q)*sin), each op rounded
-          const float o1 = round_bf16(x1 * c) + round_bf16(-x2 * s);
-          const float o2 = round_bf16(x2 * c) + round_bf16(x1 * s);
-          bf16* dst;
-          if (hh < H) dst = reinterpret_cast<bf16*>(a.y) + (long)b * a.ldy + nrow;
-          else dst = a.k_cache + (((long)b * H + (hh - H)) * a.t_max + slot) * D + i;
-          *reinterpret_cast<uint32_t*>(dst) = pack_bf16(o1, o2);
+          if (!(r & 1)) {
+            const float x1 = round_bf16(f[r * 8 + b]), x2 = round_bf16(f[(r + 1) * 8 + b]);
+            const int rp = slot - (a.pos_off ? a.pos_off[b] : 0);
+            const float c = __bfloat162float(a.rope_cos[(long)rp * (D / 2) + (i >> 1)]);
+            const float s = __bfloat162float(a.rope_sin[(long)rp * (D / 2) + (i >> 1)]);
+            // HF apply_rotary_pos_emb in bf16: (q*cos) + (rotate_half(q)*sin), each op rounded
+            const float o1 = round_bf16(x1 * c) + round_bf16(-x2 * s);
+            const float o2 = round_bf16(x2 * c) + round_bf16(x1 * s);
+            bf16* dst;
+            if (hh < H) dst = reinterpret_cast<bf16*>(a.y) + (long)b * a.ldy + nrow;
+            else dst = a.k_cache + (((long)b * H + (hh - H)) * a.t_max + slot) * D + i;
+            *reinterpret_cast<uint32_t*>(dst) = pack_bf16(o1, o2);
+          }
         } else {
           a.v_cache[(((long)b * H + (hh - 2 * H)) * a.t_max + slot) * D + i] = __float2bfloat16_rn(f[r * 8 + b]);
         }
       }
     }
   }
-  __syncthreads();
+  consumer_bar();
 }
 
-// RT: 16-row tiles per chunk (1/2/4).  KFULL: K % 256 == 0, i.e. every warp's k-block is valid in every chunk.
-template <int RT, bool KFULL>
-__global__ void __launch_bounds__(kGemvThreads, 2) gemv_kernel(const GemvParams p) {
-  constexpr int SLOTS = 8 / RT;  // ring slots, each RT*2 loads: 16 loads in flight per lane
-  const GemvArgs& a = p.a;
-  extern __shared__ __align__(16) uint8_t smem[];
-  bf16* xs = reinterpret_cast<bf16*>(smem);
-  float* red = reinterpret_cast<float*>(smem + p.red_off);  // [8 warps][RT][16][8]
-  float* fin = red + kGemvWarps * RT * 128;                 // [RT][16][8]
-  __shared__ float s_ss[kGemvWarps][8];
-  __shared__ float s_rstd[8];
-  __shared__ int s_last;
-  __shared__ GemvParams s_params;
-  if (threadIdx.x == 0) s_params = p;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
-  const int K = a.K, N = a.N, B = a.B;
-  const int KB = K >> 5, CPT = p.cpt;
-  const long G = gridDim.x;
-  const long c0 = (long)blockIdx.x * p.total / G, c1 = ((long)blockIdx.x + 1) * p.total / G;
-  const int n = (int)(c1 - c0);
-
-  // ---- load stream state: 2*RT row pointers that advance by 256 elements per chunk ----
-  int ld_grp = (int)(c0 / CPT), ld_kc = (int)(c0 % CPT);
-  const bf16* lp[RT][2];
-  auto set_ptrs = [&](int grp, int kc) {
+// ---- producer: stream this CTA's chunk range [c0, c1) of one weight matrix through the ring ----
+static __device__ __forceinline__ void tma_produce(const CUtensorMap* tm, int cpt, long c0, long c1, uint8_t* ring,
+                                                   uint64_t* full_bar, uint64_t* empty_bar, int nstages, int& stage,
+                                                   uint32_t& phase) {
+  int grp = (int)(c0 / cpt), kc = (int)(c0 % cpt);
+  for (long i = c0; i < c1; ++i) {
+    mbar_wait(&empty_bar[stage], phase ^ 1);
+    uint8_t* dst = ring + stage * kTStageBytes;
+    mbar_expect_tx(&full_bar[stage], kTStageBytes);
 #pragma unroll
-    for (int rt = 0; rt < RT; ++rt)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        int row = (grp * RT + rt) * 16 + g + 8 * h;
-        row = row < N ? row : N - 1;  // ragged last group: clamp (results of clamped rows are never stored)
-        lp[rt][h] = a.W + (long)row * K + ((long)kc * kGemvWarps + warp) * 32 + t * 8;
-      }
-  };
-  set_ptrs(ld_grp, ld_kc);
-  uint4 ring[SLOTS][RT][2];
-  auto load_next = [&](uint4(&slot)[RT][2]) {
-    const bool valid = KFULL || (ld_kc * kGemvWarps + warp < KB);
-#pragma unroll
-    for (int rt = 0; rt < RT; ++rt)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        slot[rt][h] = valid ? ldg_stream(lp[rt][h]) : make_uint4(0, 0, 0, 0);
-        lp[rt][h] += 256;
-      }
-    if (++ld_kc == CPT) {
-      ld_kc = 0;
-      ++ld_grp;
-      set_ptrs(ld_grp, 0);
-    }
-  };
-  // weights do not depend on the previous kernel: fill the ring before the grid dependency resolves
-#pragma unroll
-  for (int j = 0; j < SLOTS; ++j)
-    if (j < n) load_next(ring[j]);
-  if (a.pdl) {
-    pdl_launch_dependents();
-    pdl_wait();
+    for (int j = 0; j < 4; ++j)
+      tma_load_2d(dst + j * (kTRows * 128), tm, &full_bar[stage], kc * kTCols + j * 64, grp * kTRows);
+    if (++stage == nstages) { stage = 0; phase ^= 1; }
+    if (++kc == cpt) { kc = 0; ++grp; }
   }
+}
 
-  // ---- stage x (optionally RMS-normalised) into shared memory ----
+// ---- consumers: stage x (optionally RMS-normalised, zero padded to kpad) into shared memory ----
+// Staging sits on the critical path of every GEMV (the weight ring is full long before it ends), so it is written for
+// latency: every batch row of a segment is one bulk copy, all in flight at once, and the norm weights — which do not
+// depend on the predecessor kernel — are fetched by the caller before griddepcontrol.wait (XPre).
+// LlamaRMSNorm on two packed bf16: w * bf16(x * rstd).  cvt.rn.bf16x2.f32 rounds both products in one instruction and
+// mul.rn.bf16x2 rounds the exact bf16 x bf16 product once — bit-identical to round_bf16(round_bf16(x * rstd) * w) in fp32.
+static __device__ __forceinline__ uint32_t rmsnorm_pair(uint32_t x2, float rstd, uint32_t w2) {
+  const float lo = __uint_as_float(x2 << 16) * rstd, hi = __uint_as_float(x2 & 0xffff0000u) * rstd;
+  uint32_t n2, o2;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(n2) : "f"(hi), "f"(lo));
+  asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(o2) : "r"(n2), "r"(w2));
+  return o2;
+}
+struct XPre {
+  uint4 w[4];  // this thread's norm-weight vectors of columns (threadIdx.x + 256 j) * 8, j < 4 (K <= 8192)
+  bool have = false;
+};
+static __device__ __forceinline__ void tma_prefetch_norm_w(const GemvTmaParams& p, XPre& pre) {
+  const GemvArgs& a = p.a;
+  pre.have = false;
+  if (a.norm_w == nullptr || (a.K >> 3) > 1024) return;
+  const uint4* wsrc = reinterpret_cast<const uint4*>(a.norm_w);
+  const int vec_per_row = a.K >> 3;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int gi = (int)threadIdx.x + 256 * j;
+    pre.w[j] = gi < vec_per_row ? __ldg(wsrc + gi) : make_uint4(0, 0, 0, 0);
+  }
+  pre.have = true;
+}
+
+// per-warp sums of squares of every batch row -> s_rstd[b], folded over the warps in a fixed order
+static __device__ __forceinline__ void rstd_from_ss(const float (&ss)[8], float (*s_ss)[8], float* s_rstd, int K, float eps) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) {
+#pragma unroll
+    for (int b = 0; b < 8; ++b) s_ss[warp][b] = ss[b];
+  }
+  consumer_bar();
+  if (threadIdx.x < 8) {
+    float tot = 0.f;
+#pragma unroll
+    for (int w = 0; w < kTW; ++w) tot += s_ss[w][threadIdx.x];
+    s_rstd[threadIdx.x] = rsqrtf(tot / (float)K + eps);
+  }
+  consumer_bar();
+}
+
+// RMSNorm statistics of x read from global memory: a segmented row is never whole in shared memory
+static __device__ __forceinline__ void x_norm_stats_global(const GemvTmaParams& p, float (*s_ss)[8], float* s_rstd) {
+  const GemvArgs& a = p.a;
+  const int K = a.K, B = a.B;
   const int vec_per_row = K >> 3;
-  if (a.norm_w != nullptr) {
-    float ss[8];
+  float ss[8];
 #pragma unroll
-    for (int b = 0; b < 8; ++b) ss[b] = 0.f;
-    for (int b = 0; b < B; ++b) {
-      const uint4* src = reinterpret_cast<const uint4*>(a.x + (long)b * a.ldx);
-      float s = 0.f;
-      for (int i = threadIdx.x; i < vec_per_row; i += kGemvThreads) {
-        const uint4 v = src[i];
-        const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
+  for (int b = 0; b < 8; ++b) ss[b] = 0.f;
+  for (int b = 0; b < B; ++b) {
+    const uint4* src = reinterpret_cast<const uint4*>(a.x + (long)b * a.ldx);
+    float s = 0.f;
+    for (int i0 = 0; i0 < vec_per_row; i0 += 1024) {
+      uint4 v[4];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float lo = bf16_lo(w4[j]), hi = bf16_hi(w4[j]);
+      for (int j = 0; j < 4; ++j) {  // four independent loads in flight per thread
+        const int i = i0 + (int)threadIdx.x + 256 * j;
+        // activations may have been produced by other CTAs of this very kernel's predecessor: bypass L1
+        v[j] = i < vec_per_row ? __ldcg(src + i) : make_uint4(0, 0, 0, 0);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t w4[4] = {v[j].x, v[j].y, v[j].z, v[j].w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float lo = bf16_lo(w4[q]), hi = bf16_hi(w4[q]);
           s += lo * lo + hi * hi;
         }
       }
-      ss[b] = warp_sum(s);
     }
-    if (lane == 0) {
+    ss[b] = warp_sum(s);
+  }
+  rstd_from_ss(ss, s_ss, s_rstd, K, a.norm_eps);
+}
+
+// Columns [seg * xsc * 256, (seg + 1) * xsc * 256) of every batch row (the whole row when xsc == cpt): thread 0 issues one
+// cp.async.bulk per row, all 256 consumers wait on one mbarrier, and the RMSNorm is applied in place.  Its statistics come
+// from shared memory when the whole row is staged; a segmented row's are already in s_rstd (x_norm_stats_global).
+static __device__ __forceinline__ void stage_x(const GemvTmaParams& p, bf16* xs, float (*s_ss)[8], float* s_rstd, int seg,
+                                               const XPre* pre, uint64_t* xbar, uint32_t& xphase) {
+  const GemvArgs& a = p.a;
+  const int K = a.K, B = a.B;
+  const int col0 = seg * p.xsc * kTCols;
+  const int ncols_pad = min(p.xsc, p.cpt - seg * p.xsc) * kTCols;
+  const int ncols = min(ncols_pad, K - col0);
+  if (threadIdx.x == 0) {
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // earlier accesses of xs are ordered before the async writes
+    mbar_expect_tx(xbar, (uint32_t)B * (uint32_t)ncols * 2u);
+    for (int b = 0; b < B; ++b) bulk_load_1d(xs + (long)b * p.ldxs, a.x + (long)b * a.ldx + col0, (uint32_t)ncols * 2u, xbar);
+  }
+  const int padv = (ncols_pad - ncols) >> 3;  // zero the columns past K (generic writes, disjoint from the copies)
+  for (int i = threadIdx.x; i < B * padv; i += 256) {
+    const int b = i / padv, j = i - b * padv;
+    reinterpret_cast<uint4*>(xs + (long)b * p.ldxs + ncols)[j] = make_uint4(0, 0, 0, 0);
+  }
+  mbar_wait(xbar, xphase);
+  xphase ^= 1;
+  if (a.norm_w != nullptr) {
+    const int nvec = ncols >> 3;  // 16-byte vectors of this segment inside K
+    if (p.xsc == p.cpt) {
+      float ss[8];
 #pragma unroll
-      for (int b = 0; b < 8; ++b) s_ss[warp][b] = ss[b];
-    }
-    __syncthreads();
-    if (threadIdx.x < 8) {
-      float tot = 0.f;
+      for (int b = 0; b < 8; ++b) ss[b] = 0.f;
 #pragma unroll
-      for (int w = 0; w < kGemvWarps; ++w) tot += s_ss[w][threadIdx.x];
-      s_rstd[threadIdx.x] = rsqrtf(tot / (float)K + a.norm_eps);
+      for (int b = 0; b < 8; ++b) {
+        if (b < B) {
+          const uint4* row = reinterpret_cast<const uint4*>(xs + (long)b * p.ldxs);
+          float s = 0.f;
+          for (int i = threadIdx.x; i < nvec; i += 256) {
+            const uint4 v = row[i];
+            const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const float lo = bf16_lo(w4[q]), hi = bf16_hi(w4[q]);
+              s += lo * lo + hi * hi;
+            }
+          }
+          ss[b] = warp_sum(s);
+        }
+      }
+      rstd_from_ss(ss, s_ss, s_rstd, K, a.norm_eps);
     }
-    __syncthreads();
-    for (int b = 0; b < B; ++b) {
-      const float rstd = s_rstd[b];
-      const uint4* src = reinterpret_cast<const uint4*>(a.x + (long)b * a.ldx);
-      const uint4* wsrc = reinterpret_cast<const uint4*>(a.norm_w);
-      uint4* dst = reinterpret_cast<uint4*>(xs + (long)b * p.ldxs);
-      for (int i = threadIdx.x; i < vec_per_row; i += kGemvThreads) {
-        const uint4 v = src[i], w = wsrc[i];
-        const uint32_t v4[4] = {v.x, v.y, v.z, v.w}, w4[4] = {w.x, w.y, w.z, w.w};
+    const uint4* wsrc = reinterpret_cast<const uint4*>(a.norm_w) + (col0 >> 3);
+    // The first stage requests every row's vector before it uses the first.  Re-stages (no XPre) normalise row by row:
+    // they are inlined into the chunk loop, whose registers the batched loads would spill.
+    int i = threadIdx.x;
+    if (pre != nullptr) {
+      const bool use_pre = seg == 0 && pre->have;
+#pragma unroll
+      for (int j = 0; j < 4; ++j, i += 256) {
+        if (i >= nvec) break;
+        const uint4 w = use_pre ? pre->w[j] : __ldg(wsrc + i);
+        const uint32_t w4[4] = {w.x, w.y, w.z, w.w};
+        uint4 v[8];
+#pragma unroll
+        for (int b = 0; b < 8; ++b)
+          if (b < B) v[b] = reinterpret_cast<const uint4*>(xs + (long)b * p.ldxs)[i];
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+          if (b < B) {
+            const float rstd = s_rstd[b];
+            const uint32_t v4[4] = {v[b].x, v[b].y, v[b].z, v[b].w};
+            uint32_t o4[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) o4[q] = rmsnorm_pair(v4[q], rstd, w4[q]);  // HF: weight * (x.float() * rsqrt(var + eps)).to(bf16)
+            reinterpret_cast<uint4*>(xs + (long)b * p.ldxs)[i] = make_uint4(o4[0], o4[1], o4[2], o4[3]);
+          }
+        }
+      }
+    }
+    for (; i < nvec; i += 256) {  // re-stages, and the columns past 8192 of the first stage
+      const uint4 w = __ldg(wsrc + i);
+      const uint32_t w4[4] = {w.x, w.y, w.z, w.w};
+      for (int b = 0; b < B; ++b) {
+        uint4* row = reinterpret_cast<uint4*>(xs + (long)b * p.ldxs);
+        const float rstd = s_rstd[b];
+        const uint4 v = row[i];
+        const uint32_t v4[4] = {v.x, v.y, v.z, v.w};
         uint32_t o4[4];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          // HF: weight * (x.float() * rsqrt(var + eps)).to(bf16)
-          const float lo = round_bf16(bf16_lo(v4[j]) * rstd) * bf16_lo(w4[j]);
-          const float hi = round_bf16(bf16_hi(v4[j]) * rstd) * bf16_hi(w4[j]);
-          o4[j] = pack_bf16(lo, hi);
-        }
-        dst[i] = make_uint4(o4[0], o4[1], o4[2], o4[3]);
+        for (int q = 0; q < 4; ++q) o4[q] = rmsnorm_pair(v4[q], rstd, w4[q]);
+        row[i] = make_uint4(o4[0], o4[1], o4[2], o4[3]);
       }
     }
-  } else {
-    for (int b = 0; b < B; ++b) {
-      const uint4* src = reinterpret_cast<const uint4*>(a.x + (long)b * a.ldx);
-      uint4* dst = reinterpret_cast<uint4*>(xs + (long)b * p.ldxs);
-      for (int i = threadIdx.x; i < vec_per_row; i += kGemvThreads) dst[i] = src[i];
-    }
   }
-  __syncthreads();
+  consumer_bar();
+}
 
-  float acc[RT][4];
+// ---- consumers: pull this CTA's chunks [c0, c1) out of the ring, mma them against xs, finish row groups ----
+static __device__ __forceinline__ void tma_consume(const GemvTmaParams* sp, long c0, long c1, uint8_t* ring,
+                                                   uint64_t* full_bar, uint64_t* empty_bar, float* red, float* fin,
+                                                   bf16* xs, int* s_last, int& stage, uint32_t& phase, float* s_rstd,
+                                                   uint64_t* xbar, uint32_t& xphase) {
+  const GemvTmaParams& p = *sp;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int B = p.a.B, CPT = p.cpt;
+  const int n = (int)(c1 - c0);
+  float acc[kTRT][4];
 #pragma unroll
-  for (int rt = 0; rt < RT; ++rt)
+  for (int rt = 0; rt < kTRT; ++rt)
 #pragma unroll
     for (int q = 0; q < 4; ++q) acc[rt][q] = 0.f;
-
-  const bf16* xrow = xs + (long)g * p.ldxs + t * 8;
+  // fragment addressing inside a 128B-swizzled [32 rows x 64 cols] TMA tile
+  const int tile_j = warp >> 1;                   // which 64-column tile of the chunk this warp reads
+  const int cbase = (warp & 1) * 4;               // first logical 16-byte chunk of this warp's 32 columns
+  const int lrow = lane & 15, lhalf = lane >> 4;  // ldmatrix.x4 lane -> (row, k-half)
   const bool has_x = g < B;
+  const bf16* xrow = xs + (long)g * p.ldxs + warp * 32 + 2 * t;
   int cp_grp = (int)(c0 / CPT), cp_kc = (int)(c0 % CPT);
   int seg_lo = cp_kc;
-  const bf16* xp = xrow + (cp_kc * kGemvWarps + warp) * 32;
-  for (int base = 0; base < n; base += SLOTS) {
+  const int xsc = p.xsc;       // chunks per staged x segment
+  int cur_seg = cp_kc / xsc;   // the caller staged this segment
+  int k_in_seg = cp_kc - cur_seg * xsc;  // tracked incrementally: no division in the chunk loop
+  for (int i = 0; i < n; ++i) {
+    // leave the staged K segment?  (never when the whole row is staged: xsc == CPT)
+    bool restage = false;
+    if (cp_kc == 0) {  // a new row group starts at column 0
+      if (cur_seg != 0) { cur_seg = 0; restage = true; }
+      k_in_seg = 0;
+    } else if (k_in_seg == xsc) {  // ran off the end of the segment inside a row
+      ++cur_seg;
+      k_in_seg = 0;
+      restage = true;
+    }
+    if (restage) {  // all 8 consumer warps take this branch together (same chunk stream)
+      consumer_bar();
+      stage_x(p, xs, nullptr, s_rstd, cur_seg, nullptr, xbar, xphase);  // segmented: the statistics are in s_rstd
+    }
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t tbase = smem_u32(ring + stage * kTStageBytes + tile_j * (kTRows * 128));
+    const bf16* xk = xrow + k_in_seg * kTCols;
 #pragma unroll
-    for (int j = 0; j < SLOTS; ++j) {
-      const int i = base + j;
-      if (i < n) {
-        if (KFULL || cp_kc * kGemvWarps + warp < KB) {
-          uint4 xb = make_uint4(0, 0, 0, 0);
-          if (has_x) xb = *reinterpret_cast<const uint4*>(xp);
-          const uint32_t b1[2] = {xb.x, xb.y};
-          const uint32_t b2[2] = {xb.z, xb.w};
+    for (int ks = 0; ks < 2; ++ks) {
+      uint32_t bfr[2] = {0u, 0u};
+      if (has_x) {
+        bfr[0] = *reinterpret_cast<const uint32_t*>(xk + ks * 16);
+        bfr[1] = *reinterpret_cast<const uint32_t*>(xk + ks * 16 + 8);
+      }
 #pragma unroll
-          for (int rt = 0; rt < RT; ++rt) {
-            const uint4 wa = ring[j][rt][0], wb = ring[j][rt][1];
-            // K permutation shared by A and B: lane t feeds elements t*8+{0,1 | 2,3} to mma #1, {4,5 | 6,7} to #2
-            const uint32_t a1[4] = {wa.x, wb.x, wa.y, wb.y};
-            mma_bf16_16816(acc[rt], a1, b1);
-            const uint32_t a2[4] = {wa.z, wb.z, wa.w, wb.w};
-            mma_bf16_16816(acc[rt], a2, b2);
-          }
-        }
-        xp += 256;
-        if (i + SLOTS < n) load_next(ring[j]);
-        const bool grp_done = (cp_kc == CPT - 1) || (i == n - 1);
-        if (grp_done) {
-#pragma unroll
-          for (int rt = 0; rt < RT; ++rt) {
-            float* r = red + (warp * RT + rt) * 128;
-            r[g * 8 + 2 * t] = acc[rt][0];
-            r[g * 8 + 2 * t + 1] = acc[rt][1];
-            r[(g + 8) * 8 + 2 * t] = acc[rt][2];
-            r[(g + 8) * 8 + 2 * t + 1] = acc[rt][3];
-            acc[rt][0] = acc[rt][1] = acc[rt][2] = acc[rt][3] = 0.f;
-          }
-          gemv_flush(&s_params, red, fin, &s_last, cp_grp, seg_lo, cp_kc);
-        }
-        if (++cp_kc == CPT) { cp_kc = 0; ++cp_grp; xp = xrow + warp * 32; }
-        if (grp_done) seg_lo = cp_kc;
+      for (int rt = 0; rt < kTRT; ++rt) {
+        const int r = rt * 16 + lrow;
+        const int c = cbase + ks * 2 + lhalf;
+        uint32_t af[4];
+        ldmatrix_x4(af, tbase + r * 128 + ((c ^ (r & 7)) << 4));
+        mma_bf16_16816(acc[rt], af, bfr);
       }
     }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+    if (++stage == p.nstages) { stage = 0; phase ^= 1; }
+    const bool grp_done = (cp_kc == CPT - 1) || (i == n - 1);
+    if (grp_done) {
+#pragma unroll
+      for (int rt = 0; rt < kTRT; ++rt) {
+        float* r = red + (warp * kTRT + rt) * 128;
+        r[g * 8 + 2 * t] = acc[rt][0];
+        r[g * 8 + 2 * t + 1] = acc[rt][1];
+        r[(g + 8) * 8 + 2 * t] = acc[rt][2];
+        r[(g + 8) * 8 + 2 * t + 1] = acc[rt][3];
+        acc[rt][0] = acc[rt][1] = acc[rt][2] = acc[rt][3] = 0.f;
+      }
+      gemv_tma_flush(sp, red, fin, s_last, cp_grp, seg_lo, cp_kc);
+    }
+    ++k_in_seg;
+    if (++cp_kc == CPT) { cp_kc = 0; ++cp_grp; }
+    if (grp_done) seg_lo = cp_kc;
   }
 }
 
-static float* g_ws = nullptr;
-static int* g_counters = nullptr;
+// consumer threads (256) of the first ll_red CTAs, after their own rows are pushed: finish the tensor-parallel exchange
+// (GemvArgs::ll_h).  The words polled here are written by the epilogues of this very kernel — on this rank (all CTAs are
+// resident: grid <= SM count) and on the peers.
+static __device__ __forceinline__ void gemv_tail_reduce(const GemvArgs& a) {
+  const unsigned epoch = __ldcg(a.ll_step) * 256u + (unsigned)a.ll_idx + 1u;
+  const int R = a.ll_red;
+  const uint4* base = reinterpret_cast<const uint4*>(a.ll_peer[a.ll_rank]) + ((size_t)(a.ll_idx & 1) * a.ll_n * a.ll_slot_elems) / 2;
+  const long n2 = ((long)a.B * a.ldy) >> 1;  // element pairs of h [B, ldy]
+  const long per = (n2 + R - 1) / R;
+  const long i0 = (long)blockIdx.x * per, i1 = min(n2, i0 + per);
+  uint32_t* h = reinterpret_cast<uint32_t*>(a.ll_h);
+  for (long i = i0 + threadIdx.x; i < i1; i += 256) {
+    float a0 = 0.f, a1 = 0.f;
+    for (int r = 0; r < a.ll_n; ++r) {
+      const uint4* w = base + ((size_t)r * a.ll_slot_elems) / 2 + i;
+      uint4 v;
+      unsigned long long t0 = 0, now;
+      for (;;) {
+        asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(w));
+        if (v.y == epoch && v.w == epoch) break;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+        if (t0 == 0) t0 = now;
+        else if (now - t0 > 20000000000ull) {  // 20 s: a peer died — fail loudly instead of hanging the GPU
+          printf("emu_b200: tensor-parallel exchange %d timed out waiting for rank %d\n", a.ll_idx, r);
+          __trap();
+        }
+      }
+      a0 += __uint_as_float(v.x);  // fixed rank order: bitwise identical on every rank
+      a1 += __uint_as_float(v.z);
+    }
+    const uint32_t hv = __ldcg(h + i);
+    h[i] = pack_bf16(bf16_lo(hv) + round_bf16(a0), bf16_hi(hv) + round_bf16(a1));
+  }
+}
 
-static int ensure_ws() {
-  if (g_ws) return EMU_OK;
-  if (cudaMalloc((void**)&g_ws, (size_t)kWsTiles * kMaxParts * 128 * sizeof(float)) != cudaSuccess) return EMU_ERR_NOMEM;
-  if (cudaMalloc((void**)&g_counters, (size_t)kWsTiles * sizeof(int)) != cudaSuccess) return EMU_ERR_NOMEM;
-  if (cudaMemset(g_counters, 0, (size_t)kWsTiles * sizeof(int)) != cudaSuccess) return EMU_ERR_CUDA;
+__global__ void __launch_bounds__(kTThreads, 2) gemv_tma_kernel(const __grid_constant__ CUtensorMap tmW,
+                                                                const __grid_constant__ GemvTmaParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* ring = smem;                                                   // nstages x 16 KB
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(ring + p.nstages * kTStageBytes);
+  uint64_t* empty_bar = full_bar + kTStages;
+  float* red = reinterpret_cast<float*>(empty_bar + kTStages);            // [8 warps][kTRT*128]
+  float* fin = red + kTW * kTRT * 128;                                    // [kTRT*128]
+  bf16* xs = reinterpret_cast<bf16*>(fin + kTRT * 128);                   // [B][ldxs]
+  __shared__ float s_ss[kTW][8];
+  __shared__ float s_rstd[8];
+  __shared__ int s_last;
+  __shared__ GemvTmaParams s_params;
+  __shared__ __align__(8) uint64_t s_xbar;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // diagnostics: {globaltimer at entry; clock64 at entry, barriers ready, dependency resolved, x staged, first weight chunk
+  // landed (consumer side), own chunks consumed + rows flushed, exit}
+  unsigned long long* dbg = p.a.dbg ? p.a.dbg + (size_t)blockIdx.x * 8 : nullptr;
+  auto clk = [] { unsigned long long t; asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)); return t; };
+  if (dbg && threadIdx.x == 0) {
+    unsigned long long g;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
+    dbg[0] = g;
+    dbg[1] = clk();
+  }
+  const long G = p.geff;  // == gridDim.x for this kernel
+  const long c0 = (long)blockIdx.x * p.total / G, c1 = ((long)blockIdx.x + 1) * p.total / G;
+  // the launch parameters are re-read from shared memory by the flush routine: copy them with the whole CTA (one word
+  // per thread) instead of one thread walking ~350 bytes
+  for (int i = threadIdx.x; i < (int)(sizeof(GemvTmaParams) / 4); i += blockDim.x)
+    reinterpret_cast<uint32_t*>(&s_params)[i] = reinterpret_cast<const uint32_t*>(&p)[i];
+  if (threadIdx.x == 0) tma_prefetch_desc(&tmW);
+  if (threadIdx.x < kTStages) {  // one barrier pair per thread: a single thread walking 20 inits costs ~0.3 us per launch
+    mbar_init(&full_bar[threadIdx.x], 1);
+    mbar_init(&empty_bar[threadIdx.x], kTW);
+    mbar_fence_init();
+  } else if (threadIdx.x == 32) {
+    mbar_init(&s_xbar, 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  if (dbg && threadIdx.x == 0) dbg[2] = clk();
+  if (p.a.pdl) pdl_launch_dependents();
+  int stage = 0;
+  uint32_t phase = 0;
+  if (warp == kTW) {
+    // producer: weights do not depend on the previous kernel, so the ring fills before griddepcontrol.wait resolves
+    if (lane == 0) tma_produce(&tmW, p.cpt, c0, c1, ring, full_bar, empty_bar, p.nstages, stage, phase);
+    return;
+  }
+  XPre pre;
+  tma_prefetch_norm_w(p, pre);  // weights of the fused RMSNorm: independent of the predecessor, fetched while it drains
+  if (p.a.pdl) pdl_wait();
+  if (dbg && threadIdx.x == 0) dbg[3] = clk();
+  if (p.a.norm_w != nullptr && p.xsc < p.cpt) x_norm_stats_global(p, s_ss, s_rstd);
+  uint32_t xphase = 0;
+  stage_x(p, xs, s_ss, s_rstd, (int)(c0 % p.cpt) / p.xsc, &pre, &s_xbar, xphase);
+  if (dbg && threadIdx.x == 0) {
+    dbg[4] = clk();
+    if (c0 < c1) mbar_wait(&full_bar[0], 0);  // (diagnostic only) when did the first chunk land?
+    dbg[5] = clk();
+  }
+  tma_consume(&s_params, c0, c1, ring, full_bar, empty_bar, red, fin, xs, &s_last, stage, phase, s_rstd, &s_xbar, xphase);
+  if (dbg && threadIdx.x == 0) dbg[6] = clk();
+  if (p.a.ll_n > 0 && p.a.ll_h != nullptr && (int)blockIdx.x < p.a.ll_red) gemv_tail_reduce(p.a);
+  if (dbg && threadIdx.x == 0) dbg[7] = clk();
+}
+
+static float* g_tws = nullptr;
+static int* g_tcounters = nullptr;
+
+int gemv_init() {
+  if (g_tws) return EMU_OK;
+  if (cudaMalloc((void**)&g_tws, (size_t)kTWsGroups * kTMaxParts * kTRT * 128 * sizeof(float)) != cudaSuccess) return EMU_ERR_NOMEM;
+  if (cudaMalloc((void**)&g_tcounters, (size_t)kTWsGroups * sizeof(int)) != cudaSuccess) return EMU_ERR_NOMEM;
+  if (cudaMemset(g_tcounters, 0, (size_t)kTWsGroups * sizeof(int)) != cudaSuccess) return EMU_ERR_CUDA;
+  if (cudaFuncSetAttribute(gemv_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
+    return EMU_ERR_CUDA;
+  // ask for the largest shared-memory carve-out so that this kernel's CTA and its PDL successor's CTA (2 x ~105 KB)
+  // can be resident on one SM at the same time
+  if (cudaFuncSetAttribute(gemv_tma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) !=
+      cudaSuccess)
+    return EMU_ERR_CUDA;
   return EMU_OK;
 }
-int gemv_init() {
-  int rc = ensure_ws();
-  if (rc) return rc;
-  return gemv_tma_init();
-}
 
-template <int RT, bool KFULL>
-static int launch_gemv(const GemvParams& p, int grid, size_t smem, cudaStream_t st) {
-  static size_t cur_max = 0;
-  if (smem > cur_max) {
-    if (cudaFuncSetAttribute(gemv_kernel<RT, KFULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-      return EMU_ERR_CUDA;
-    cur_max = smem;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(kGemvThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = p.a.pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, gemv_kernel<RT, KFULL>, p) == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
-}
-
-// dispatcher: TMA-fed kernel whenever the shape fits, register-ring kernel otherwise (EMU_GEMV=reg forces the latter)
 int gemv_bf16(const GemvArgs& a, cudaStream_t st) {
+  // everything the kernel cannot take is refused here, before any CUDA call
   if (a.B < 1 || a.B > 8 || a.N < 1 || a.K < 32 || (a.K % 32) || (a.ldx % 8)) return EMU_ERR_INVALID;
   if ((a.mode == EPI_SWIGLU || a.mode == GEMV_ROPE_QKV) && (a.N % 16)) return EMU_ERR_INVALID;
-  static int force_reg = -1;
-  if (force_reg < 0) {
-    const char* v = getenv("EMU_GEMV");
-    force_reg = (v && v[0] == 'r') ? 1 : 0;
+  // W is read by TMA and x by bulk copies: both need 16-byte aligned rows (ldx % 8 == 0 carries x's alignment to every row)
+  if ((reinterpret_cast<uintptr_t>(a.W) | reinterpret_cast<uintptr_t>(a.x)) & 15) return EMU_ERR_INVALID;
+  const int groups = (a.N + kTRows - 1) / kTRows;
+  if (groups > kTWsGroups) return EMU_ERR_INVALID;  // the stream-K workspace holds N <= 262144 rows
+  if (a.ll_n > 0 && a.ll_h && (a.ll_red < 1 || (a.ldy & 1))) return EMU_ERR_INVALID;
+  if (!g_tws) {  // first use must happen outside stream capture (the engine calls gemv_init() at create)
+    int rc = gemv_init();
+    if (rc) return rc;
   }
-  if (!force_reg) {
-    const int rc = gemv_tma_bf16(a, st);
-    if (rc != EMU_ERR_UNSUPPORTED) return rc;
-  }
-  if (a.ll_n > 0) return EMU_ERR_UNSUPPORTED;  // the fused exchange epilogue exists in the TMA kernel only
-  return gemv_reg_bf16(a, st);
-}
-
-int gemv_reg_bf16(const GemvArgs& a, cudaStream_t st) {
-  if (a.B < 1 || a.B > 8 || a.N < 1 || a.K < 32 || (a.K % 32) || (a.ldx % 8)) return EMU_ERR_INVALID;
-  if ((a.mode == EPI_SWIGLU || a.mode == GEMV_ROPE_QKV) && (a.N % 16)) return EMU_ERR_INVALID;
-  const int tiles = (a.N + 15) / 16;
-  if (tiles > kWsTiles) return EMU_ERR_UNSUPPORTED;
-  int rc = ensure_ws();  // NOTE: first use must happen outside stream capture (the engine calls gemv_init())
-  if (rc) return rc;
-  GemvParams p;
+  GemvTmaParams p;
   p.a = a;
-  p.ldxs = a.K + 32;  // row stride = 64 B (mod 128 B): conflict-free B-fragment reads
-  p.ws = g_ws;
-  p.counters = g_counters;
-  const int KB = a.K / 32;
-  p.cpt = (KB + kGemvWarps - 1) / kGemvWarps;
-  const size_t xs_bytes = (size_t)a.B * p.ldxs * sizeof(bf16);
-  p.red_off = (int)((xs_bytes + 15) & ~size_t(15));
-  // tallest row group that still leaves >= 9 chunks per CTA: the RT=4 inner loop is ~4x leaner in instructions
-  // per byte than RT=1, which outweighs up to ~10 % chunk-count imbalance (measured on the 6656x6656 o_proj)
-  const long slots = 2L * kNumSMs;
-  int rt = 1;
-  if ((long)((tiles + 3) / 4) * p.cpt >= 9 * slots) rt = 4;
-  else if ((long)((tiles + 1) / 2) * p.cpt >= 9 * slots) rt = 2;
-  const size_t smem = p.red_off + (size_t)(kGemvWarps + 1) * rt * 128 * sizeof(float);
-  if (smem > 220 * 1024) return EMU_ERR_UNSUPPORTED;
-  const int occ = smem > 100 * 1024 ? 1 : 2;
-  p.rt = rt;
-  const int groups = (tiles + rt - 1) / rt;
-  p.total = (long)groups * p.cpt;
-  long grid = (long)kNumSMs * occ;
-  if (grid > p.total) grid = p.total;
-  // a row group may be shared by at most kMaxParts CTAs: keep every CTA's share >= cpt / (kMaxParts - 3)
-  const long max_grid = (long)groups * (kMaxParts - 3);
-  if (grid > max_grid) grid = max_grid;
-  const bool kfull = (a.K % 256) == 0;
-  if (kfull) {
-    if (rt == 4) return launch_gemv<4, true>(p, (int)grid, smem, st);
-    if (rt == 2) return launch_gemv<2, true>(p, (int)grid, smem, st);
-    return launch_gemv<1, true>(p, (int)grid, smem, st);
+  p.kpad = (a.K + kTCols - 1) / kTCols * kTCols;
+  p.cpt = p.kpad / kTCols;
+  p.xsc = p.cpt;
+  p.ldxs = p.kpad + 8;  // row stride = 16 B (mod 128 B): the 8 batch rows hit distinct bank groups
+  // batch x K too large to keep all of x in shared memory next to a deep ring (5 beams x 17920 = 179 KB): stage x in K
+  // segments of <= 88 KB instead, re-staged as the chunk stream crosses them.  With B <= 8 a segment holds >= 21 chunks.
+  const size_t budget = 88 * 1024;
+  if ((size_t)a.B * p.ldxs * 2 > budget) {
+    p.xsc = (int)((budget / ((size_t)a.B * 2) - 8) / kTCols);
+    p.ldxs = p.xsc * kTCols + 8;
   }
-  if (rt == 4) return launch_gemv<4, false>(p, (int)grid, smem, st);
-  if (rt == 2) return launch_gemv<2, false>(p, (int)grid, smem, st);
-  return launch_gemv<1, false>(p, (int)grid, smem, st);
+  p.total = (long)groups * p.cpt;
+  p.ws = g_tws;
+  p.counters = g_tcounters;
+  const size_t xs_bytes = (size_t)a.B * p.ldxs * 2;
+  // the ring buffers are carved for kTStages; 8 stages = 128 KB in flight per SM, and a CTA with a wide x uses fewer so
+  // that this kernel (<= ~110 KB) and its PDL successor still fit one SM together.  x is at most 88 KB, so even the
+  // 3-stage floor fits the 200 KB the kernel is allowed.
+  p.nstages = 8;
+  size_t smem;
+  for (;;) {  // shrink the ring until the CTA fits (wide x at batch > 1)
+    smem = 1024 + (size_t)p.nstages * kTStageBytes + 2 * kTStages * 8 + (size_t)(kTW + 1) * kTRT * 128 * 4 + xs_bytes + 64;
+    if (smem <= 200 * 1024 || p.nstages <= 3) break;
+    --p.nstages;
+  }
+  long grid = kNumSMs;
+  if (grid > p.total) grid = p.total;
+  const long max_grid = (long)groups * (kTMaxParts - 3);  // a row group is shared by at most kTMaxParts CTAs
+  if (grid > max_grid) grid = max_grid;
+  p.geff = (int)grid;
+  if (p.a.ll_n > 0 && p.a.ll_h && p.a.ll_red > (int)grid) p.a.ll_red = (int)grid;
+  CUtensorMap tm;
+  if (int rc = make_tmap_2d(&tm, a.W, a.N, a.K, a.K, kTRows)) return rc;
+  return launch_kernel(gemv_tma_kernel, dim3((unsigned)grid), dim3(kTThreads), smem, st, a.pdl, tm, p);
 }
 
 }  // namespace emu

@@ -171,6 +171,7 @@ int emu_op_gemm_skinny(const void* X, int ldx, const void* W, int ldw, int B, in
                        int epi_mode, void* C, int ldc, int out_fp32, emu_stream_t s);
 int emu_op_conv3x3(const void* x_nhwc, int NB, int H, int W, int Cin, const void* w_k /*[Cout, 9*Cin]*/, int Cout,
                    const void* bias, const void* residual, void* y_nhwc, emu_stream_t s);
+/* B <= 8, K % 32 == 0, ldx % 8 == 0, W and x 16-byte aligned; otherwise EMU_ERR_INVALID. */
 int emu_op_gemv(const void* W, int N, int K, const void* x, int ldx, int B, const void* norm_w, float eps,
                 int mode, const void* bias, const void* residual, int ldr, void* y, int ldy, int out_fp32, int pdl,
                 emu_stream_t s);

@@ -161,3 +161,15 @@ def test_null_arguments_are_refused_not_dereferenced(lib):
             fn.argtypes = saved
         assert rc == -1, (name, rc)
     assert lib.emu_llm_cur_len(None) == -1
+
+
+@pytest.mark.parametrize("w_off,x_off", [(8, 0), (0, 8), (2, 2)])
+def test_gemv_refuses_misaligned_operands(lib, w_off, x_off):
+    """W is read by TMA and x by bulk copies, so both must be 16-byte aligned: anything else is EMU_ERR_INVALID, decided before
+    any pointer is dereferenced or any CUDA call is made (the addresses below are never touched)."""
+    P = ctypes.c_void_p
+    base = 0x10000000
+    W, x, y = P(base + w_off), P(base + 0x100000 + x_off), P(base + 0x200000)
+    N = K = 64
+    rc = lib.emu_op_gemv(W, N, K, x, K, 1, None, ctypes.c_float(1e-6), 0, None, None, 0, y, N, 0, 0, None)
+    assert rc == -1

@@ -171,17 +171,22 @@ def test_gemv_plain(cuda, N, K, B):
 
 
 def test_gemv_segmented_x_with_norm(cuda):
-    """batch x K too large for shared memory: x is staged in K segments (fused RMSNorm statistics span all segments)"""
+    """batch x K too large for shared memory: x is staged in K segments (fused RMSNorm statistics span all segments).
+    K = 5664 pads to 23 chunks of 256 staged as 21 + 2, so the last segment is ragged and zero filled past K."""
     from emu_b200 import _lib
-    N, K, B = 2048, 6656, 8
-    W, x, nw = _rand((N, K), 16, 0.05), _rand((B, K), 17), (1 + 0.1 * _rand((K,), 18).float()).to(torch.bfloat16)
-    xn = O.rms_norm(x, nw, 1e-6)
-    ref = O.op_linear(xn, W)
-    assert O.rel_err(_lib.op_gemv(W.cuda(), x.cuda(), norm_w=nw.cuda(), out_fp32=True).cpu(), ref) < TOL_F32
-    g, u = O.op_linear(xn, W[0::2]), O.op_linear(xn, W[1::2])
+    B = 8
     bf = lambda t: t.to(torch.bfloat16)
-    assert O.rel_err(_lib.op_gemv(W.cuda(), x.cuda(), norm_w=nw.cuda(), mode=_lib.EPI_SWIGLU).cpu(),
-                     torch.nn.functional.silu(bf(g)) * bf(u)) < TOL_BF16
+    for N, K in [(2048, 6656), (1024, 5664)]:
+        W, x, nw = _rand((N, K), 16, 0.05), _rand((B, K), 17), (1 + 0.1 * _rand((K,), 18).float()).to(torch.bfloat16)
+        r = _rand((B, N), 19)
+        xn = O.rms_norm(x, nw, 1e-6)
+        ref = O.op_linear(xn, W)
+        assert O.rel_err(_lib.op_gemv(W.cuda(), x.cuda(), norm_w=nw.cuda(), out_fp32=True).cpu(), ref) < TOL_F32, (N, K)
+        assert O.rel_err(_lib.op_gemv(W.cuda(), x.cuda(), norm_w=nw.cuda(), residual=r.cuda()).cpu(),
+                         bf(ref).float() + r.float()) < TOL_BF16, (N, K)
+        g, u = O.op_linear(xn, W[0::2]), O.op_linear(xn, W[1::2])
+        assert O.rel_err(_lib.op_gemv(W.cuda(), x.cuda(), norm_w=nw.cuda(), mode=_lib.EPI_SWIGLU).cpu(),
+                         torch.nn.functional.silu(bf(g)) * bf(u)) < TOL_BF16, (N, K)
 
 
 def test_gemv_fused(cuda):

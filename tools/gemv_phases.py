@@ -16,7 +16,7 @@ def main():
     lib = _lib.load()
     B = int(sys.argv[1]) if len(sys.argv) > 1 else 1       # batch rows (5 = the reference's default beam search)
     tps = [int(v) for v in sys.argv[2].split(",")] if len(sys.argv) > 2 else [1, 2, 8]
-    print("batch rows = %d, EMU_GEMV_XBULK=%s" % (B, os.environ.get("EMU_GEMV_XBULK", "1")))
+    print("batch rows = %d" % B)
     for tp in tps:
         Hl = (52 + tp - 1) // tp * 128
         Fl = F // tp

@@ -36,7 +36,7 @@ def time_gemv(N, K, B, mode=0, norm=False, residual=False, iters=40, pdl=False):
 def main():
     H, F, V = 6656, 17920, 32272
     out = {}
-    for B in (1, 5):
+    for B in (1, 5, 8):
         for name, (N, K, mode, norm, res) in {
             "qkv": (3 * H, H, 0, True, False), "o": (H, H, 0, False, True), "gate_up": (2 * F, H, 2, True, False),
             "down": (H, F, 0, False, True), "lm_head": (V, H, 0, True, False)}.items():
@@ -86,3 +86,4 @@ def chain_bench(B=1, layers=8, iters=5):
 if __name__ == "__main__" and os.environ.get("EMU_CHAIN", "1") == "1":
     chain_bench(1)
     chain_bench(5)
+    chain_bench(8)
