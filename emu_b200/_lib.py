@@ -15,7 +15,7 @@ EMU_OK = 0
 ERRORS = {-1: "EMU_ERR_INVALID", -2: "EMU_ERR_CUDA", -3: "EMU_ERR_NOMEM", -4: "EMU_ERR_STATE",
           -5: "EMU_ERR_UNSUPPORTED", -6: "EMU_ERR_NCCL"}
 DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2
-EPI_NONE, EPI_GELU, EPI_SWIGLU, EPI_GEGLU, EPI_RELU = 0, 1, 2, 3, 4
+EPI_NONE, EPI_GELU, EPI_SWIGLU, EPI_GEGLU, EPI_RELU, EPI_QUICK_GELU = 0, 1, 2, 3, 4, 5
 
 
 class EmuError(RuntimeError):
@@ -55,6 +55,14 @@ class EmuVAEConfig(C.Structure):
     ]
 
 
+class EmuSafetyConfig(C.Structure):
+    _fields_ = [
+        ("image_size", C.c_int), ("patch_size", C.c_int), ("width", C.c_int), ("layers", C.c_int), ("heads", C.c_int),
+        ("mlp", C.c_int), ("proj_dim", C.c_int), ("n_special", C.c_int), ("n_concepts", C.c_int), ("ln_eps", C.c_float),
+        ("resize_shortest_edge", C.c_int), ("crop_size", C.c_int), ("image_mean", C.c_float * 3), ("image_std", C.c_float * 3),
+    ]
+
+
 # every symbol declared in include/emu_b200.h (tests/test_abi.py checks the header against this list)
 SYMBOLS = [
     "emu_beam_topk", "emu_beam_step", "emu_sample_tokens", "emu_image_to_uint8", "emu_preprocess_image", "emu_engine_create", "emu_engine_destroy", "emu_last_error", "emu_nccl_unique_id", "emu_tp_head_range", "emu_engine_load_tensor",
@@ -65,6 +73,8 @@ SYMBOLS = [
     "emu_debug_gemm_phases", "emu_debug_gemv_phases",
     "emu_version",
 ]
+# ... and in include/emu_b200_safety.h (the safety checker)
+SAFETY_SYMBOLS = ["emu_safety_configure", "emu_safety_check", "emu_safety_embed", "emu_preprocess_clip"]
 
 _lib = None
 
@@ -266,6 +276,30 @@ class Engine:
         check(self.lib.emu_vae_decode(self.h, _ptr(latents), B, h, w, _ptr(out), _stream()), self.h)
         return out
 
+    # ---- safety checker ----
+    def safety_configure(self, scfg: "EmuSafetyConfig"):
+        self.scfg = scfg
+        check(self.lib.emu_safety_configure(self.h, C.byref(scfg)), self.h)
+
+    def safety_check(self, images_u8, scores=False):
+        """images [B, H, W, 3] uint8 CUDA (flagged ones are zeroed in place) -> flags int32 [B] (and the scores
+        fp32 [B, n_special + n_concepts] with scores=True), all on the device"""
+        assert images_u8.dtype == torch.uint8 and images_u8.dim() == 4 and images_u8.shape[3] == 3 and images_u8.is_cuda
+        assert images_u8.is_contiguous(), "the check blacks out flagged images in place: pass a contiguous tensor"
+        B, H, W, _ = images_u8.shape
+        flags = torch.empty(B, dtype=torch.int32, device=images_u8.device)
+        sc = (torch.empty(B, self.scfg.n_special + self.scfg.n_concepts, dtype=torch.float32, device=images_u8.device)
+              if scores else None)
+        check(self.lib.emu_safety_check(self.h, _ptr(images_u8), B, H, W, _ptr(flags), _ptr(sc), _stream()), self.h)
+        return (flags, sc) if scores else flags
+
+    def safety_embed(self, pixel_values):
+        """pixel_values [B, 3, S, S] (CLIP-normalised) -> image_embeds [B, proj_dim] bf16"""
+        pv = pixel_values.to(torch.bfloat16).contiguous()
+        out = torch.empty(pv.shape[0], self.scfg.proj_dim, dtype=torch.bfloat16, device=pv.device)
+        check(self.lib.emu_safety_embed(self.h, _ptr(pv), pv.shape[0], _ptr(out), _stream()), self.h)
+        return out
+
     # ---- diffusion ----
     def unet_configure(self, ucfg: "EmuUNetConfig"):
         self.ucfg = ucfg
@@ -420,6 +454,23 @@ def op_preprocess_image(img_u8_hwc, out_h, out_w, mean, std, dtype=torch.float32
     s3 = (C.c_float * 3)(*[float(v) for v in std])
     code = {torch.float32: DTYPE_F32, torch.bfloat16: DTYPE_BF16}[dtype]
     check(lib.emu_preprocess_image(_ptr(img), H, W, out_h, out_w, m3, s3, _ptr(out), code, _stream()))
+    return out
+
+
+def op_preprocess_clip(images_u8_bhwc, size=224, crop=224, mean=(0.48145466, 0.4578275, 0.40821073),
+                       std=(0.26862954, 0.26130258, 0.27577711), dtype=torch.bfloat16):
+    """[B, H, W, 3] uint8 CUDA -> [B, 3, crop, crop]: CLIPImageProcessor (shortest-edge bicubic resize, centre crop, rescale,
+    normalise), bit-exact with transformers' CLIPImageProcessorPil."""
+    require_cuda()
+    x = images_u8_bhwc
+    assert x.dtype == torch.uint8 and x.dim() == 4 and x.shape[3] == 3 and x.is_cuda
+    x = x.contiguous()
+    B, H, W, _ = x.shape
+    out = torch.empty(B, 3, crop, crop, dtype=dtype, device=x.device)
+    m3 = (C.c_float * 3)(*[float(v) for v in mean])
+    s3 = (C.c_float * 3)(*[float(v) for v in std])
+    code = {torch.float32: DTYPE_F32, torch.bfloat16: DTYPE_BF16}[dtype]
+    check(load().emu_preprocess_clip(_ptr(x), B, H, W, int(size), int(crop), m3, s3, _ptr(out), code, _stream()))
     return out
 
 

@@ -25,7 +25,7 @@ def sources():
 
 def _digest():
     h = hashlib.sha256()
-    for f in sorted(os.listdir(CSRC)) + ["../../include/emu_b200.h"]:
+    for f in sorted(os.listdir(CSRC)) + ["../../include/emu_b200.h", "../../include/emu_b200_safety.h"]:
         p = os.path.join(CSRC, f)
         if os.path.isfile(p):
             h.update(f.encode())

@@ -100,6 +100,8 @@ __device__ __forceinline__ float erf_fast(float x) {
 }
 __device__ __forceinline__ float gelu_erf_fast(float x) { return 0.5f * x * (1.f + erf_fast(x * 0.70710678118654752440f)); }
 __device__ __forceinline__ float silu(float x) { return x / (1.f + __expf(-x)); }
+// torch.sigmoid's fp32 formula, 1 / (1 + exp(-x)), with the accurate expf and an IEEE division
+__device__ __forceinline__ float sigmoid_f(float x) { return __fdiv_rn(1.f, 1.f + expf(-x)); }
 __device__ __forceinline__ float silu_fast(float x) { return x * rcp_approx(1.f + ex2_approx_ftz(-x * 1.4426950408889634f)); }
 
 // streaming 16-byte global load that does not pollute L1 (weights are read exactly once)

@@ -376,6 +376,7 @@ extern "C" void emu_engine_destroy(EmuEngine* e) {
   if (e->unet) unet_destroy(e->unet);
   if (e->vae) vae_destroy(e->vae);
   if (e->cformer) cformer_destroy(e->cformer);
+  if (e->safety) safety_destroy(e->safety);
   for (void* p : e->owned) cudaFree(p);
   tp_exchange_teardown(e);
   if (e->nccl_comm && g_nccl.CommDestroy) g_nccl.CommDestroy(e->nccl_comm);
@@ -577,6 +578,7 @@ extern "C" int emu_engine_load_tensor(EmuEngine* e, const char* state_dict_key, 
   } else if (starts_with(key, "unet.")) rc = unet_load_tensor(e, key.substr(5), dsrc, shape, ndim, st);
   else if (starts_with(key, "vae.")) rc = vae_load_tensor(e, key.substr(4), dsrc, shape, ndim, st);
   else if (starts_with(key, "cformer.")) rc = cformer_load_tensor(e, key.substr(8), dsrc, shape, ndim, st);
+  else if (starts_with(key, "safety_checker.")) rc = safety_load_tensor(e, key.substr(15), dsrc, shape, ndim, st);
   else rc = e->fail(EMU_ERR_INVALID, "unknown state-dict key " + key);
   if (temp) {
     cudaStreamSynchronize(st);

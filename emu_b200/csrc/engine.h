@@ -40,6 +40,7 @@ struct DevBuf {
 struct UNetModel;  // unet.cu
 struct VaeModel;   // vae.cu
 struct CFormerModel;  // cformer.cu
+struct SafetyModel;   // safety.cu
 
 }  // namespace emu
 
@@ -102,6 +103,7 @@ struct EmuEngine {
   emu::UNetModel* unet = nullptr;
   emu::VaeModel* vae = nullptr;
   emu::CFormerModel* cformer = nullptr;
+  emu::SafetyModel* safety = nullptr;
 
   // helpers
   int fail(int code, const std::string& msg) {
@@ -125,6 +127,20 @@ int tp_ll_prepare(EmuEngine* e, GemvArgs& g, int idx);
 int tp_ll_reduce(EmuEngine* e, bf16* h, long n_elem, int idx, int pdl, cudaStream_t st);
 unsigned* tp_step_counter(EmuEngine* e);
 
+// preprocess.cu: CLIPImageProcessor (shortest-edge bicubic resize + centre crop) restricted to the crop window
+struct ClipPlan {
+  int H = 0, W = 0, rh = 0, rw = 0, top = 0, left = 0, crop = 0;
+  bool need_h = false, need_v = false;
+  int row0 = 0, rows = 0;  // input rows the horizontal pass produces
+  int ksh = 0, ksv = 0;
+  std::vector<int> tab;    // [bounds_h | coeffs_h | bounds_v | coeffs_v] of the window
+  size_t off_kh = 0, off_bv = 0, off_kv = 0;
+};
+int clip_plan(int H, int W, int size, int crop, ClipPlan* p);
+size_t clip_tmp_bytes(const ClipPlan& p, int B);
+int clip_launch(const ClipPlan& p, const int* d_tab, const uint8_t* in, int B, uint8_t* tmp, void* out, const float* mean3,
+                const float* std3, int out_bf16, cudaStream_t st);
+
 // sub-model entry points
 int unet_load_tensor(EmuEngine* e, const std::string& key, const bf16* src, const int64_t* shape, int ndim, cudaStream_t st);
 int vae_load_tensor(EmuEngine* e, const std::string& key, const bf16* src, const int64_t* shape, int ndim, cudaStream_t st);
@@ -132,4 +148,6 @@ int cformer_load_tensor(EmuEngine* e, const std::string& key, const bf16* src, c
 void unet_destroy(UNetModel*);
 void vae_destroy(VaeModel*);
 void cformer_destroy(CFormerModel*);
+int safety_load_tensor(EmuEngine* e, const std::string& key, const bf16* src, const int64_t* shape, int ndim, cudaStream_t st);
+void safety_destroy(SafetyModel*);
 }  // namespace emu

@@ -6,7 +6,7 @@
 // the UNet/VAE 3x3 convolutions (diffusers UNet2DConditionModel, called from Emu2/emu/diffusion.py:136-141).
 //
 // 128 x BN output tiles, persistent CTAs (one per SM), a TMA producer feeding a ring of 128B-swizzled stages and two
-// consumer warpgroups that run wgmma (fp32 accumulators in registers) and the fused epilogue — bias / GELU / residual /
+// consumer warpgroups that run wgmma (fp32 accumulators in registers) and the fused epilogue — bias / GELU / quick GELU / residual /
 // SwiGLU / GEGLU.  bf16 outputs are STAGED: the tile is assembled in shared memory as 64B-swizzled [rows x 32 columns]
 // slabs and leaves with TMA stores; a residual tile arrives the same way (TMA load issued before the tile's main loop
 // ends).  fp32 outputs, unaligned or very wide (> 192 columns) tiles store straight from registers.
@@ -120,10 +120,15 @@ __device__ __forceinline__ uint32_t slab_off(int row, int c) {
 // CL = thread-block cluster size along M (1 or 2).  With CL == 2 the two CTAs of a cluster work on vertically adjacent
 // output tiles (same weight columns): each loads HALF of the W tile and TMA-multicasts it into both CTAs' shared memory,
 // so W crosses the L2->SM fabric once per pair; a stage is released in both CTAs once both have consumed it.
-template <int BN, int CL>
+// CLF = CL, or CL | kQuickGeluKernel for the instantiations with the quick-GELU epilogue (CLIP MLP): that epilogue is a
+// compile-time choice, so the kernels every other model runs carry no trace of it.
+constexpr int kQuickGeluKernel = 16;
+template <int BN, int CLF>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
+  constexpr int CL = CLF & (kQuickGeluKernel - 1);
+  constexpr bool QG = (CLF & kQuickGeluKernel) != 0;
   constexpr int kStages = GemmSmem<BN>::kStages;
   constexpr int kStageBytes = GemmSmem<BN>::kStageBytes;
 
@@ -340,7 +345,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
             continue;
           }
-          if (p.epi == EPI_GELU) {
+          if (QG) {
+            // transformers QuickGELUActivation on the bf16 Linear output, x * sigmoid(1.702 * x), with the rounding points
+            // of its bf16 eager run: Linear -> bf16, 1.702 * x -> bf16, sigmoid -> bf16, product -> bf16 (at the store)
+            round_bf16x2(f0, f1);
+            f0 *= round_bf16(sigmoid_f(round_bf16(1.702f * f0)));
+            f1 *= round_bf16(sigmoid_f(round_bf16(1.702f * f1)));
+          } else if (p.epi == EPI_GELU) {
             round_bf16x2(f0, f1);
             f0 = gelu_erf_fast(f0);
             f1 = gelu_erf_fast(f1);
@@ -505,13 +516,15 @@ int make_tmap_bnhd(CUtensorMap* out, const void* base, int D, long N, int H, int
   return r == CUDA_SUCCESS ? EMU_OK : EMU_ERR_CUDA;
 }
 
-template <int BN, int CL>
+template <int BN, int CL, bool QG = false>
 static int launch_gemm_cl(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
                           const GemmParams& p, cudaStream_t st) {
+  static_assert(!QG || CL == 1, "the quick-GELU kernels are built without clusters");
+  auto kern = gemm_tc_kernel<BN, QG ? (CL | kQuickGeluKernel) : CL>;
   static bool attr_set = false;
   static int max_ctas = kNumSMs;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(gemm_tc_kernel<BN, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmSmem<BN>::kBytes) !=
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmSmem<BN>::kBytes) !=
         cudaSuccess)
       return EMU_ERR_CUDA;
     if (CL > 1) {
@@ -553,7 +566,7 @@ static int launch_gemm_cl(const CUtensorMap& tmA, const CUtensorMap& tmB, const 
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  return cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL>, tmA, tmB, tmC, tmR, p) == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
+  return cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmC, tmR, p) == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
 // Cluster mode (W tile TMA-multicast over a 2-CTA cluster): halves the W traffic into shared memory at the price of
@@ -600,7 +613,7 @@ static int pick_bn(int M, int N, int K, const GemmEpilogue& e) {
   static const int cand[] = {256, 224, 192, 160, 128, 96, 64};
   const long tm = (M + BM - 1) / BM;
   const long kb = (K + BK - 1) / BK;
-  const bool act = e.mode == EPI_GELU || e.mode == EPI_SWIGLU || e.mode == EPI_GEGLU;
+  const bool act = e.mode == EPI_GELU || e.mode == EPI_SWIGLU || e.mode == EPI_GEGLU || e.mode == EPI_QUICK_GELU;
   int best = 128;
   double best_cost = 1e30;
   for (int bn : cand) {
@@ -667,13 +680,14 @@ int gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int 
     return EMU_ERR_INVALID;
   const bool pair = e.mode == EPI_SWIGLU || e.mode == EPI_GEGLU;
   if (pair && (N & 1)) return EMU_ERR_INVALID;
+  const bool qg = e.mode == EPI_QUICK_GELU;
   GemmParams p{};
   p.M = M; p.N = N; p.K = K;
   p.C = e.C; p.ldc = e.ldc; p.bias = e.bias; p.residual = e.residual; p.ldr = e.ldr;
   p.bias2 = e.bias2; p.bias2_rows = e.bias2_rows > 0 ? e.bias2_rows : 1;
   p.epi = e.mode; p.out_fp32 = e.out_fp32; p.conv = 0; p.pdl = g_pdl_chain; p.dbg = e.dbg;
   const int bn = (e.force_bn & 1023) ? (e.force_bn & 1023) : pick_bn(M, N, K, e);
-  const bool cl = use_cluster(M, e.force_bn, false);
+  const bool cl = !qg && use_cluster(M, e.force_bn, false);
   CUtensorMap tmA, tmB, tmC, tmR;
   int rc = make_tmap_2d(&tmA, A, M, K, lda, BM);
   if (rc) return rc;
@@ -683,6 +697,7 @@ int gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int 
   if (rc) return rc;
   return dispatch_bn(bn, [&](auto w) {
     constexpr int kBN = decltype(w)::value;
+    if (qg) return launch_gemm_cl<kBN, 1, true>(tmA, tmB, tmC, tmR, p, st);
     return cl ? launch_gemm_cl<kBN, 2>(tmA, tmB, tmC, tmR, p, st) : launch_gemm_cl<kBN, 1>(tmA, tmB, tmC, tmR, p, st);
   });
 }
@@ -690,7 +705,7 @@ int gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int 
 // 3x3 stride-1 pad-1 convolution on NHWC bf16 as an implicit GEMM. Wk is [Cout, 9*Cin] with k = (r*3+s)*Cin + c.
 int conv3x3_bf16(const bf16* X, int NB, int H, int W, int Cin, const bf16* Wk, int Cout, const GemmEpilogue& e,
                  cudaStream_t st) {
-  if (Cin % 8) return EMU_ERR_INVALID;
+  if (Cin % 8 || e.mode == EPI_QUICK_GELU) return EMU_ERR_INVALID;  // quick GELU: Linear layers only
   int tw = W >= 128 ? 128 : W;  // tile = th x tw pixels, th*tw = 128
   if (128 % tw) return EMU_ERR_UNSUPPORTED;
   int th = 128 / tw;

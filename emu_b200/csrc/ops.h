@@ -15,6 +15,7 @@ enum EpiMode {
   EPI_SWIGLU = 2,  // W rows interleaved (gate_j, up_j): C[:, j] = silu(g_j) * u_j          (N_out = N/2)
   EPI_GEGLU = 3,   // W rows interleaved (hidden_j, gate_j): C[:, j] = h_j * gelu_erf(g_j)   (N_out = N/2)
   EPI_RELU = 4,    // C = relu(A W^T + bias)   (T5 DenseReluDense)
+  EPI_QUICK_GELU = 5,  // C = h * sigmoid(1.702 h), h = A W^T + bias   (CLIP MLP; Linear layers only, no cluster)
 };
 
 struct GemmEpilogue {

@@ -67,16 +67,21 @@ __device__ __forceinline__ int clip8(int v) {
   return v < 0 ? 0 : (v > 255 ? 255 : v);
 }
 
-// horizontal pass: in [H, W, 3] -> out [H, outW, 3]
+// horizontal pass: input rows [y0, y0 + H) of in [*, W, 3] -> out [H, outW, 3]; image blockIdx.y of a batch at in_bs / out_bs
+// bytes.  The tables may cover a window of the resized width only (the CLIP centre crop): a pass is separable, so the
+// columns it computes do not depend on the ones it skips.
 __global__ void resample_h_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, int H, int W, int outW,
-                                  const int* __restrict__ bounds, const int* __restrict__ kk, int ksize) {
+                                  const int* __restrict__ bounds, const int* __restrict__ kk, int ksize, int y0, long in_bs,
+                                  long out_bs) {
+  in += blockIdx.y * in_bs;
+  out += blockIdx.y * out_bs;
   const long total = (long)H * outW;
   for (long idx = blockIdx.x * (long)blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
     const int xx = (int)(idx % outW);
     const long y = idx / outW;
     const int x0 = bounds[2 * xx], n = bounds[2 * xx + 1];
     const int* k = kk + (long)xx * ksize;
-    const uint8_t* p = in + (y * W + x0) * 3;
+    const uint8_t* p = in + ((y0 + y) * W + x0) * 3;
     int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
     for (int x = 0; x < n; ++x) {
       const int kv = k[x];
@@ -91,24 +96,27 @@ __global__ void resample_h_kernel(const uint8_t* __restrict__ in, uint8_t* __res
   }
 }
 
-// vertical pass + ToTensor + Normalize: in [H, outW, 3] uint8 -> out [3, outH, outW] fp32 / bf16.  has_v == 0: no resize
+// vertical pass + ToTensor + Normalize: columns [x0, x0 + outW) of in [*, in_w, 3] uint8 -> out [3, outH, outW] fp32 / bf16.
+// has_v == 0: no resize, output row yy is input row y0 + yy.  Batch as in resample_h_kernel (out_bs in elements).
 struct NormParams {
   float mean[3], stdv[3];
 };
 __global__ void resample_v_norm_kernel(const uint8_t* __restrict__ in, void* out, int H, int outH, int outW,
                                        const int* __restrict__ bounds, const int* __restrict__ kk, int ksize, int has_v,
-                                       NormParams np, int out_bf16) {
+                                       NormParams np, int out_bf16, int in_w, int x0, int y0, long in_bs, long out_bs) {
+  in += blockIdx.y * in_bs + (long)x0 * 3;
   const long plane = (long)outH * outW;
+  const long obase = blockIdx.y * out_bs;
   for (long idx = blockIdx.x * (long)blockDim.x + threadIdx.x; idx < plane; idx += (long)gridDim.x * blockDim.x) {
     const int xx = (int)(idx % outW);
     const int yy = (int)(idx / outW);
     int u[3];
     if (has_v) {
-      const int y0 = bounds[2 * yy], n = bounds[2 * yy + 1];
+      const int r0 = bounds[2 * yy], n = bounds[2 * yy + 1];
       const int* k = kk + (long)yy * ksize;
       int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
       for (int y = 0; y < n; ++y) {
-        const uint8_t* p = in + ((long)(y0 + y) * outW + xx) * 3;
+        const uint8_t* p = in + ((long)(r0 + y) * in_w + xx) * 3;
         const int kv = k[y];
         a0 += p[0] * kv;
         a1 += p[1] * kv;
@@ -116,14 +124,14 @@ __global__ void resample_v_norm_kernel(const uint8_t* __restrict__ in, void* out
       }
       u[0] = clip8(a0); u[1] = clip8(a1); u[2] = clip8(a2);
     } else {
-      const uint8_t* p = in + ((long)yy * outW + xx) * 3;
+      const uint8_t* p = in + ((long)(y0 + yy) * in_w + xx) * 3;
       u[0] = p[0]; u[1] = p[1]; u[2] = p[2];
     }
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const float f = __fdiv_rn(__fsub_rn(__fdiv_rn((float)u[c], 255.0f), np.mean[c]), np.stdv[c]);
-      if (out_bf16) reinterpret_cast<bf16*>(out)[c * plane + idx] = __float2bfloat16_rn(f);
-      else reinterpret_cast<float*>(out)[c * plane + idx] = f;
+      if (out_bf16) reinterpret_cast<bf16*>(out)[obase + c * plane + idx] = __float2bfloat16_rn(f);
+      else reinterpret_cast<float*>(out)[obase + c * plane + idx] = f;
     }
   }
 }
@@ -135,6 +143,87 @@ __global__ void to_uint8_kernel(const float* __restrict__ x, uint8_t* __restrict
     const float v = rintf(__fmul_rn(x[i], 255.0f));
     y[i] = (uint8_t)(v < 0.f ? 0.f : (v > 255.f ? 255.f : v));
   }
+}
+
+// ---- CLIPImageProcessor (the safety checker's feature extractor) ----
+// resize so that the shortest edge is `size` (long edge int(size * long / short), transformers get_resize_output_image_size),
+// PIL bicubic on uint8, then the centre crop top = (h' - crop) // 2, left = (w' - crop) // 2.  Only the crop window of the
+// resized image is computed: the coefficient tables are sliced to it, and the horizontal pass runs only over the input rows
+// the window's vertical taps reach.
+int clip_plan(int H, int W, int size, int crop, ClipPlan* p) {
+  if (H < 1 || W < 1 || size < 1 || crop < 1) return EMU_ERR_INVALID;
+  const int sh = H <= W ? H : W, lo = H <= W ? W : H;
+  const int rl = (int)((double)((long)size * lo) / sh);
+  p->H = H; p->W = W; p->crop = crop;
+  p->rh = H <= W ? size : rl;
+  p->rw = H <= W ? rl : size;
+  if (crop > p->rh || crop > p->rw) return EMU_ERR_INVALID;
+  p->top = (p->rh - crop) / 2;
+  p->left = (p->rw - crop) / 2;
+  p->need_h = p->rw != W;
+  p->need_v = p->rh != H;
+  std::vector<int> bh, kh, bv, kv;
+  p->ksh = p->need_h ? precompute_coeffs(W, p->rw, bh, kh) : 0;
+  p->ksv = p->need_v ? precompute_coeffs(H, p->rh, bv, kv) : 0;
+  // rows of the input the vertical window reads (all of the crop rows when there is no vertical resize)
+  p->row0 = p->top;
+  p->rows = crop;
+  if (p->need_v) {
+    int r0 = H, r1 = 0;
+    for (int yy = p->top; yy < p->top + crop; ++yy) {
+      r0 = bv[2 * yy] < r0 ? bv[2 * yy] : r0;
+      r1 = bv[2 * yy] + bv[2 * yy + 1] > r1 ? bv[2 * yy] + bv[2 * yy + 1] : r1;
+    }
+    p->row0 = r0;
+    p->rows = r1 - r0;
+  }
+  // table = [bounds_h | coeffs_h | bounds_v | coeffs_v] over the window; vertical starts relative to the first row the
+  // horizontal pass produced (it writes rows [row0, row0 + rows) of the input as rows 0.. of its output)
+  p->tab.clear();
+  p->off_kh = p->off_bv = p->off_kv = 0;
+  if (p->need_h) {
+    for (int xx = p->left; xx < p->left + crop; ++xx) { p->tab.push_back(bh[2 * xx]); p->tab.push_back(bh[2 * xx + 1]); }
+    p->off_kh = p->tab.size();
+    p->tab.insert(p->tab.end(), kh.begin() + (size_t)p->left * p->ksh, kh.begin() + (size_t)(p->left + crop) * p->ksh);
+  }
+  p->off_bv = p->tab.size();
+  if (p->need_v) {
+    const int base = p->need_h ? p->row0 : 0;
+    for (int yy = p->top; yy < p->top + crop; ++yy) { p->tab.push_back(bv[2 * yy] - base); p->tab.push_back(bv[2 * yy + 1]); }
+    p->off_kv = p->tab.size();
+    p->tab.insert(p->tab.end(), kv.begin() + (size_t)p->top * p->ksv, kv.begin() + (size_t)(p->top + crop) * p->ksv);
+  }
+  if (p->tab.empty()) p->tab.push_back(0);
+  return EMU_OK;
+}
+
+size_t clip_tmp_bytes(const ClipPlan& p, int B) { return p.need_h ? (size_t)B * p.rows * p.crop * 3 : 0; }
+
+int clip_launch(const ClipPlan& p, const int* d_tab, const uint8_t* in, int B, uint8_t* tmp, void* out, const float* mean3,
+                const float* std3, int out_bf16, cudaStream_t st) {
+  const long in_bs = (long)p.H * p.W * 3;
+  const uint8_t* v_in = in;
+  long v_bs = in_bs;
+  int in_w = p.W, x0 = p.left, y0 = p.top;
+  if (p.need_h) {
+    const long total = (long)p.rows * p.crop;
+    const int grid = (int)((total + 255) / 256 < 2 * kNumSMs ? (total + 255) / 256 : 2 * kNumSMs);
+    resample_h_kernel<<<dim3(grid, B), 256, 0, st>>>(in, tmp, p.rows, p.W, p.crop, d_tab, d_tab + p.off_kh, p.ksh, p.row0,
+                                                     in_bs, (long)p.rows * p.crop * 3);
+    count_launch();
+    v_in = tmp;
+    v_bs = (long)p.rows * p.crop * 3;
+    in_w = p.crop; x0 = 0; y0 = 0;  // the horizontal pass already cut the window (rows from row0 == top when no v-resize)
+  }
+  NormParams np;
+  for (int c = 0; c < 3; ++c) { np.mean[c] = mean3[c]; np.stdv[c] = std3[c]; }
+  const long plane = (long)p.crop * p.crop;
+  const int grid = (int)((plane + 255) / 256 < 2 * kNumSMs ? (plane + 255) / 256 : 2 * kNumSMs);
+  resample_v_norm_kernel<<<dim3(grid, B), 256, 0, st>>>(v_in, out, p.rows, p.crop, p.crop, d_tab + p.off_bv,
+                                                        d_tab + p.off_kv, p.ksv, p.need_v ? 1 : 0, np, out_bf16, in_w, x0, y0,
+                                                        v_bs, 3 * plane);
+  count_launch();
+  return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
 }  // namespace emu
@@ -178,7 +267,7 @@ extern "C" int emu_preprocess_image(const uint8_t* rgb_hwc, int H, int W, int ou
     if (!rc) {
       const long total = (long)H * out_w;
       const int grid = (int)((total + 255) / 256 < 8 * kNumSMs ? (total + 255) / 256 : 8 * kNumSMs);
-      resample_h_kernel<<<grid, 256, 0, st>>>(rgb_hwc, d_tmp, H, W, out_w, d_bh, d_kh, ksh);
+      resample_h_kernel<<<grid, 256, 0, st>>>(rgb_hwc, d_tmp, H, W, out_w, d_bh, d_kh, ksh, 0, 0, 0);
       v_in = d_tmp;
       count_launch();
     }
@@ -189,11 +278,31 @@ extern "C" int emu_preprocess_image(const uint8_t* rgb_hwc, int H, int W, int ou
     const long plane = (long)out_h * out_w;
     const int grid = (int)((plane + 255) / 256 < 8 * kNumSMs ? (plane + 255) / 256 : 8 * kNumSMs);
     resample_v_norm_kernel<<<grid, 256, 0, st>>>(v_in, out_chw, H, out_h, out_w, d_bv, d_kv, ksv, need_v ? 1 : 0, np,
-                                                 out_dtype == EMU_DTYPE_BF16 ? 1 : 0);
+                                                 out_dtype == EMU_DTYPE_BF16 ? 1 : 0, out_w, 0, 0, 0, 0);
     count_launch();
     if (cudaGetLastError() != cudaSuccess) rc = EMU_ERR_CUDA;
   }
   if (d_tmp) cudaFreeAsync(d_tmp, st);
   if (d_tab) cudaFreeAsync(d_tab, st);
+  return rc;
+}
+
+extern "C" int emu_preprocess_clip(const uint8_t* images_bhwc, int B, int H, int W, int size, int crop, const float* mean3,
+                                   const float* std3, void* out_bchw, int out_dtype, emu_stream_t stream) {
+  if (!images_bhwc || !out_bchw || !mean3 || !std3 || B < 1 || H < 1 || W < 1 || size < 1 || crop < 1) return EMU_ERR_INVALID;
+  if (out_dtype != EMU_DTYPE_F32 && out_dtype != EMU_DTYPE_BF16) return EMU_ERR_INVALID;
+  ClipPlan p;
+  if (clip_plan(H, W, size, crop, &p) != EMU_OK) return EMU_ERR_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  int* d_tab = nullptr;
+  uint8_t* d_tmp = nullptr;
+  if (cudaMallocAsync((void**)&d_tab, p.tab.size() * sizeof(int), st) != cudaSuccess) return EMU_ERR_NOMEM;
+  int rc = cudaMemcpyAsync(d_tab, p.tab.data(), p.tab.size() * sizeof(int), cudaMemcpyHostToDevice, st) == cudaSuccess
+               ? EMU_OK : EMU_ERR_CUDA;
+  const size_t tb = clip_tmp_bytes(p, B);
+  if (!rc && tb && cudaMallocAsync((void**)&d_tmp, tb, st) != cudaSuccess) rc = EMU_ERR_NOMEM;
+  if (!rc) rc = clip_launch(p, d_tab, images_bhwc, B, d_tmp, out_bchw, mean3, std3, out_dtype == EMU_DTYPE_BF16, st);
+  if (d_tmp) cudaFreeAsync(d_tmp, st);
+  cudaFreeAsync(d_tab, st);
   return rc;
 }

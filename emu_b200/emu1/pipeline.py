@@ -11,10 +11,12 @@ embeddings, cached form) for [prompt, ""] -> Stable-Diffusion-1.5-topology UNet 
 widths 40 / 80 / 160, no added conditioning) under classifier-free guidance with the PNDM / PLMS scheduler, one CUDA-graphed
 fused iteration per timestep (emu_denoise_step_multistep) -> VAE decode -> uint8 on the device.
 
-Safety stage: the reference runs diffusers' StableDiffusionSafetyChecker on the decoded image (:142-147, :218-232).  That CLIP
-classifier is third-party and not part of this engine; pass ``safety_checker=callable(images_uint8) -> (images, [bool])`` to keep
-the stage.  Without one the image is returned unfiltered, the flag is None (what the reference returns when built without a
-checker) and a UserWarning says so; ``requires_safety_checker=True`` turns a missing hook into an error.
+Safety stage: the reference runs diffusers' StableDiffusionSafetyChecker on the decoded image (:142-147, :218-232).
+``safety_checker=emu_b200.safety.SafetyChecker.from_pretrained(f"{path}/safety_checker")`` runs it on the engine (bound to this
+pipeline's engine, weights from that directory, the check on the device before the copy to the host); any other
+``safety_checker=callable(images_uint8) -> (images, [bool])`` is called as a host hook.  Without one the image is returned
+unfiltered, the flag is None (what the reference returns when built without a checker) and a UserWarning says so;
+``requires_safety_checker=True`` turns a missing checker into an error.
 """
 import json
 import os.path as osp
@@ -26,6 +28,7 @@ import torch
 from PIL import Image
 
 from .. import _lib, checkpoint
+from ..safety import SafetyChecker
 from ..emu2.diffusion import image_transform, image_transform_cuda, unet_config_from_json, vae_config_from_json
 from .modeling_emu import Emu
 from .scheduler import PNDMScheduler
@@ -51,6 +54,8 @@ class EmuGenerationPipeline:
         self.emu_encoder = emu_encoder if emu_encoder is not None else self.prepare_emu("Emu-14B", multimodal_model, **kwargs)
         self.engine = self.emu_encoder.engine
         self.device_ = self.emu_encoder.device_
+        if isinstance(self.safety_checker, SafetyChecker):
+            self.safety_checker.bind(self.engine)
         if unet_config is None:
             unet_config = json.load(open(osp.join(unet, "config.json")))
         if vae_config is None and vae is not None:
@@ -93,7 +98,7 @@ class EmuGenerationPipeline:
     def load_state_dict(self, sd, strict=True):
         """unet.* / vae.* (decoder half) / emu_encoder.* keys in one dict (tests, synthetic weights)."""
         for k, v in sd.items():
-            if k.startswith("safety_checker."):
+            if k.startswith("safety_checker.") and not isinstance(self.safety_checker, SafetyChecker):
                 self._note_unfiltered("the state dict carries safety_checker.* weights")
                 continue
             if k.startswith("vae.") and (self.vae_config is None or ".encoder." in k or k.startswith("vae.quant_conv")):
@@ -123,8 +128,7 @@ class EmuGenerationPipeline:
                                guidance_scale, generator=generator, latents=latents)
         if output_type == "latent":
             return latents
-        u8 = self.decode_latents_uint8(latents)
-        u8, flags = self.run_safety_checker(u8)
+        u8, flags = self.decode_and_check(latents)
         return Image.fromarray(u8[0]), (None if flags is None else flags[0])
 
     __call__ = forward
@@ -169,6 +173,15 @@ class EmuGenerationPipeline:
     def decode_latents_uint8(self, latents: torch.Tensor) -> np.ndarray:
         z = (latents.float() / self.vae_scaling).to(torch.bfloat16).contiguous()
         return _lib.op_image_to_uint8(self.engine.vae_decode(z)).cpu().numpy()
+
+    def decode_and_check(self, latents: torch.Tensor):
+        """decode -> uint8 -> safety stage; a built-in SafetyChecker runs on the device image before the copy to the host"""
+        if isinstance(self.safety_checker, SafetyChecker):
+            z = (latents.float() / self.vae_scaling).to(torch.bfloat16).contiguous()
+            dev = _lib.op_image_to_uint8(self.engine.vae_decode(z))
+            flags = self.safety_checker.check_device(dev)
+            return dev.cpu().numpy(), [bool(f) for f in flags.tolist()]
+        return self.run_safety_checker(self.decode_latents_uint8(latents))
 
     def decode_latents(self, latents: torch.Tensor) -> np.ndarray:
         z = (latents.float() / self.vae_scaling).to(torch.bfloat16).contiguous()

@@ -77,6 +77,18 @@ EMU2_GEN_SCHEDULER = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end
                           prediction_type="epsilon", interpolation_type="linear", timestep_spacing="leading", steps_offset=1,
                           use_karras_sigmas=False)
 
+# The published safety checker (Emu2/emu/conf/diffusion_config/safety_checker/config.json, vision part + projection_dim: a CLIP
+# ViT-L/14 tower) and its feature extractor (feature_extractor/preprocessor_config.json): what `SafetyChecker()` uses when no
+# configuration directory is given.
+EMU2_GEN_SAFETY_CHECKER = dict(
+    projection_dim=768,
+    vision_config=dict(hidden_size=1024, intermediate_size=4096, num_hidden_layers=24, num_attention_heads=16, patch_size=14,
+                       image_size=224, num_channels=3, hidden_act="quick_gelu", layer_norm_eps=1e-5))
+EMU2_GEN_FEATURE_EXTRACTOR = dict(
+    do_resize=True, size={"shortest_edge": 224}, resample=3, do_center_crop=True, crop_size={"height": 224, "width": 224},
+    do_rescale=True, rescale_factor=0.00392156862745098, do_normalize=True, do_convert_rgb=True,
+    image_mean=[0.48145466, 0.4578275, 0.40821073], image_std=[0.26862954, 0.26130258, 0.27577711])
+
 
 def load_diffusion_config(config_path=None):
     """-> (unet, vae, scheduler) config dicts from a diffusers-style directory (`unet/config.json`, `vae/config.json`,

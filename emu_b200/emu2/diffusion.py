@@ -7,11 +7,12 @@ prompt encoding through ``EmuModel.generate_image`` / ``encode_image``, the deno
 ``emu_denoise_step`` per iteration (cat + scale_model_input + UNet + CFG + Euler fused), VAE decode on device.
 
 Safety stage.  The reference runs diffusers' ``StableDiffusionSafetyChecker`` on the decoded image and blanks flagged ones
-(Emu2/emu/diffusion.py:154-166, 236-249).  That CLIP classifier is third-party and not part of this engine, so it is NOT
-silently dropped: pass ``safety_checker=callable(images_uint8 [B,H,W,3] numpy) -> (images, [bool])`` to keep the stage
-(e.g. the diffusers module wrapped by the caller), or construct with the default ``safety_checker=None`` and get a
-``UserWarning`` the first time an image is returned unfiltered (``nsfw_content_detected`` is then None, which is what the
-reference reports for a pipeline built without a checker).  ``requires_safety_checker=True`` makes a missing hook an error.
+(Emu2/emu/diffusion.py:154-166, 236-249).  ``safety_checker=emu_b200.safety.SafetyChecker()`` runs that checker on the engine:
+it is bound to this pipeline's engine, takes the checkpoint's ``safety_checker.*`` weights, and checks the uint8 image on the
+device before it is copied to the host.  Any other ``safety_checker=callable(images_uint8 [B,H,W,3] numpy) -> (images,
+[bool])`` is called as a hook on the host.  With the default ``safety_checker=None`` a ``UserWarning`` comes the first time an
+image is returned unfiltered (``nsfw_content_detected`` is then None, which is what the reference reports for a pipeline built
+without a checker).  ``requires_safety_checker=True`` makes a missing checker an error.
 """
 import json
 import os
@@ -25,6 +26,7 @@ import torch
 from PIL import Image
 
 from .. import _lib
+from ..safety import SafetyChecker
 from .conf import CLIPVisionCfg, TextDecoderCfg
 from .constants import DEFAULT_IMG_PLACEHOLDER, EVA_IMAGE_SIZE, OPENAI_DATASET_MEAN, OPENAI_DATASET_STD
 from .emu import EmuModel
@@ -110,6 +112,8 @@ class EmuVisualGeneration:
         self._warned_unfiltered = False
         self.multimodal_encoder = multimodal_encoder
         self.engine = multimodal_encoder.engine
+        if isinstance(safety_checker, SafetyChecker):
+            safety_checker.bind(self.engine)
         self.scheduler = scheduler
         self.unet_config, self.vae_config = unet_config, vae_config
         self.engine.unet_configure(unet_config_from_json(unet_config))
@@ -131,10 +135,14 @@ class EmuVisualGeneration:
     def eval(self):
         return self
 
+    def _builtin_checker(self):
+        return isinstance(self.safety_checker, SafetyChecker)
+
     def load_state_dict(self, sd, strict=True):
-        """Keys as saved by the reference pipeline: multimodal_encoder.*, unet.*, vae.* (safety_checker.* ignored)."""
+        """Keys as saved by the reference pipeline: multimodal_encoder.*, unet.*, vae.*, and safety_checker.* (loaded into a
+        built-in SafetyChecker, ignored otherwise)."""
         for k, v in sd.items():
-            if k.startswith("safety_checker."):
+            if k.startswith("safety_checker.") and not self._builtin_checker():
                 self._note_checker_weights()
                 continue
             if k.endswith("rotary_emb.inv_freq"):
@@ -178,8 +186,7 @@ class EmuVisualGeneration:
                                original_size, generator=generator, latents=latents)
         if output_type == "latent":
             return latents
-        u8 = self.decode_latents_uint8(latents)
-        u8, flags = self.run_safety_checker(u8)
+        u8, flags = self.decode_and_check(latents)
         return EmuVisualGenerationPipelineOutput(image=Image.fromarray(u8[0]),
                                                  nsfw_content_detected=None if flags is None else flags[0])
 
@@ -204,8 +211,7 @@ class EmuVisualGeneration:
         prompt_embeds = torch.cat(cond + uncond, dim=0).to(torch.bfloat16).contiguous()
         latents = self.denoise(prompt_embeds, len(batch_inputs), height, width, num_inference_steps, guidance_scale,
                                crop_info, original_size, generator=generator)
-        u8 = self.decode_latents_uint8(latents)
-        u8, flags = self.run_safety_checker(u8)
+        u8, flags = self.decode_and_check(latents)
         return [EmuVisualGenerationPipelineOutput(image=Image.fromarray(u8[i]),
                                                   nsfw_content_detected=None if flags is None else flags[i])
                 for i in range(len(batch_inputs))]
@@ -283,6 +289,16 @@ class EmuVisualGeneration:
         z = (latents.float() / self.vae_scaling).to(torch.bfloat16).contiguous()
         return _lib.op_image_to_uint8(self.engine.vae_decode(z)).cpu().numpy()
 
+    def decode_and_check(self, latents: torch.Tensor):
+        """decode -> uint8 -> safety stage -> (images [B, H, W, 3] uint8 numpy, flags list or None).  A built-in SafetyChecker
+        checks (and blacks out) the images on the device before the one device->host copy; a hook runs on the host copy."""
+        if self._builtin_checker():
+            z = (latents.float() / self.vae_scaling).to(torch.bfloat16).contiguous()
+            dev = _lib.op_image_to_uint8(self.engine.vae_decode(z))
+            flags = self.safety_checker.check_device(dev)
+            return dev.cpu().numpy(), [bool(f) for f in flags.tolist()]
+        return self.run_safety_checker(self.decode_latents_uint8(latents))
+
     def decode_latents_pil(self, latents: torch.Tensor):
         return [Image.fromarray(im) for im in self.decode_latents_uint8(latents)]
 
@@ -331,8 +347,8 @@ class EmuVisualGeneration:
         ins = cls.from_config(config_path, **kwargs)
         from .. import checkpoint
 
-        def keep(k):  # same filter as load_state_dict: no safety checker, only the decoder half of the VAE
-            if k.startswith("safety_checker."):
+        def keep(k):  # same filter as load_state_dict: the safety checker only when built in, the decoder half of the VAE
+            if k.startswith("safety_checker.") and not ins._builtin_checker():
                 ins._note_checker_weights()
                 return None
             if k.startswith("vae.") and (ins.vae_config is None or ".encoder." in k or k.startswith("vae.quant_conv")):

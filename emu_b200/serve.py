@@ -378,6 +378,9 @@ def main(argv=None):
     ap.add_argument("--max-wait-ms", type=float, default=2.0)
     ap.add_argument("--max-images-per-batch", type=int, default=4)
     ap.add_argument("--cache-dir", type=str, default="", help="keep request pictures / results here (the reference always does)")
+    ap.add_argument("--safety-checker", action="store_true",
+                    help="run the built-in NSFW safety checker (the checkpoint's safety_checker.* weights) on every generated "
+                         "image: flagged images come back black, with nsfw_content_detected set")
     args = ap.parse_args(argv)
     logging.basicConfig(level=logging.INFO, format="%(asctime)s %(name)s %(levelname)s %(message)s")
     import torch
@@ -408,9 +411,13 @@ def main(argv=None):
     if not args.disable_generate and rank == 0:     # the UNet is not tensor parallel: generation lives on rank 0 only
         for i in range(args.generate_concurrency):
             torch.cuda.set_device(device)
+            extra = {}
+            if args.safety_checker:
+                from .safety import SafetyChecker
+                extra["safety_checker"] = SafetyChecker()
             gen.append(EmuVisualGeneration.from_pretrained(osp.join(args.model_path, "Emu2-Gen_pytorch_model.bf16.safetensors"),
                                                            dtype=torch.bfloat16, use_safetensors=True,
-                                                           device="cuda:%d" % device))
+                                                           device="cuda:%d" % device, **extra))
             device += 1 if world == 1 else 0
     if not args.disable_chat:
         for i in range(args.chat_concurrency):
