@@ -75,6 +75,8 @@ SYMBOLS = [
 ]
 # ... and in include/emu_b200_safety.h (the safety checker)
 SAFETY_SYMBOLS = ["emu_safety_configure", "emu_safety_check", "emu_safety_embed", "emu_preprocess_clip"]
+# ... and in include/emu_b200_slots.h (slot mode: continuous batching)
+SLOT_SYMBOLS = ["emu_llm_slots_begin", "emu_llm_join", "emu_llm_fork", "emu_llm_leave", "emu_llm_slot_len"]
 
 _lib = None
 
@@ -227,6 +229,44 @@ class Engine:
         """cache row b <- row src_idx[b] for b < new_B (beam search: one prefill per prompt, then num_beams cache rows)"""
         src = src_idx.to(torch.int32).contiguous()
         check(self.lib.emu_llm_expand(self.h, _ptr(src), int(new_B), _stream()), self.h)
+
+    # ---- slot mode (include/emu_b200_slots.h): continuous batching ----
+    def slots_begin(self, n_slots):
+        """forget the cache and enter slot mode with n_slots free slots (emu_llm_reset leaves it)"""
+        check(self.lib.emu_llm_slots_begin(self.h, int(n_slots), _stream()), self.h)
+
+    @staticmethod
+    def _host_slots(slots):
+        slots = [int(s) for s in slots]
+        return (C.c_int32 * max(1, len(slots)))(*slots), len(slots)
+
+    def join(self, slots, embeds, attention_mask=None, want_logits=True):
+        """prefill len(slots) new sequences [n, N, hidden] (left-padded mask [n, N]) into the given free slots; returns the
+        logits of every sequence's last position [n, vocab] fp32 (or None)"""
+        n, N, H = embeds.shape
+        if n != len(slots):
+            raise ValueError("join: %d sequences for %d slots" % (n, len(slots)))
+        embeds = embeds.to(torch.bfloat16).contiguous()
+        mask = attention_mask.to(torch.int32).contiguous() if attention_mask is not None else None
+        if mask is not None and tuple(mask.shape) != (n, N):
+            raise ValueError("join: attention_mask must be [%d, %d], got %s" % (n, N, tuple(mask.shape)))
+        logits = torch.empty(n, self.cfg.llm_vocab, dtype=torch.float32, device=embeds.device) if want_logits else None
+        hs, cnt = self._host_slots(slots)
+        check(self.lib.emu_llm_join(self.h, hs, cnt, _ptr(embeds), _ptr(mask), N, _ptr(logits), _stream()), self.h)
+        return logits
+
+    def fork(self, src_slot, dst_slots):
+        """the free dst_slots continue the sequence of src_slot (beam expansion; no KV is moved)"""
+        hs, cnt = self._host_slots(dst_slots)
+        check(self.lib.emu_llm_fork(self.h, int(src_slot), hs, cnt, _stream()), self.h)
+
+    def leave(self, slots):
+        """free the given live slots (a beam group leaves together)"""
+        hs, cnt = self._host_slots(slots)
+        check(self.lib.emu_llm_leave(self.h, hs, cnt, _stream()), self.h)
+
+    def slot_len(self, slot):
+        return int(self.lib.emu_llm_slot_len(self.h, int(slot)))
 
     def sample_tokens(self, logits, temperature=1.0, top_k=0, top_p=1.0, ban_id=-1, seed=0, offset=0):
         return op_sample_tokens(logits, temperature, top_k, top_p, -1 if ban_id is None else ban_id, seed, offset)

@@ -1,0 +1,415 @@
+"""Continuous batching for chat: requests join and leave the decode batch between steps (iteration-level scheduling).
+
+`SlotScheduler` drives the engine's slot mode (include/emu_b200_slots.h): every KV-cache row is a slot holding one sequence of
+its own length.  One `step()` is one iteration:
+
+  1. admit: waiting requests take free slots, lowest first (a beam request takes `num_beams` contiguous slots); their
+     pictures go through the ViT, their prompts are embedded and spliced, and ONE emu_llm_join prefills all of them
+     (left-padded to the longest) while the live slots keep their cache.  A beam request joins into its first slot and is
+     forked to the others.  The join stalls the live requests for one ViT + prefill;
+  2. select: every live request picks its next tokens from ITS OWN rows of the logits with ITS OWN knobs, through the same
+     kernels generation.py uses on a batch of one (beam_topk / sample_tokens / beam_step on the request's contiguous slice),
+     so a request's tokens are the ones it would get alone;
+  3. retire: finished requests leave (their slots are freed) and are answered;
+  4. decode: ONE emu_llm_decode over B = highest occupied slot + 1 advances every live request by one token (free slots
+     below B are computed and ignored).
+
+Each step reads ONE small tensor back to the host: the finish flag of every live request (EOS of a greedy / sampled request,
+`done` of a beam search), which is what lets a request leave as soon as it is finished.
+
+Strategies: greedy, sampling, beam search and beam-sample with min_len, repetition_penalty, no_repeat_ngram_size,
+temperature / top_k / top_p and length_penalty — what the demo's /v1/mmc form can send.  Requests with different knobs share
+a decode step.  A request's output is what generation.generate returns for it alone (beam search: its best hypothesis;
+greedy / sampling: its tokens up to EOS).  Contrastive search, prefix_allowed_tokens_fn and num_return_sequences > 1 are
+refused.  Sampled requests reproduce their solo draws when they carry a `generator`; without one they draw from torch's
+global generator, shared with whatever else runs in the process.
+"""
+import collections
+import threading
+
+import torch
+
+from . import generation
+
+
+class SlotRequest:
+    """One generate call's worth of work: a one-row prompt (token ids, optional pictures) and its decoding knobs, with
+    EmuModel.generate_from_ids' names and defaults.  `result` (token ids [1, T] or the decoded text) or `error` is set
+    when it is finished, then `done` is set and `on_done(request)` is called."""
+
+    def __init__(self, input_ids, attention_mask=None, image=None, video=None, image_token_id=32003, video_token_id=32004,
+                 num_beams=5, max_new_tokens=10, min_len=1, do_sample=False, temperature=None, top_k=None, top_p=None,
+                 length_penalty=-1, repetition_penalty=1.0, no_repeat_ngram_size=0, early_stopping=False, penalty_alpha=None,
+                 num_return_sequences=1, prefix_allowed_tokens_fn=None, generator=None, eos_token_id=None,
+                 pad_token_id=None, finish=None, on_done=None, tag=None):
+        ids = torch.as_tensor(input_ids)
+        self.input_ids = ids.view(1, -1) if ids.dim() == 1 else ids
+        if self.input_ids.shape[0] != 1:
+            raise ValueError("a request holds one prompt, got input_ids of shape %s" % (tuple(self.input_ids.shape),))
+        self.attention_mask = (torch.ones_like(self.input_ids) if attention_mask is None
+                               else torch.as_tensor(attention_mask).view(1, -1))
+        self.image, self.video = image, video
+        self.image_token_id, self.video_token_id = image_token_id, video_token_id
+        self.num_beams = int(num_beams or 1)
+        self.max_new_tokens, self.min_len = int(max_new_tokens), int(min_len or 0)
+        self.do_sample = bool(do_sample)
+        self.temperature, self.top_k, self.top_p = temperature, top_k, top_p
+        self.length_penalty, self.early_stopping = length_penalty, early_stopping
+        self.repetition_penalty = 1.0 if repetition_penalty is None else float(repetition_penalty)
+        self.ngram = int(no_repeat_ngram_size or 0)
+        self.generator = generator
+        self.eos, self.pad = eos_token_id, pad_token_id
+        self.finish, self.on_done, self.tag = finish, on_done, tag
+        self.done = threading.Event()
+        self.result = self.error = None
+        if self.num_beams < 1:
+            raise ValueError("num_beams has to be an integer >= 1")
+        if self.max_new_tokens < 1:
+            raise ValueError("max_new_tokens has to be >= 1")
+        if self.num_beams == 1 and not self.do_sample and penalty_alpha is not None and penalty_alpha > 0 \
+                and top_k is not None and top_k > 1:
+            raise ValueError("continuous batching does not run contrastive search (penalty_alpha with top_k > 1)")
+        if prefix_allowed_tokens_fn is not None:
+            raise ValueError("continuous batching does not take prefix_allowed_tokens_fn")
+        if int(num_return_sequences or 1) != 1:
+            raise ValueError("continuous batching returns one sequence per request (num_return_sequences = 1)")
+        # set at admission
+        self.slots = []
+        self.engine_slots = []      # the slots the engine holds for this request (joined / forked): they must leave
+        self.step = 0
+        self.logits = None
+
+
+class SlotScheduler:
+    """Continuous batching over `emu_model` (an EmuModel: its engine, tokenizer ids, ViT and projection) with `n_slots`
+    KV-cache slots (at most the engine's llm_max_batch).  Owns the engine while it lives: nothing else may use the engine's
+    LLM between steps.  Single-threaded: `submit` may be called from any thread, `step` from one."""
+
+    def __init__(self, emu_model, n_slots=None):
+        self.model = emu_model
+        self.engine = emu_model.engine
+        cfg = self.engine.cfg
+        self.n_slots = int(n_slots or cfg.llm_max_batch)
+        if not 1 <= self.n_slots <= cfg.llm_max_batch:
+            raise ValueError("n_slots = %d must be in [1, llm_max_batch = %d]" % (self.n_slots, cfg.llm_max_batch))
+        self.max_seq = int(getattr(cfg, "llm_max_seq", 0) or 0)
+        self.V = cfg.llm_vocab
+        self.device = torch.device(emu_model.device())
+        tok = getattr(getattr(emu_model, "decoder", None), "tokenizer", None)
+        self.eos = getattr(tok, "eos_token_id", None)
+        self.pad = getattr(tok, "pad_token_id", None)
+        self.waiting = collections.deque()
+        self.live = []                                      # admitted requests, in admission order
+        self.owner = [None] * self.n_slots                  # slot -> request
+        self.steps = 0
+        self.batch_sizes = collections.deque(maxlen=1024)   # B of the recent decode steps (observability; the tests read it)
+        self._lock = threading.Lock()
+        i32 = dict(dtype=torch.int32, device=self.device)
+        self.tok_buf = torch.zeros(self.n_slots, **i32)      # fixed buffers: the decode graphs are keyed by their pointers
+        self.ident = torch.arange(self.n_slots, **i32)
+        self.src_buf = self.ident.clone()                    # identity except the rows of live beam groups
+        self.logits_buf = torch.zeros(self.n_slots, self.V, dtype=torch.float32, device=self.device)
+        with _on_device(self.device):
+            self.engine.slots_begin(self.n_slots)
+
+    # ---- producer side ----
+    def submit(self, request: SlotRequest):
+        if request.eos is None:
+            request.eos = self.eos
+        if request.pad is None:
+            request.pad = self.pad
+        if request.num_beams > self.n_slots:
+            raise ValueError("num_beams = %d exceeds the scheduler's %d slots" % (request.num_beams, self.n_slots))
+        n_prompt = request.input_ids.shape[1]
+        if self.max_seq and n_prompt > self.max_seq:
+            raise ValueError("prompt of %d tokens exceeds llm_max_seq = %d" % (n_prompt, self.max_seq))
+        with self._lock:
+            self.waiting.append(request)
+        return request
+
+    def busy(self):
+        return bool(self.live) or bool(self.waiting)
+
+    def load(self):
+        """requests admitted or waiting"""
+        return len(self.live) + len(self.waiting)
+
+    # ---- one iteration ----
+    @torch.no_grad()
+    def step(self):
+        """admit -> select -> retire -> decode (module docstring); returns the requests finished in this step"""
+        with _on_device(self.device):
+            return self._step()
+
+    def _step(self):
+        self._admit()
+        finished = self._select()
+        for r in finished:
+            self._retire(r)
+        if self.live:
+            self._decode()
+        self.steps += 1
+        return finished
+
+    def abort(self, ex):
+        """fail every live and waiting request with `ex` (the scheduler itself stays usable)"""
+        for r in list(self.live):
+            self._fail(r, ex)
+        with self._lock:
+            waiting, self.waiting = list(self.waiting), collections.deque()
+        for r in waiting:
+            self._fail(r, ex)
+
+    def run_until_idle(self):
+        out = []
+        while self.busy():
+            out += self.step()
+        return out
+
+    # ---- admission ----
+    def _free_run(self, n):
+        """lowest first slot of n contiguous free slots, or None"""
+        run = 0
+        for s in range(self.n_slots):
+            run = run + 1 if self.owner[s] is None else 0
+            if run == n:
+                return s - n + 1
+        return None
+
+    def _admit(self):
+        batch = []
+        with self._lock:
+            while self.waiting:
+                r = self.waiting[0]
+                first = self._free_run(r.num_beams)
+                if first is None:
+                    break                                   # first come, first served: the head waits for room
+                self.waiting.popleft()
+                r.slots = list(range(first, first + r.num_beams))
+                for s in r.slots:
+                    self.owner[s] = r
+                batch.append(r)
+        if not batch:
+            return
+        ready = []
+        for r in batch:                                     # a prompt that cannot be embedded fails on its own
+            try:
+                ready.append((r, self._embed(r)))
+            except Exception as ex:
+                self._fail(r, ex)
+        for group in self._join_groups(ready):
+            try:
+                self._join(group)
+            except Exception as ex:                         # nothing of this group was joined
+                if len(group) == 1:
+                    self._fail(group[0][0], ex)
+                    continue
+                for item in group:                          # a shared join failed: join one by one, only the culprit fails
+                    try:
+                        self._join([item])
+                    except Exception as ex1:
+                        self._fail(item[0], ex1)
+
+    def _cap(self, r, n):
+        """r's max_new_tokens in a slot that holds n prompt positions: the last token is never fed back, so the slot ends
+        at n + max_new_tokens - 1 positions, which must fit llm_max_seq"""
+        return min(r.max_new_tokens, self.max_seq - n + 1) if self.max_seq else r.max_new_tokens
+
+    def _join_groups(self, ready):
+        """split the admitted prompts into joins (usually one) such that left-padding a prompt to its join's length never
+        leaves it less room than it has alone"""
+        groups = []
+        for item in ready:
+            for g in groups:
+                N = max(e.shape[1] for _, (e, _) in g + [item])
+                if all(self._cap(r, N) == self._cap(r, e.shape[1]) for r, (e, _) in g + [item]):
+                    g.append(item)
+                    break
+            else:
+                groups.append([item])
+        return groups
+
+    def _embed(self, r):
+        m = self.model
+        ids = r.input_ids.to(self.device)
+        return m.embed_prompt(ids, r.image, r.video, r.image_token_id, r.video_token_id), r.attention_mask.to(self.device)
+
+    def _join(self, items):
+        """one emu_llm_join for `items`; raises only if nothing was joined.  After the join every request is on its own: a
+        request that fails later leaves the slots the engine holds for it."""
+        N = max(e.shape[1] for _, (e, _) in items)
+        embeds = torch.zeros(len(items), N, items[0][1][0].shape[-1], dtype=items[0][1][0].dtype, device=self.device)
+        mask = torch.zeros(len(items), N, dtype=torch.int32, device=self.device)
+        for i, (_, (e, m)) in enumerate(items):            # left padding, as the tokenizer pads a batch
+            embeds[i, N - e.shape[1]:] = e[0]
+            mask[i, N - e.shape[1]:] = m[0].to(torch.int32)
+        logits = self.engine.join([r.slots[0] for r, _ in items], embeds, mask)
+        for r, _ in items:
+            r.engine_slots = [r.slots[0]]
+        for i, (r, _) in enumerate(items):
+            try:
+                r.max_new_tokens = self._cap(r, N)          # the room it has alone (_join_groups)
+                if r.num_beams > 1:
+                    self.engine.fork(r.slots[0], r.slots[1:])
+                    r.engine_slots = list(r.slots)
+                r.logits = logits[i:i + 1].repeat(r.num_beams, 1).contiguous() if r.num_beams > 1 else logits[i:i + 1]
+                self._start(r)
+            except Exception as ex:
+                self._fail(r, ex)
+                continue
+            self.live.append(r)
+
+    def _start(self, r):
+        """per-request selection state, as the solo loop of its strategy sets it up (generation.py)"""
+        dev, nb = self.device, r.num_beams
+        r.processed = r.repetition_penalty != 1.0 or bool(r.ngram)
+        if nb > 1:
+            r.kind = "beam"
+            r.beams = self.engine.beam_state(1, nb, r.max_new_tokens, r.pad, dev)
+            r.zero_run = torch.zeros(1, nb, dtype=torch.float32, device=dev) if r.do_sample else None
+            return
+        r.kind = "sample" if r.do_sample else "greedy"
+        r.zero_run = torch.zeros(1, 1, dtype=torch.float32, device=dev)
+        r.prev = torch.full((1, r.max_new_tokens), r.pad, dtype=torch.int32, device=dev)
+        r.out = []
+        if r.do_sample:   # sample_search's per-call seed, drawn from the request's generator
+            g = r.generator
+            r.seed = int(torch.randint(0, 2 ** 62, (1,), generator=g, device="cpu" if g is None else g.device))
+
+    # ---- selection ----
+    def _select(self):
+        flags, order = [], []
+        for r in list(self.live):
+            try:
+                flags.append(self._select_one(r))
+                order.append(r)
+            except Exception as ex:
+                self._fail(r, ex)
+        if not order:
+            return []
+        hit = torch.stack([f.reshape(()).to(torch.int32) for f in flags]).tolist()   # the one read-back of the step
+        done = []
+        for r, h in zip(order, hit):
+            if h or r.step >= r.max_new_tokens:
+                done.append(r)
+        return done
+
+    def _select_one(self, r):
+        """r's next tokens from r.logits ([num_beams, V]); writes them (and the beam re-parenting) into the decode inputs
+        of r's slots and returns a device flag: r is finished"""
+        eng, step, first, nb = self.engine, r.step, r.slots[0], r.num_beams
+        ban = r.eos if step < r.min_len else -1
+        if r.kind == "beam":
+            st = r.beams
+            live = st.running_seq[st.live(step)]
+            need_prev = r.processed and step > 0
+            topk_lp, topk_i = eng.beam_topk(r.logits, r.zero_run if r.do_sample else st.running_scores, 1, nb, 2 * nb,
+                                            ban_id=ban, prev_tokens=live.view(nb, st.max_length) if need_prev else None,
+                                            prev_len=step, repetition_penalty=r.repetition_penalty, penalty_on_logits=False,
+                                            no_repeat_ngram=r.ngram)
+            if r.do_sample:
+                lp = generation._warp_log_probs(r.logits.view(nb, self.V), r.temperature, r.top_k, r.top_p, min_keep=2)
+                acc = (lp.view(1, nb, self.V) + st.running_scores.view(1, nb, 1)).view(1, nb * self.V)
+                pick = torch.multinomial(torch.softmax(acc, dim=-1), num_samples=2 * nb, generator=r.generator)
+                topk_lp, topk_i = torch.gather(acc, 1, pick).contiguous(), pick.to(torch.int32).contiguous()
+            eng.beam_step(st, topk_lp, topk_i, step, r.eos, r.length_penalty, r.early_stopping)
+            r.step = step + 1
+            self.tok_buf[first:first + nb] = st.next_tokens
+            self.src_buf[first:first + nb] = st.beam_src + first
+            return st.done
+        if r.kind == "greedy" and not r.processed:
+            lg = r.logits
+            if ban >= 0:
+                lg[:, ban] = float("-inf")
+            nxt = lg.argmax(-1).to(torch.int32)
+        else:
+            if r.processed:   # the processor kernels (one beam) leave the processed log-probabilities in r.logits
+                _, idx = eng.beam_topk(r.logits, r.zero_run, 1, 1, 2, ban_id=ban, prev_tokens=r.prev if step > 0 else None,
+                                       prev_len=step, repetition_penalty=r.repetition_penalty, penalty_on_logits=True,
+                                       no_repeat_ngram=r.ngram)
+            if r.kind == "greedy":
+                nxt = idx[:, 0].to(torch.int32)
+            else:
+                nxt = eng.sample_tokens(r.logits, r.temperature or 1.0, r.top_k or 0, 1.0 if r.top_p is None else r.top_p, ban,
+                                        r.seed, step).to(torch.int32)
+        r.prev[:, step] = nxt
+        r.out.append(nxt)
+        r.step = step + 1
+        self.tok_buf[first:first + 1] = nxt
+        return nxt == r.eos
+
+    # ---- retirement ----
+    def _output(self, r):
+        if r.kind == "beam":
+            return r.beams.result(r.step, 1).to(self.device)
+        toks = torch.stack(r.out, dim=1).to(torch.int64)
+        if r.kind == "greedy":
+            return generation._finish_rows(toks, r.eos, r.pad)
+        return toks
+
+    def _release(self, r):
+        if r in self.live:
+            self.live.remove(r)
+        for s in r.slots:
+            if self.owner[s] is r:
+                self.owner[s] = None
+        if r.num_beams > 1 and r.slots:                       # its rows of the re-parenting input go back to identity
+            self.src_buf[r.slots[0]:r.slots[-1] + 1] = self.ident[r.slots[0]:r.slots[-1] + 1]
+        held, r.engine_slots = r.engine_slots, []
+        if held:
+            try:
+                self.engine.leave(held)
+            except Exception:
+                pass
+
+    def _answer(self, r):
+        r.done.set()
+        if r.on_done is not None:
+            r.on_done(r)
+
+    def _retire(self, r):
+        try:
+            ids = self._output(r)
+            r.result = r.finish(ids) if r.finish is not None else ids
+        except Exception as ex:
+            r.error = ex
+        self._release(r)
+        self._answer(r)
+
+    def _fail(self, r, ex):
+        r.error = ex
+        self._release(r)
+        self._answer(r)
+
+    # ---- decode ----
+    def _decode(self):
+        B = max(s for r in self.live for s in r.slots) + 1
+        beams = any(r.num_beams > 1 for r in self.live)
+        try:
+            self.engine.llm_decode(token_ids=self.tok_buf, beam_src=self.src_buf if beams else None, logits=self.logits_buf, B=B)
+        except Exception as ex:       # an engine-level failure: every live request fails, the scheduler stays usable
+            for r in list(self.live):
+                self._fail(r, ex)
+            return
+        self.batch_sizes.append(B)
+        for r in self.live:
+            r.logits = self.logits_buf[r.slots[0]:r.slots[0] + r.num_beams]
+
+
+def _on_device(device):
+    """the engine enqueues on the current stream of the current device: make that the scheduler's device"""
+    import contextlib
+    return torch.cuda.device(device) if device.type == "cuda" else contextlib.nullcontext()
+
+
+def chat_request(chat, inputs, is_grounding=False, skip_special_tokens=True, **knobs):
+    """one EmuChatGeneration call (`chat(inputs, **knobs)`) as a SlotRequest whose result is the decoded answer: the same
+    prompt assembly, tokenisation and picture transform as `forward`, and the same `skip_special_tokens` decoding"""
+    model = chat.emu_model
+    text, image, video, iph, vph = chat.prepare(inputs, is_grounding)
+    input_ids, mask, IMAGE, VIDEO = model.tokenize_prompt(text, iph, vph)
+    tok = model.decoder.tokenizer
+    knobs = dict(knobs)
+    knobs.pop("synced_gpus", None)
+    return SlotRequest(input_ids, mask, image=image, video=video, image_token_id=IMAGE, video_token_id=VIDEO,
+                       finish=lambda ids: tok.batch_decode(ids, skip_special_tokens=skip_special_tokens)[0], **knobs)

@@ -25,7 +25,8 @@ def sources():
 
 def _digest():
     h = hashlib.sha256()
-    for f in sorted(os.listdir(CSRC)) + ["../../include/emu_b200.h", "../../include/emu_b200_safety.h"]:
+    for f in sorted(os.listdir(CSRC)) + ["../../include/emu_b200.h", "../../include/emu_b200_safety.h",
+                                        "../../include/emu_b200_slots.h"]:
         p = os.path.join(CSRC, f)
         if os.path.isfile(p):
             h.update(f.encode())

@@ -285,8 +285,9 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
   const int q0 = qb * kFaBM;
 
   const bf16* qp = a.q + (long)b * a.q_bs + (long)h * a.q_hs;
-  const bf16* kp = a.k + (long)b * a.k_bs + (long)h * a.k_hs;
-  const bf16* vp = a.v + (long)b * a.v_bs + (long)h * a.v_hs;
+  const int kvb = a.kv_row ? a.kv_row[b] : b;
+  const bf16* kp = a.k + (long)kvb * a.k_bs + (long)h * a.k_hs;
+  const bf16* vp = a.v + (long)kvb * a.v_bs + (long)h * a.v_hs;
   const int kv_lo = a.kv_start ? a.kv_start[b] : 0;
   const int shift = a.Nk - a.Nq;  // causal: key j visible to query i iff j <= i + shift
   int kv_hi = a.Nk;

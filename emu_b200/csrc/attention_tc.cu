@@ -46,6 +46,7 @@ struct AtParams {
   bf16* out;
   long o_bs, o_ts, o_hs;
   const int* kv_start;
+  const int* kv_row;  // [B] K/V batch coordinate of query batch b, or null = b
   int Nq, Nk, D;  // D = real head dim (<= DT)
   int causal;
   float scale_log2;  // scale * log2(e)
@@ -100,6 +101,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     // ===================== TMA producer =====================
     if (warp == 0 && lane == 0 && nb > 0) {
       if (p.pdl) pdl_wait();  // Q/K/V are the predecessor's output; all stores of this kernel happen after these loads
+      const int kvb = p.kv_row ? p.kv_row[batch] : batch;
       mbar_expect_tx(q_full, C::kQBytes);
       for (int c = 0; c < C::kDC; ++c) load_rows(smem + c * (128 * 128), &tmQ, q_full, c * 64, q0, head, batch, p.q_hf);
       for (int j = 0; j < nb; ++j) {
@@ -108,11 +110,11 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
         mbar_wait(&k_empty[s], ph ^ 1);
         mbar_expect_tx(&k_full[s], C::kKVBytes);
         for (int c = 0; c < C::kDC; ++c)
-          load_rows(smem + C::kOffK + s * C::kKVBytes + c * (BN * 128), &tmK, &k_full[s], c * 64, j * BN, head, batch, p.k_hf);
+          load_rows(smem + C::kOffK + s * C::kKVBytes + c * (BN * 128), &tmK, &k_full[s], c * 64, j * BN, head, kvb, p.k_hf);
         mbar_wait(&v_empty[s], ph ^ 1);
         mbar_expect_tx(&v_full[s], C::kKVBytes);
         for (int c = 0; c < C::kDC; ++c)
-          load_rows(smem + C::kOffV + s * C::kKVBytes + c * (BN * 128), &tmV, &v_full[s], c * 64, j * BN, head, batch, p.v_hf);
+          load_rows(smem + C::kOffV + s * C::kKVBytes + c * (BN * 128), &tmV, &v_full[s], c * 64, j * BN, head, kvb, p.v_hf);
       }
     }
   } else {
@@ -232,10 +234,11 @@ int launch_attn_tc(const AttnArgs& a, cudaStream_t st) {
   CUtensorMap tq, tk, tv;
   AtParams p;
   if (make_tmap_bnhd(&tq, a.q, a.D, a.Nq, a.H, a.B, a.q_ts, a.q_hs, a.q_bs, 128, &p.q_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
-  if (make_tmap_bnhd(&tk, a.k, a.D, a.Nk, a.H, a.B, a.k_ts, a.k_hs, a.k_bs, BN, &p.k_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
-  if (make_tmap_bnhd(&tv, a.v, a.D, a.Nk, a.H, a.B, a.v_ts, a.v_hs, a.v_bs, BN, &p.v_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
+  const int kvB = a.kv_row && a.kv_rows > 0 ? a.kv_rows : a.B;  // a row-mapped K/V map spans every cache row
+  if (make_tmap_bnhd(&tk, a.k, a.D, a.Nk, a.H, kvB, a.k_ts, a.k_hs, a.k_bs, BN, &p.k_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
+  if (make_tmap_bnhd(&tv, a.v, a.D, a.Nk, a.H, kvB, a.v_ts, a.v_hs, a.v_bs, BN, &p.v_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
   p.out = a.out; p.o_bs = a.o_bs; p.o_ts = a.o_ts; p.o_hs = a.o_hs;
-  p.kv_start = a.kv_start; p.Nq = a.Nq; p.Nk = a.Nk; p.D = a.D; p.causal = a.causal;
+  p.kv_start = a.kv_start; p.kv_row = a.kv_row; p.Nq = a.Nq; p.Nk = a.Nk; p.D = a.D; p.causal = a.causal;
   p.scale_log2 = a.scale * 1.4426950408889634f;
   p.pdl = g_pdl_chain;
   dim3 grid((a.Nq + 127) / 128, a.H, a.B);

@@ -197,9 +197,9 @@ int layernorm(const bf16* x, const bf16* w, const bf16* b, const bf16* residual,
 // ----------------------------------------------------------------------------------------------
 __global__ void rope_kv_write_kernel(bf16* qkv, int B, int N, int H, int D, const bf16* __restrict__ cos_t,
                                      const bf16* __restrict__ sin_t, const int* pos_off, int pos0, bf16* k_cache,
-                                     bf16* v_cache, int t_max, const int* __restrict__ pos_dev, bf16* q_out) {
+                                     bf16* v_cache, int t_max, const int* __restrict__ pos_dev, bf16* q_out,
+                                     const int* __restrict__ kv_row) {
   const int half = D >> 1;
-  if (pos_dev) pos0 = pos_dev[0];  // CUDA-graphed decode: the cache slot of the new token lives on the device
   const long total = (long)B * N * H * half;
   for (long idx = blockIdx.x * (long)blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
     const int j = idx % half;
@@ -207,7 +207,10 @@ __global__ void rope_kv_write_kernel(bf16* qkv, int B, int N, int H, int D, cons
     const int n = (idx / ((long)half * H)) % N;
     const int b = idx / ((long)half * H * N);
     bf16* base = qkv + ((long)b * N + n) * 3 * H * D;
-    int rp = pos0 + n - (pos_off ? pos_off[b] : 0);
+    // CUDA-graphed decode: the cache slot of every row's new token lives on the device (rows differ in slot mode)
+    const int p0 = pos_dev ? pos_dev[b] : pos0;
+    const int row = kv_row ? kv_row[b] : b;
+    int rp = p0 + n - (pos_off ? pos_off[b] : 0);
     rp = rp < 0 ? 0 : rp;
     const float c = __bfloat162float(cos_t[(long)rp * half + j]);
     const float s = __bfloat162float(sin_t[(long)rp * half + j]);
@@ -219,7 +222,7 @@ __global__ void rope_kv_write_kernel(bf16* qkv, int B, int N, int H, int D, cons
     *qd = pack_bf16(round_bf16(q1 * c) + round_bf16(-q2 * s), round_bf16(q2 * c) + round_bf16(q1 * s));
     const uint32_t kv = *reinterpret_cast<const uint32_t*>(base + (H + h) * D + 2 * j);
     const float k1 = bf16_lo(kv), k2 = bf16_hi(kv);
-    const long coff = (((long)b * H + h) * t_max + pos0 + n) * D + 2 * j;
+    const long coff = (((long)row * H + h) * t_max + p0 + n) * D + 2 * j;
     *reinterpret_cast<uint32_t*>(k_cache + coff) =
         pack_bf16(round_bf16(k1 * c) + round_bf16(-k2 * s), round_bf16(k2 * c) + round_bf16(k1 * s));
     *reinterpret_cast<uint32_t*>(v_cache + coff) = *reinterpret_cast<const uint32_t*>(base + (2 * H + h) * D + 2 * j);
@@ -227,10 +230,12 @@ __global__ void rope_kv_write_kernel(bf16* qkv, int B, int N, int H, int D, cons
 }
 
 int rope_kv_write(bf16* qkv, int B, int N, int H, int D, const bf16* cos_t, const bf16* sin_t, const int* pos_off,
-                  int pos0, bf16* k_cache, bf16* v_cache, int t_max, cudaStream_t st, const int* pos_dev, bf16* q_out) {
+                  int pos0, bf16* k_cache, bf16* v_cache, int t_max, cudaStream_t st, const int* pos_dev, bf16* q_out,
+                  const int* kv_row) {
   const long total = (long)B * N * H * (D / 2);
   const int grid = (int)((total + 255) / 256 < 4 * kNumSMs ? (total + 255) / 256 : 4 * kNumSMs);
-  rope_kv_write_kernel<<<grid, 256, 0, st>>>(qkv, B, N, H, D, cos_t, sin_t, pos_off, pos0, k_cache, v_cache, t_max, pos_dev, q_out);
+  rope_kv_write_kernel<<<grid, 256, 0, st>>>(qkv, B, N, H, D, cos_t, sin_t, pos_off, pos0, k_cache, v_cache, t_max, pos_dev, q_out,
+                                             kv_row);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
@@ -395,21 +400,22 @@ int kv_reorder(bf16* cache, int Bcap, const int* src_idx, int B, long outer, int
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
-__global__ void kv_indir_update_kernel(int* indir, const int* __restrict__ src_idx, int B, int t_max, int n_tok) {
+__global__ void kv_indir_update_kernel(int* indir, const int* __restrict__ src_idx, int B, int t_max, int n_tok,
+                                       const int* __restrict__ row_len) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= n_tok) return;
   int vals[32];
 #pragma unroll
   for (int b = 0; b < 32; ++b)
-    if (b < B) vals[b] = indir[(long)src_idx[b] * t_max + t];
+    if (b < B && (!row_len || t < row_len[b])) vals[b] = indir[(long)src_idx[b] * t_max + t];
 #pragma unroll
   for (int b = 0; b < 32; ++b)
-    if (b < B) indir[(long)b * t_max + t] = vals[b];
+    if (b < B && (!row_len || t < row_len[b])) indir[(long)b * t_max + t] = vals[b];
 }
-int kv_indir_update(int* indir, const int* src_idx, int B, int t_max, int n_tok, cudaStream_t st) {
+int kv_indir_update(int* indir, const int* src_idx, int B, int t_max, int n_tok, cudaStream_t st, const int* row_len) {
   if (B > 32) return EMU_ERR_INVALID;
   if (n_tok <= 0) return EMU_OK;
-  kv_indir_update_kernel<<<(n_tok + 127) / 128, 128, 0, st>>>(indir, src_idx, B, t_max, n_tok);
+  kv_indir_update_kernel<<<(n_tok + 127) / 128, 128, 0, st>>>(indir, src_idx, B, t_max, n_tok, row_len);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 __global__ void kv_indir_identity_kernel(int* indir, int rows, int t_max) {

@@ -6,6 +6,7 @@
 //   LLaMA    : HF LlamaModel.forward as driven by Emu2/emu/emu.py:133-138 (prefill, hidden_states[-1]) and
 //              :213-229 (generate: prefill + one-token steps with KV cache)
 #include "engine.h"
+#include "../../include/emu_b200_slots.h"
 
 #include <dlfcn.h>
 #include <math.h>
@@ -80,8 +81,9 @@ __global__ void rope_table_kernel(bf16* cos_t, bf16* sin_t, int max_pos, int hal
 __global__ void set_int_kernel(int* p, int n, int v) {
   if (threadIdx.x < n) p[threadIdx.x] = v;
 }
-__global__ void advance_pos_kernel(int* p, int n, unsigned* tp_step) {
-  if (threadIdx.x < n) p[threadIdx.x] += 1;
+// active: slot mode's live-row mask (a free slot's position stays 0), or null = every row
+__global__ void advance_pos_kernel(int* p, int n, unsigned* tp_step, const int* __restrict__ active) {
+  if (threadIdx.x < n) p[threadIdx.x] += active ? active[threadIdx.x] : 1;
   if (tp_step && threadIdx.x == 0) *tp_step += 1;  // decode-step counter behind the tensor-parallel exchange flags
 }
 // start[b] = number of leading zeros in mask row b; posoff[b] = hf ? start[b] : 0
@@ -92,6 +94,37 @@ __global__ void mask_start_kernel(const int* __restrict__ mask, int N, int* star
     while (s < N && mask[(long)b * N + s] == 0) ++s;
     start[b] = base + s;
     posoff[b] = hf ? base + s : 0;
+  }
+}
+// slot mode: the per-row state of a set of slots.  A join sets length `len`, the left-pad start / position offset from the
+// join-local arrays and marks the slot live; a leave (len 0, no arrays) zeroes and frees it.  Either way the slot's row of
+// the re-parenting table becomes identity (it may have belonged to a beam group).  One CTA per slot.
+struct SlotList {
+  int r[kLlmMaxRows];
+};
+__global__ void slot_set_kernel(SlotList rows, const int* __restrict__ src_start, const int* __restrict__ src_posoff, int len,
+                                int* pos, int* start, int* posoff, int* active, int* indir, int t_max) {
+  const int b = blockIdx.x, row = rows.r[b];
+  if (threadIdx.x == 0) {
+    pos[row] = len;
+    start[row] = src_start ? src_start[b] : 0;
+    posoff[row] = src_posoff ? src_posoff[b] : 0;
+    active[row] = len > 0 ? 1 : 0;
+  }
+  for (int t = threadIdx.x; t < t_max; t += blockDim.x) indir[(long)row * t_max + t] = row;
+}
+// slot mode: the slots dst continue slot src's sequence — its table row up to its length (identity beyond: a slot's own
+// new tokens are in its own row), its length, start and position offset.  One CTA per destination.
+__global__ void slot_fork_kernel(int src, SlotList dst, int* pos, int* start, int* posoff, int* active, int* indir, int t_max) {
+  const int row = dst.r[blockIdx.x];
+  const int len = pos[src];
+  for (int t = threadIdx.x; t < t_max; t += blockDim.x)
+    indir[(long)row * t_max + t] = t < len ? indir[(long)src * t_max + t] : row;
+  if (threadIdx.x == 0) {
+    pos[row] = len;
+    start[row] = start[src];
+    posoff[row] = posoff[src];
+    active[row] = 1;
   }
 }
 __global__ void argmax_ban_kernel(float* logits, int cols, int ban) {
@@ -296,6 +329,10 @@ extern "C" int emu_engine_create(const EmuConfig* cfg, int tp_rank, int tp_size,
     e->d_pos = (int*)e->dmalloc(3 * kLlmMaxRows * sizeof(int));
     e->d_start = e->d_pos + kLlmMaxRows;
     e->d_posoff = e->d_pos + 2 * kLlmMaxRows;
+    e->d_active = (int*)e->dmalloc(4 * kLlmMaxRows * sizeof(int));
+    e->d_join_rows = e->d_active + kLlmMaxRows;
+    e->d_join_start = e->d_active + 2 * kLlmMaxRows;
+    e->d_join_posoff = e->d_active + 3 * kLlmMaxRows;
     if (c.llm_max_batch > 8) {  // wide decode (more than 8 cache rows: the C4 workload, 4 prompts x 5 beams) runs on the GEMM path
       e->dec_xn = (bf16*)e->dmalloc((size_t)c.llm_max_batch * c.llm_hidden * 2);
       e->dec_qkv = (bf16*)e->dmalloc((size_t)c.llm_max_batch * 3 * e->Hl * c.llm_head_dim * 2);
@@ -326,7 +363,7 @@ extern "C" int emu_engine_create(const EmuConfig* cfg, int tp_rank, int tp_size,
     e->dec_logits_shard = (float*)e->dmalloc(((size_t)Bm * e->Vl + 4) * sizeof(float));
     e->dec_part = (float*)e->dmalloc((size_t)Bm * c.llm_hidden * sizeof(float));
     e->dec_logits_gather = (float*)e->dmalloc((size_t)Bm * e->Vl * tp_size * sizeof(float));
-    if (!e->rope_cos || !e->rope_sin || !e->kv || !e->d_pos || !e->dec_h || !e->dec_q || !e->dec_attn || !e->dec_act ||
+    if (!e->rope_cos || !e->rope_sin || !e->kv || !e->d_pos || !e->d_active || !e->dec_h || !e->dec_q || !e->dec_attn || !e->dec_act ||
         !e->dec_tmp || !e->dec_attn_ws || !e->dec_counters || !e->dec_logits_local || !e->kv_indir) {
       emu_engine_destroy(e);
       return EMU_ERR_NOMEM;
@@ -334,6 +371,7 @@ extern "C" int emu_engine_create(const EmuConfig* cfg, int tp_rank, int tp_size,
     rope_table_kernel<<<2 * kNumSMs, 256>>>(e->rope_cos, e->rope_sin, max_pos, half, c.llm_rope_theta);
     cudaMemset(e->dec_counters, 0, (size_t)Bm * e->Hl * sizeof(int));
     cudaMemset(e->d_pos, 0, 3 * kLlmMaxRows * sizeof(int));
+    cudaMemset(e->d_active, 0, 4 * kLlmMaxRows * sizeof(int));
     kv_indir_identity(e->kv_indir, Bm, c.llm_max_seq, 0);
   }
   if (c.vit_layers > 0) {
@@ -722,6 +760,9 @@ extern "C" int emu_llm_reset(EmuEngine* e, emu_stream_t s) {
   if (!e) return EMU_ERR_INVALID;
   e->cur_len = 0;
   e->cache_B = 0;
+  e->n_slots = 0;
+  e->slot_len.clear();
+  e->slot_group.clear();
   if (e->d_pos && cudaMemsetAsync(e->d_pos, 0, 3 * kLlmMaxRows * sizeof(int), (cudaStream_t)s) != cudaSuccess) return EMU_ERR_CUDA;
   if (e->kv_indir && e->kv_indir_dirty) {
     EMU_TRY(kv_indir_identity(e->kv_indir, e->cfg.llm_max_batch, e->cfg.llm_max_seq, (cudaStream_t)s));
@@ -752,6 +793,11 @@ static int kv_reparent(EmuEngine* e, const int32_t* src_idx, int B, cudaStream_t
     return kv_reorder(e->kv, c.llm_max_batch, src_idx, B, (long)c.llm_layers * 2, e->cur_len, e->Hl, c.llm_head_dim,
                       c.llm_max_seq, st);
   e->kv_indir_dirty = true;
+  if (e->n_slots > 0) {  // slots differ in length: every row copies its own, read from the device positions
+    int n_tok = 0;
+    for (int b = 0; b < B; ++b) n_tok = e->slot_len[b] > n_tok ? e->slot_len[b] : n_tok;
+    return kv_indir_update(e->kv_indir, src_idx, B, c.llm_max_seq, n_tok, st, e->d_pos);
+  }
   return kv_indir_update(e->kv_indir, src_idx, B, c.llm_max_seq, e->cur_len, st);
 }
 
@@ -759,6 +805,7 @@ extern "C" int emu_llm_expand(EmuEngine* e, const int32_t* src_idx, int new_B, e
   if (!e || !src_idx || new_B < 1) return EMU_ERR_INVALID;
   const EmuConfig& c = e->cfg;
   if (new_B > c.llm_max_batch) return e->fail(EMU_ERR_INVALID, "expanded batch exceeds llm_max_batch");
+  if (e->n_slots > 0) return e->fail(EMU_ERR_STATE, "expand in slot mode: use emu_llm_fork");
   if (e->cur_len < 1) return e->fail(EMU_ERR_STATE, "expand before prefill");
   cudaStream_t st = (cudaStream_t)stream;
   EMU_TRY(kv_reparent(e, src_idx, new_B, st));
@@ -793,41 +840,34 @@ extern "C" int emu_project(EmuEngine* e, int which, const void* x, int M, void* 
   return gemm_bf16((const bf16*)x, in, W, in, M, out, in, ep, st);
 }
 
-extern "C" int emu_llm_prefill(EmuEngine* e, const void* inputs_embeds, const int32_t* attention_mask, int B, int N,
-                               int hf_positions, void* last_hidden, float* logits_last, emu_stream_t stream) {
-  if (!e || !inputs_embeds || B < 1 || N < 1) return EMU_ERR_INVALID;
-  EMU_TRY(llm_ready(e));
+// prefill workspaces for M = B x N prompt tokens; the embeddings go to pf_h
+static int prefill_stage(EmuEngine* e, const void* inputs_embeds, long M, cudaStream_t st) {
   const EmuConfig& c = e->cfg;
-  cudaStream_t st = (cudaStream_t)stream;
-  PdlScope pdl_chain(1);
-  if (B > c.llm_max_batch) return e->fail(EMU_ERR_INVALID, "batch exceeds llm_max_batch");
-  if (e->cur_len + N > c.llm_max_seq) return e->fail(EMU_ERR_INVALID, "sequence exceeds llm_max_seq");
-  if (e->cur_len > 0 && B != e->cache_B) return e->fail(EMU_ERR_STATE, "batch differs from cached batch");
-  if (e->cur_len > 0 && e->kv_indir_dirty)
-    return e->fail(EMU_ERR_STATE, "a further prompt chunk after a beam re-parent needs EMU_KV_COPY=1 (the prefill attention reads rows directly)");
   const int Hd = c.llm_hidden, D = c.llm_head_dim, Hl = e->Hl, Fl = e->Fl;
-  const long M = (long)B * N;
-  const int pos0 = e->cur_len;
   EMU_TRY(e->ensure(e->pf_h, (size_t)M * Hd * 2));
   EMU_TRY(e->ensure(e->pf_xn, (size_t)M * Hd * 2));
   EMU_TRY(e->ensure(e->pf_qkv, (size_t)M * 3 * Hl * D * 2));
   EMU_TRY(e->ensure(e->pf_attn, (size_t)M * Hl * D * 2));
   EMU_TRY(e->ensure(e->pf_act, (size_t)M * Fl * 2));
   if (e->tp_size > 1) EMU_TRY(e->ensure(e->pf_tmp, (size_t)M * Hd * 2));
+  if (cudaMemcpyAsync(e->pf_h.p, inputs_embeds, (size_t)M * Hd * 2, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "embeds copy failed");
+  return EMU_OK;
+}
+
+// the decoder layers over the B x N prompt tokens in pf_h: k / v of batch b go to cache row kv_row[b] (null: row b) at
+// slots [pos0, pos0 + N), rotated at position slot - posoff[b]; the attention reads keys [start[b], pos0 + N) of that row
+static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start, const int* posoff, const int* kv_row,
+                          cudaStream_t st) {
+  const EmuConfig& c = e->cfg;
+  const int Hd = c.llm_hidden, D = c.llm_head_dim, Hl = e->Hl, Fl = e->Fl;
+  const long M = (long)B * N;
   bf16* h = (bf16*)e->pf_h.p;
   bf16* xn = (bf16*)e->pf_xn.p;
   bf16* qkv = (bf16*)e->pf_qkv.p;
   bf16* att = (bf16*)e->pf_attn.p;
   bf16* act = (bf16*)e->pf_act.p;
   bf16* tmp = (bf16*)e->pf_tmp.p;
-  if (cudaMemcpyAsync(h, inputs_embeds, (size_t)M * Hd * 2, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
-    return e->fail(EMU_ERR_CUDA, "embeds copy failed");
-  if (pos0 == 0) {
-    if (attention_mask) mask_start_kernel<<<B, 32, 0, st>>>(attention_mask, N, e->d_start, e->d_posoff, hf_positions, 0);
-    else cudaMemsetAsync(e->d_start, 0, 2 * kLlmMaxRows * sizeof(int), st);
-    count_launch();
-    e->cache_B = B;
-  }
   const float scale = 1.0f / sqrtf((float)D);
   for (int l = 0; l < c.llm_layers; ++l) {
     const LlmLayer& L = e->layers[l];
@@ -837,13 +877,15 @@ extern "C" int emu_llm_prefill(EmuEngine* e, const void* inputs_embeds, const in
     GemmEpilogue ep;
     ep.C = qkv; ep.ldc = 3 * Hl * D;
     EMU_TRY(gemm_bf16(xn, Hd, L.wqkv, Hd, (int)M, 3 * Hl * D, Hd, ep, st));
-    EMU_TRY(rope_kv_write(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, e->d_posoff, pos0, kc, vc, c.llm_max_seq, st));
+    EMU_TRY(rope_kv_write(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, pos0, kc, vc, c.llm_max_seq, st, nullptr, nullptr,
+                          kv_row));
     AttnArgs a;
     a.q = qkv; a.q_bs = (long)N * 3 * Hl * D; a.q_ts = 3 * Hl * D; a.q_hs = D;
     a.k = kc; a.k_bs = (long)Hl * c.llm_max_seq * D; a.k_hs = (long)c.llm_max_seq * D; a.k_ts = D;
     a.v = vc; a.v_bs = a.k_bs; a.v_hs = a.k_hs; a.v_ts = D;
     a.out = att; a.o_bs = (long)N * Hl * D; a.o_ts = Hl * D; a.o_hs = D;
-    a.B = B; a.H = Hl; a.Nq = N; a.Nk = pos0 + N; a.D = D; a.scale = scale; a.causal = 1; a.kv_start = e->d_start;
+    a.B = B; a.H = Hl; a.Nq = N; a.Nk = pos0 + N; a.D = D; a.scale = scale; a.causal = 1; a.kv_start = start;
+    a.kv_row = kv_row; a.kv_rows = kv_row ? c.llm_max_batch : 0;
     EMU_TRY(attn_prefill(a, st));
     if (e->tp_size == 1) {
       GemmEpilogue eo;
@@ -875,9 +917,15 @@ extern "C" int emu_llm_prefill(EmuEngine* e, const void* inputs_embeds, const in
     }
     count_launch(8);
   }
-  e->cur_len = pos0 + N;
-  set_int_kernel<<<1, 32, 0, st>>>(e->d_pos, kLlmMaxRows, e->cur_len);  // slot of the next token
-  count_launch();
+  return EMU_OK;
+}
+
+// final norm of every prompt token (last_hidden) and the logits of every sequence's last position (logits_last)
+static int prefill_outputs(EmuEngine* e, int B, int N, void* last_hidden, float* logits_last, cudaStream_t st) {
+  const EmuConfig& c = e->cfg;
+  const int Hd = c.llm_hidden;
+  const long M = (long)B * N;
+  bf16* h = (bf16*)e->pf_h.p;
   if (last_hidden) {
     EMU_TRY(rmsnorm(h, e->final_norm, (bf16*)last_hidden, (int)M, Hd, c.llm_rms_eps, 0, st));
     count_launch();
@@ -920,6 +968,34 @@ extern "C" int emu_llm_prefill(EmuEngine* e, const void* inputs_embeds, const in
     count_launch();
   }
   return EMU_OK;
+}
+
+extern "C" int emu_llm_prefill(EmuEngine* e, const void* inputs_embeds, const int32_t* attention_mask, int B, int N,
+                               int hf_positions, void* last_hidden, float* logits_last, emu_stream_t stream) {
+  if (!e || !inputs_embeds || B < 1 || N < 1) return EMU_ERR_INVALID;
+  EMU_TRY(llm_ready(e));
+  const EmuConfig& c = e->cfg;
+  cudaStream_t st = (cudaStream_t)stream;
+  PdlScope pdl_chain(1);
+  if (e->n_slots > 0) return e->fail(EMU_ERR_STATE, "prefill in slot mode: use emu_llm_join (emu_llm_reset leaves slot mode)");
+  if (B > c.llm_max_batch) return e->fail(EMU_ERR_INVALID, "batch exceeds llm_max_batch");
+  if (e->cur_len + N > c.llm_max_seq) return e->fail(EMU_ERR_INVALID, "sequence exceeds llm_max_seq");
+  if (e->cur_len > 0 && B != e->cache_B) return e->fail(EMU_ERR_STATE, "batch differs from cached batch");
+  if (e->cur_len > 0 && e->kv_indir_dirty)
+    return e->fail(EMU_ERR_STATE, "a further prompt chunk after a beam re-parent needs EMU_KV_COPY=1 (the prefill attention reads rows directly)");
+  const int pos0 = e->cur_len;
+  EMU_TRY(prefill_stage(e, inputs_embeds, (long)B * N, st));
+  if (pos0 == 0) {
+    if (attention_mask) mask_start_kernel<<<B, 32, 0, st>>>(attention_mask, N, e->d_start, e->d_posoff, hf_positions, 0);
+    else cudaMemsetAsync(e->d_start, 0, 2 * kLlmMaxRows * sizeof(int), st);
+    count_launch();
+    e->cache_B = B;
+  }
+  EMU_TRY(prefill_layers(e, B, N, pos0, e->d_start, e->d_posoff, nullptr, st));
+  e->cur_len = pos0 + N;
+  set_int_kernel<<<1, 32, 0, st>>>(e->d_pos, kLlmMaxRows, e->cur_len);  // slot of the next token
+  count_launch();
+  return prefill_outputs(e, B, N, last_hidden, logits_last, st);
 }
 
 // tensor-parallel tail of a row-parallel projection (o_proj / down_proj) in the decode loop: h += sum over ranks of W_r x_r.
@@ -1074,7 +1150,7 @@ static int decode_step_body_wide(EmuEngine* e, const int32_t* token_ids, const v
       ++nl;
     }
   }
-  advance_pos_kernel<<<1, 32, 0, st>>>(e->d_pos, kLlmMaxRows, tp_step_counter(e));
+  advance_pos_kernel<<<1, 32, 0, st>>>(e->d_pos, kLlmMaxRows, tp_step_counter(e), e->n_slots > 0 ? e->d_active : nullptr);
   ++nl;
   *n_launch = nl;
   return EMU_OK;
@@ -1167,7 +1243,7 @@ static int decode_step_body(EmuEngine* e, const int32_t* token_ids, const void* 
       ++nl;
     }
   }
-  advance_pos_kernel<<<1, 32, 0, st>>>(e->d_pos, kLlmMaxRows, tp_step_counter(e));
+  advance_pos_kernel<<<1, 32, 0, st>>>(e->d_pos, kLlmMaxRows, tp_step_counter(e), e->n_slots > 0 ? e->d_active : nullptr);
   ++nl;
   *n_launch = nl;
   return EMU_OK;
@@ -1179,9 +1255,22 @@ extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void
   EMU_TRY(llm_ready(e));
   const EmuConfig& c = e->cfg;
   cudaStream_t st = (cudaStream_t)stream;
-  if (e->cur_len < 1) return e->fail(EMU_ERR_STATE, "decode before prefill");
-  if (B != e->cache_B) return e->fail(EMU_ERR_STATE, "batch differs from cached batch");
-  if (e->cur_len + 1 > c.llm_max_seq) return e->fail(EMU_ERR_INVALID, "KV cache full");
+  if (e->n_slots > 0) {
+    int hi = -1;
+    for (int b = 0; b < e->n_slots; ++b)
+      if (e->slot_group[b] >= 0) hi = b;
+    if (hi < 0) return e->fail(EMU_ERR_STATE, "decode with no live slot");
+    if (B <= hi || B > e->n_slots)
+      return e->fail(EMU_ERR_INVALID, "slot mode: B = " + std::to_string(B) + " must cover the highest live slot " +
+                                          std::to_string(hi) + " and stay within " + std::to_string(e->n_slots) + " slots");
+    for (int b = 0; b < B; ++b)
+      if (e->slot_group[b] >= 0 && e->slot_len[b] + 1 > c.llm_max_seq)
+        return e->fail(EMU_ERR_INVALID, "KV cache full at slot " + std::to_string(b));
+  } else {
+    if (e->cur_len < 1) return e->fail(EMU_ERR_STATE, "decode before prefill");
+    if (B != e->cache_B) return e->fail(EMU_ERR_STATE, "batch differs from cached batch");
+    if (e->cur_len + 1 > c.llm_max_seq) return e->fail(EMU_ERR_INVALID, "KV cache full");
+  }
   if (beam_src_idx) {
     EMU_TRY(kv_reparent(e, beam_src_idx, B, st));
     count_launch();
@@ -1193,7 +1282,7 @@ extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void
     EMU_TRY(decode_step_body(e, token_ids, embeds, B, logits, hidden, next_ids, ban_id, st, &nl));
     count_launch(nl);
   } else {
-    EmuEngine::GraphKey key(B, token_ids, embeds, logits, hidden, next_ids, (const void*)st, ban_id);
+    EmuEngine::GraphKey key(B, token_ids, embeds, logits, hidden, next_ids, (const void*)st, ban_id, e->n_slots > 0 ? 1 : 0);
     auto it = e->graphs.find(key);
     if (it == e->graphs.end()) {
       if (e->graphs.size() > 64) {
@@ -1226,6 +1315,137 @@ extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void
     if (cudaGraphLaunch(it->second, st) != cudaSuccess) return e->fail(EMU_ERR_CUDA, "graph launch failed");
     count_launch(e->graph_nodes[key]);
   }
-  e->cur_len += 1;
+  if (e->n_slots > 0) {
+    for (int b = 0; b < B; ++b)
+      if (e->slot_group[b] >= 0) e->slot_len[b] += 1;
+  } else {
+    e->cur_len += 1;
+  }
   return EMU_OK;
+}
+
+// ================================================================================================
+// slot mode: continuous batching (include/emu_b200_slots.h)
+// ================================================================================================
+static int slot_mode_ok(EmuEngine* e) {
+  if (e->cfg.llm_layers < 1) return e->fail(EMU_ERR_STATE, "engine has no LLM");
+  if (e->n_slots < 1) return e->fail(EMU_ERR_STATE, "not in slot mode (emu_llm_slots_begin)");
+  return EMU_OK;
+}
+
+// a host slot list: n in [1, n_slots], every index in range, distinct, and free (want_free) or live
+static int check_slots(EmuEngine* e, const int32_t* slots, int n, bool want_free, SlotList* out) {
+  if (n < 1 || n > e->n_slots) return e->fail(EMU_ERR_INVALID, "slot count " + std::to_string(n) + " out of range");
+  for (int i = 0; i < n; ++i) {
+    const int s = slots[i];
+    if (s < 0 || s >= e->n_slots)
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " out of range [0, " + std::to_string(e->n_slots) + ")");
+    for (int j = 0; j < i; ++j)
+      if (slots[j] == s) return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " named twice");
+    if (want_free && e->slot_group[s] >= 0) return e->fail(EMU_ERR_STATE, "slot " + std::to_string(s) + " is occupied");
+    if (!want_free && e->slot_group[s] < 0) return e->fail(EMU_ERR_STATE, "slot " + std::to_string(s) + " is free");
+    out->r[i] = s;
+  }
+  return EMU_OK;
+}
+
+extern "C" int emu_llm_slots_begin(EmuEngine* e, int n_slots, emu_stream_t s) {
+  if (!e) return EMU_ERR_INVALID;
+  const EmuConfig& c = e->cfg;
+  if (c.llm_layers < 1) return e->fail(EMU_ERR_STATE, "engine has no LLM");
+  if (n_slots < 1 || n_slots > c.llm_max_batch)
+    return e->fail(EMU_ERR_INVALID, "n_slots = " + std::to_string(n_slots) + " must be in [1, llm_max_batch = " +
+                                        std::to_string(c.llm_max_batch) + "]");
+  if (e->tp_size > 1) return e->fail(EMU_ERR_UNSUPPORTED, "slot mode under tensor parallelism");
+  if (e->kv_copy) return e->fail(EMU_ERR_UNSUPPORTED, "slot mode with EMU_KV_COPY=1 (slots re-parent through the row table)");
+  EMU_TRY(emu_llm_reset(e, s));
+  if (cudaMemsetAsync(e->d_active, 0, kLlmMaxRows * sizeof(int), (cudaStream_t)s) != cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "slot state reset failed");
+  e->n_slots = n_slots;
+  e->slot_len.assign(n_slots, 0);
+  e->slot_group.assign(n_slots, -1);
+  e->kv_indir_dirty = true;  // joins, forks and leaves rewrite table rows: emu_llm_reset restores the identity
+  return EMU_OK;
+}
+
+extern "C" int emu_llm_join(EmuEngine* e, const int32_t* host_slots, int n, const void* inputs_embeds,
+                            const int32_t* attention_mask, int N, float* logits_last, emu_stream_t stream) {
+  if (!e || !host_slots || !inputs_embeds || n < 1 || N < 1) return EMU_ERR_INVALID;
+  EMU_TRY(slot_mode_ok(e));
+  EMU_TRY(llm_ready(e));
+  const EmuConfig& c = e->cfg;
+  if (N > c.llm_max_seq) return e->fail(EMU_ERR_INVALID, "prompt of " + std::to_string(N) + " tokens exceeds llm_max_seq");
+  SlotList rows;
+  EMU_TRY(check_slots(e, host_slots, n, true, &rows));
+  cudaStream_t st = (cudaStream_t)stream;
+  PdlScope pdl_chain(1);
+  if (cudaMemcpyAsync(e->d_join_rows, rows.r, n * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "slot list upload failed");
+  EMU_TRY(prefill_stage(e, inputs_embeds, (long)n * N, st));
+  // left-pad starts and HF position offsets of the joining sequences, join-local; scattered to their slots below
+  if (attention_mask) mask_start_kernel<<<n, 32, 0, st>>>(attention_mask, N, e->d_join_start, e->d_join_posoff, 1, 0);
+  else cudaMemsetAsync(e->d_join_start, 0, 2 * kLlmMaxRows * sizeof(int), st);
+  count_launch();
+  EMU_TRY(prefill_layers(e, n, N, 0, e->d_join_start, e->d_join_posoff, e->d_join_rows, st));
+  slot_set_kernel<<<n, 256, 0, st>>>(rows, e->d_join_start, e->d_join_posoff, N, e->d_pos, e->d_start, e->d_posoff, e->d_active,
+                                     e->kv_indir, c.llm_max_seq);
+  count_launch();
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot join failed");
+  for (int i = 0; i < n; ++i) {
+    e->slot_len[rows.r[i]] = N;
+    e->slot_group[rows.r[i]] = rows.r[i];
+  }
+  return prefill_outputs(e, n, N, nullptr, logits_last, st);
+}
+
+extern "C" int emu_llm_fork(EmuEngine* e, int src_slot, const int32_t* host_dst_slots, int n, emu_stream_t stream) {
+  if (!e || !host_dst_slots || n < 1) return EMU_ERR_INVALID;
+  EMU_TRY(slot_mode_ok(e));
+  if (src_slot < 0 || src_slot >= e->n_slots) return e->fail(EMU_ERR_INVALID, "source slot " + std::to_string(src_slot) + " out of range");
+  if (e->slot_group[src_slot] < 0) return e->fail(EMU_ERR_STATE, "source slot " + std::to_string(src_slot) + " is free");
+  SlotList dst;
+  EMU_TRY(check_slots(e, host_dst_slots, n, true, &dst));
+  const EmuConfig& c = e->cfg;
+  slot_fork_kernel<<<n, 256, 0, (cudaStream_t)stream>>>(src_slot, dst, e->d_pos, e->d_start, e->d_posoff, e->d_active, e->kv_indir,
+                                                        c.llm_max_seq);
+  count_launch();
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot fork failed");
+  for (int i = 0; i < n; ++i) {
+    e->slot_len[dst.r[i]] = e->slot_len[src_slot];
+    e->slot_group[dst.r[i]] = e->slot_group[src_slot];
+  }
+  return EMU_OK;
+}
+
+extern "C" int emu_llm_leave(EmuEngine* e, const int32_t* host_slots, int n, emu_stream_t stream) {
+  if (!e || !host_slots || n < 1) return EMU_ERR_INVALID;
+  EMU_TRY(slot_mode_ok(e));
+  SlotList rows;
+  EMU_TRY(check_slots(e, host_slots, n, false, &rows));
+  // a beam group leaves together: its slots' table rows point into each other
+  for (int b = 0; b < e->n_slots; ++b) {
+    if (e->slot_group[b] < 0) continue;
+    bool named = false, group_named = false;
+    for (int i = 0; i < n; ++i) {
+      named |= rows.r[i] == b;
+      group_named |= e->slot_group[rows.r[i]] == e->slot_group[b];
+    }
+    if (group_named && !named)
+      return e->fail(EMU_ERR_STATE, "slot " + std::to_string(b) + " belongs to a leaving beam group and must leave with it");
+  }
+  const EmuConfig& c = e->cfg;
+  slot_set_kernel<<<n, 256, 0, (cudaStream_t)stream>>>(rows, nullptr, nullptr, 0, e->d_pos, e->d_start, e->d_posoff, e->d_active,
+                                                       e->kv_indir, c.llm_max_seq);
+  count_launch();
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot leave failed");
+  for (int i = 0; i < n; ++i) {
+    e->slot_len[rows.r[i]] = 0;
+    e->slot_group[rows.r[i]] = -1;
+  }
+  return EMU_OK;
+}
+
+extern "C" int emu_llm_slot_len(EmuEngine* e, int slot) {
+  if (!e || e->n_slots < 1 || slot < 0 || slot >= e->n_slots) return -1;
+  return e->slot_len[slot];
 }

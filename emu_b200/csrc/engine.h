@@ -85,8 +85,15 @@ struct EmuEngine {
   float *dec_logits_shard = nullptr, *dec_logits_gather = nullptr;
   // prefill workspaces (grown on demand)
   emu::DevBuf pf_h, pf_xn, pf_qkv, pf_attn, pf_act, pf_tmp, pf_last;
-  // decode graphs keyed by the baked-in arguments
-  typedef std::tuple<int, const void*, const void*, const void*, const void*, const void*, const void*, int> GraphKey;
+  // slot mode (continuous batching, include/emu_b200_slots.h): every cache row is a slot holding its own sequence
+  int n_slots = 0;               // > 0: slot mode with this many slots
+  std::vector<int> slot_len;     // host mirror of d_pos per slot (0 = free)
+  std::vector<int> slot_group;   // first slot of the slot's beam group, -1 = free
+  int* d_active = nullptr;       // [kLlmMaxRows] 1 = live slot: the decode step advances its position
+  int* d_join_rows = nullptr;    // [kLlmMaxRows] cache rows of the sequences being joined
+  int *d_join_start = nullptr, *d_join_posoff = nullptr;  // [kLlmMaxRows] their left-pad starts / position offsets
+  // decode graphs keyed by the baked-in arguments (the last int: slot mode, whose step advances live rows only)
+  typedef std::tuple<int, const void*, const void*, const void*, const void*, const void*, const void*, int, int> GraphKey;
   std::map<GraphKey, cudaGraphExec_t> graphs;
   std::map<GraphKey, int> graph_nodes;
   bool use_graphs = true;

@@ -114,6 +114,10 @@ struct AttnArgs {
   int causal = 0;                 // query i attends keys j <= i + (Nk - Nq)
   const int* kv_start = nullptr;  // [B] first valid key (left padding) or null
   const float* bias = nullptr;    // [H, Nq, Nk] additive (T5 relative position bias) or null
+  // [B] batch index of k / v read by query batch b (a join prefills new sequences into chosen KV-cache rows), or null =
+  // b itself; kv_rows = how many batch entries the k / v views span (0 = B)
+  const int* kv_row = nullptr;
+  int kv_rows = 0;
 };
 int attn_prefill(const AttnArgs& a, cudaStream_t st);
 int attn_prefill_tc(const AttnArgs& a, cudaStream_t st);  // attention_tc.cu; EMU_ERR_UNSUPPORTED -> use attn_prefill's own kernel
@@ -150,8 +154,9 @@ int layernorm(const bf16* x, const bf16* w, const bf16* b, const bf16* residual,
               cudaStream_t st);  // y = residual + LN(x)  (residual may be null)
 int rope_kv_write(bf16* qkv /*[B,N,3*H*D] pair-interleaved q,k*/, int B, int N, int H, int D, const bf16* cos,
                   const bf16* sin, const int* pos_off /*[B]*/, int pos0, bf16* k_cache, bf16* v_cache, int t_max,
-                  cudaStream_t st, const int* pos_dev = nullptr /*device slot of the new token (N == 1), overrides pos0*/,
-                  bf16* q_out = nullptr /*decode: the rotated q goes compact [B*N, H*D] here instead of in place*/);
+                  cudaStream_t st, const int* pos_dev = nullptr /*[B] device slot of the new token (N == 1), overrides pos0*/,
+                  bf16* q_out = nullptr /*decode: the rotated q goes compact [B*N, H*D] here instead of in place*/,
+                  const int* kv_row = nullptr /*[B] cache row of batch b (join into chosen rows), null = b*/);
 int embed_gather(const bf16* table, const int* ids, bf16* out, int n, int dim, cudaStream_t st);
 int argmax_rows(const float* logits, int rows, int cols, int* out_idx, cudaStream_t st);
 int vit_im2col(const bf16* img_nchw, bf16* out, int B, int C, int HW, int P, int Kpad, cudaStream_t st);
@@ -161,8 +166,10 @@ int vit_pool(const bf16* x /*[B,1+G*G,dim]*/, bf16* out /*[B,n_query,dim]*/, int
              cudaStream_t st);
 int kv_reorder(bf16* cache /*[outer][Bcap][H][t_max][D]*/, int Bcap, const int* src_idx, int B, long outer,
                int n_used_tokens, int H, int D, int t_max, cudaStream_t st);
-// beam re-parenting without moving the cache: indir[b][t] <- indir[src[b]][t] for t < n_tok (in place, column-wise)
-int kv_indir_update(int* indir /*[rows][t_max]*/, const int* src_idx, int B, int t_max, int n_tok, cudaStream_t st);
+// beam re-parenting without moving the cache: indir[b][t] <- indir[src[b]][t] for t < n_tok (in place, column-wise);
+// with row_len (device [B], the cached length of every row) row b copies only t < row_len[b]
+int kv_indir_update(int* indir /*[rows][t_max]*/, const int* src_idx, int B, int t_max, int n_tok, cudaStream_t st,
+                    const int* row_len = nullptr);
 int kv_indir_identity(int* indir, int rows, int t_max, cudaStream_t st);
 int add_rows(const bf16* a, const bf16* b, bf16* out, long n, cudaStream_t st);
 

@@ -35,16 +35,7 @@ class EmuChatGeneration:
                 top_p: Optional[float] = None, top_k: Optional[int] = None, temperature: Optional[float] = None,
                 length_penalty: float = -1, repetition_penalty: float = 1.0, synced_gpus: bool = False,
                 skip_special_tokens: bool = True, **kwargs):
-        assert isinstance(inputs, list), "inputs must be a list"
-        device, dtype = self.emu_model.device(), self.emu_model.dtype()
-        if isinstance(inputs[0], list):
-            assert len(inputs) % 2 == 1, "last message must be user input"
-            prep = self._prepare_chat_inputs(inputs, is_grounding, device, dtype)
-        else:
-            assert all(isinstance(i, (str, Image.Image)) for i in inputs), \
-                "input can't be list of list for normal generation"
-            prep = self._prepare_inputs(inputs, device, dtype)
-        text_prompt, image_prompt, video_prompt, image_placeholder, video_placeholder = prep
+        text_prompt, image_prompt, video_prompt, image_placeholder, video_placeholder = self.prepare(inputs, is_grounding)
         output = self.emu_model.generate(
             text=text_prompt, image=image_prompt, video=video_prompt, image_placeholder=image_placeholder,
             video_placeholder=video_placeholder, num_beams=num_beams, max_new_tokens=max_new_tokens, min_len=min_len,
@@ -54,6 +45,18 @@ class EmuChatGeneration:
         return output[0]
 
     __call__ = forward
+
+    def prepare(self, inputs, is_grounding: bool = False):
+        """one request's `inputs` (a plain list of strings and pictures, or chat turns) -> (prompt texts [1], image
+        [n, 3, S, S] | None, video | None, image placeholder, video placeholder): what `forward` hands to
+        EmuModel.generate, also used by the continuous-batching scheduler (emu_b200/batching.py)"""
+        assert isinstance(inputs, list), "inputs must be a list"
+        device, dtype = self.emu_model.device(), self.emu_model.dtype()
+        if isinstance(inputs[0], list):
+            assert len(inputs) % 2 == 1, "last message must be user input"
+            return self._prepare_chat_inputs(inputs, is_grounding, device, dtype)
+        assert all(isinstance(i, (str, Image.Image)) for i in inputs), "input can't be list of list for normal generation"
+        return self._prepare_inputs(inputs, device, dtype)
 
     @torch.no_grad()
     def forward_batch(self, batch_inputs, is_grounding: bool = False, num_beams: int = 5, max_new_tokens: int = 10,

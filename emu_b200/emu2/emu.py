@@ -155,16 +155,39 @@ class EmuModel:
                  top_k=None, temperature=None, length_penalty=-1, repetition_penalty=1.0, synced_gpus=False,
                  skip_special_tokens=True, **kwargs):
         tok = self.decoder.tokenizer
-        IMAGE, VIDEO = tok.convert_tokens_to_ids([DEFAULT_IMAGE_TOKEN, DEFAULT_gIMG_TOKEN])
-        text = [t.replace(image_placeholder, self.image_placeholder).replace(video_placeholder, self.video_placeholder)
-                for t in text]
-        input_ids, attention_mask = self._tokenize(text)
+        input_ids, attention_mask, IMAGE, VIDEO = self.tokenize_prompt(text, image_placeholder, video_placeholder)
         outputs = self.generate_from_ids(input_ids, attention_mask, image=image, video=video, image_token_id=IMAGE,
                                          video_token_id=VIDEO, num_beams=num_beams, max_new_tokens=max_new_tokens,
                                          min_len=min_len, do_sample=do_sample, penalty_alpha=penalty_alpha, top_p=top_p,
                                          top_k=top_k, temperature=temperature, length_penalty=length_penalty,
                                          repetition_penalty=repetition_penalty, **kwargs)
         return tok.batch_decode(outputs, skip_special_tokens=skip_special_tokens)
+
+    def tokenize_prompt(self, text: List[str], image_placeholder: str = DEFAULT_IMG_PLACEHOLDER,
+                        video_placeholder: str = DEFAULT_VID_PLACEHOLDER):
+        """the prompt texts with their picture placeholders expanded to the query slots, tokenised (left padded) ->
+        (input_ids, attention_mask, <image> token id, [gIMG] token id) — the first half of `generate`"""
+        tok = self.decoder.tokenizer
+        IMAGE, VIDEO = tok.convert_tokens_to_ids([DEFAULT_IMAGE_TOKEN, DEFAULT_gIMG_TOKEN])
+        text = [t.replace(image_placeholder, self.image_placeholder).replace(video_placeholder, self.video_placeholder)
+                for t in text]
+        input_ids, attention_mask = self._tokenize(text)
+        return input_ids, attention_mask, IMAGE, VIDEO
+
+    @torch.no_grad()
+    def embed_prompt(self, input_ids, image=None, video=None, image_token_id=32003, video_token_id=32004):
+        """token embeddings [B, N, hidden] with the projected ViT tokens of the pictures / video frames spliced into their
+        slots, in order (Emu2/emu/emu.py:193-203)"""
+        text_embeds = self.engine.llm_embed(input_ids)  # [B, N, H]
+        if image is not None:
+            e = self.encode_image(image, n_query=self.n_query)
+            e = self._project_up(e.reshape(-1, e.shape[-1]))
+            text_embeds[input_ids == image_token_id] = e
+        if video is not None:
+            e = self.encode_image(video, n_query=self.v_query)
+            e = self._project_up(e.reshape(-1, e.shape[-1]))
+            text_embeds[input_ids == video_token_id] = e
+        return text_embeds
 
     @torch.no_grad()
     def generate_from_ids(self, input_ids, attention_mask, image=None, video=None, image_token_id=32003,
@@ -177,15 +200,7 @@ class EmuModel:
         pad = pad_token_id if pad_token_id is not None else tok.pad_token_id
         input_ids = input_ids.to(self.device_)
         attention_mask = attention_mask.to(self.device_)
-        text_embeds = self.engine.llm_embed(input_ids)  # [B, N, H]
-        if image is not None:
-            e = self.encode_image(image, n_query=self.n_query)
-            e = self._project_up(e.reshape(-1, e.shape[-1]))
-            text_embeds[input_ids == image_token_id] = e
-        if video is not None:
-            e = self.encode_image(video, n_query=self.v_query)
-            e = self._project_up(e.reshape(-1, e.shape[-1]))
-            text_embeds[input_ids == video_token_id] = e
+        text_embeds = self.embed_prompt(input_ids, image, video, image_token_id, video_token_id)
         # strategy selection as GenerationMixin does it from these knobs; the extra HF knobs the reference lets through its
         # **kwargs (no_repeat_ngram_size, prefix_allowed_tokens_fn, num_return_sequences, early_stopping) are honoured too
         return generation.generate(self.engine, text_embeds, attention_mask, max_new_tokens, eos, pad, do_sample=do_sample,

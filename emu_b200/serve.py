@@ -18,6 +18,10 @@ decoding knobs when the pipeline becomes free is sent through ONE `forward_batch
 so concurrent requests share each weight pass.  Admission is per generate call, not per decode step: the engine advances all
 cache rows in lock-step (one `cur_len`), so a request cannot join a batch that is already decoding — it waits for the next one.
 
+Opt-in continuous batching for chat (`EmuServer(chat_scheduler="continuous")`, `--continuous-batching`): a ContinuousWorker
+runs the pipeline's model under emu_b200/batching.py's SlotScheduler instead — requests join the decode batch between two
+steps and leave it as soon as they are finished, each with its own knobs.  Single GPU only.
+
 With tensor parallelism (launched under torchrun, one process per GPU) rank 0 serves HTTP and broadcasts every admitted batch;
 the other ranks run `follow()` and execute the same calls, which is what the engine's collectives need.
 
@@ -78,6 +82,10 @@ class BatchingWorker(threading.Thread):
         self._halt = threading.Event()
 
     # ---- producer side (HTTP handler threads) ----
+    def load(self):
+        """requests waiting in front of this worker (EmuServer sends a request to the least loaded one)"""
+        return self.q.qsize() + len(self.held)
+
     def submit(self, inputs, knobs, log_id="", timeout=None):
         r = _Request(inputs, knobs, log_id)
         self.q.put(r)
@@ -157,6 +165,86 @@ class BatchingWorker(threading.Thread):
                 r.done.set()
 
 
+class ContinuousWorker(threading.Thread):
+    """One chat pipeline (an EmuChatGeneration) under continuous batching: its thread owns the pipeline's engine and loops
+    SlotScheduler.step() while anything is live or queued, and blocks on the queue when idle.  Same submit / stop surface as
+    BatchingWorker.  A request that fails (prompt assembly, embedding, selection) answers with its own error and frees its
+    slots; the others continue.  `n_slots`: KV-cache slots (default: the engine's llm_max_batch).  `make_request(pipeline,
+    inputs, knobs) -> SlotRequest` turns a submitted request into scheduler work (default: batching.chat_request)."""
+
+    def __init__(self, pipeline, n_slots=None, name=None, make_request=None):
+        super().__init__(daemon=True, name=name or "emu-chat-continuous")
+        self.pipeline, self.n_slots = pipeline, n_slots
+        self.make_request = make_request
+        self.kind = "chat"
+        self.q = queue.Queue()
+        self.scheduler = None
+        self._halt = threading.Event()
+
+    def start(self):
+        """enter slot mode before the thread starts: an engine that cannot (EMU_KV_COPY=1, tensor parallel) fails here, in
+        the caller, instead of leaving a dead worker behind a queue"""
+        from .batching import SlotScheduler
+        self.scheduler = SlotScheduler(self.pipeline.emu_model, self.n_slots)
+        super().start()
+
+    def load(self):
+        """queued + waiting for slots + decoding"""
+        return self.q.qsize() + (self.scheduler.load() if self.scheduler is not None else 0)
+
+    def submit(self, inputs, knobs, log_id="", timeout=None):
+        r = _Request(inputs, knobs, log_id)
+        self.q.put(r)
+        if not r.done.wait(timeout):
+            raise TimeoutError("request %s timed out" % log_id)
+        if r.error is not None:
+            raise r.error
+        return r.result
+
+    def stop(self):
+        self._halt.set()
+        self.q.put(None)
+
+    def _admit(self, r):
+        from .batching import chat_request
+        make = self.make_request or (lambda pipe, inputs, knobs: chat_request(pipe, inputs, **knobs))
+
+        def answer(sr, r=r):
+            r.result, r.error = sr.result, sr.error
+            log.info("%s: chat done in %.1f ms", r.log_id, (time.time() - r.t_in) * 1e3)
+            r.done.set()
+        try:
+            sr = make(self.pipeline, r.inputs, r.knobs)
+            sr.on_done, sr.tag = answer, r.log_id
+            self.scheduler.submit(sr)
+        except Exception as ex:  # the request fails, the server lives
+            log.error("%s: chat request refused: %s\n%s", r.log_id, ex, traceback.format_exc())
+            r.error = ex
+            r.done.set()
+
+    def run(self):
+        while True:
+            idle = not self.scheduler.busy()
+            if idle and self._halt.is_set():
+                break
+            try:
+                r = self.q.get(block=idle)
+                while True:
+                    if r is None:
+                        self._halt.set()
+                    else:
+                        self._admit(r)
+                    r = self.q.get_nowait()
+            except queue.Empty:
+                pass
+            if self.scheduler.busy():
+                try:
+                    self.scheduler.step()
+                except Exception as ex:
+                    log.error("continuous batching step failed: %s\n%s", ex, traceback.format_exc())
+                    self.scheduler.abort(ex)
+
+
 # ---- the form encoding of the demo front end (Emu2/demo/frontend/libs/chat_frontend.py:96-127) ----
 def parse_form(content_type, body):
     """-> (fields: {name: str}, files: {name: bytes}) for multipart/form-data (what `requests.post(files=..., data=...)` sends
@@ -222,7 +310,7 @@ class EmuServer:
     --chat-concurrency / --generate-concurrency instances); requests go to the worker with the shortest queue."""
 
     def __init__(self, chat=None, generate=None, host="0.0.0.0", port=9000, max_wait_ms=0.0, max_images_per_batch=4,
-                 cache_dir=None, announce=None, max_body_bytes=256 << 20):
+                 cache_dir=None, announce=None, max_body_bytes=256 << 20, chat_scheduler="batching"):
         self.cache_dir = cache_dir
         self.max_body_bytes = int(max_body_bytes)
         if cache_dir:
@@ -234,8 +322,15 @@ class EmuServer:
         def chat_cap(pipe):
             fn = getattr(pipe, "max_requests_per_batch", None)
             return (lambda knobs: fn(knobs.get("num_beams", 1))) if fn else (lambda knobs: 1)
-        self.chat_workers = [BatchingWorker(p, "chat", chat_cap(p), max_wait_ms, announce, "emu-chat-%d" % i)
-                             for i, p in enumerate(as_list(chat))]
+        if chat_scheduler == "continuous":
+            if announce is not None:
+                raise ValueError("continuous batching runs on one GPU: it cannot follow a tensor-parallel instance")
+            self.chat_workers = [ContinuousWorker(p, name="emu-chat-%d" % i) for i, p in enumerate(as_list(chat))]
+        elif chat_scheduler == "batching":
+            self.chat_workers = [BatchingWorker(p, "chat", chat_cap(p), max_wait_ms, announce, "emu-chat-%d" % i)
+                                 for i, p in enumerate(as_list(chat))]
+        else:
+            raise ValueError("chat_scheduler must be 'batching' or 'continuous', got %r" % (chat_scheduler,))
         # (no announce for generation: the UNet is not tensor parallel, follower ranks hold no generation pipeline)
         self.gen_workers = [BatchingWorker(p, "generate", (lambda knobs: max_images_per_batch)
                                            if hasattr(p, "forward_batch") else None, max_wait_ms, None, "emu-gen-%d" % i)
@@ -273,7 +368,7 @@ class EmuServer:
     def _pick(self, workers, what):
         if not workers:
             raise RuntimeError("%s is disabled on this server" % what)
-        return min(workers, key=lambda w: w.q.qsize() + len(w.held))
+        return min(workers, key=lambda w: w.load())
 
     def _save(self, log_id, name, image):
         if self.cache_dir:
@@ -377,6 +472,8 @@ def main(argv=None):
     ap.add_argument("--chat-max-rows", type=int, default=20, help="KV-cache rows of the chat engine (requests x num_beams)")
     ap.add_argument("--max-wait-ms", type=float, default=2.0)
     ap.add_argument("--max-images-per-batch", type=int, default=4)
+    ap.add_argument("--continuous-batching", action="store_true",
+                    help="chat requests join and leave the decode batch between steps (one GPU per chat instance)")
     ap.add_argument("--cache-dir", type=str, default="", help="keep request pictures / results here (the reference always does)")
     ap.add_argument("--safety-checker", action="store_true",
                     help="run the built-in NSFW safety checker (the checkpoint's safety_checker.* weights) on every generated "
@@ -392,6 +489,8 @@ def main(argv=None):
         ap.error("more than one GPU per instance = tensor parallelism: launch with torchrun, one process per GPU")
     if world > 1 and (args.chat_concurrency > 1 or args.generate_concurrency > 1):
         ap.error("under torchrun all ranks form ONE tensor-parallel instance; run more servers for more instances")
+    if world > 1 and args.continuous_batching:
+        ap.error("--continuous-batching runs on one GPU per chat instance: it is not available under torchrun")
     tp = {}
     if world > 1:
         # one tensor-parallel chat instance over all ranks: the library's communicator is created from an id made by rank 0
@@ -431,7 +530,8 @@ def main(argv=None):
         return
     srv = EmuServer(chat=chat, generate=gen, host=args.host, port=args.port, max_wait_ms=args.max_wait_ms,
                     max_images_per_batch=args.max_images_per_batch, cache_dir=args.cache_dir or None,
-                    announce=make_announce() if world > 1 else None)
+                    announce=make_announce() if world > 1 else None,
+                    chat_scheduler="continuous" if args.continuous_batching else "batching")
     log.info("serving on %s:%d (chat x%d, generate x%d)", args.host, srv.port, len(chat), len(gen))
     try:
         srv.serve_forever()
