@@ -77,6 +77,9 @@ SYMBOLS = [
 SAFETY_SYMBOLS = ["emu_safety_configure", "emu_safety_check", "emu_safety_embed", "emu_preprocess_clip"]
 # ... and in include/emu_b200_slots.h (slot mode: continuous batching)
 SLOT_SYMBOLS = ["emu_llm_slots_begin", "emu_llm_join", "emu_llm_fork", "emu_llm_leave", "emu_llm_slot_len"]
+# ... and in include/emu_b200_ops.h (the decode-step kernels as stand-alone operators)
+OPS_SYMBOLS = ["emu_op_attn_decode_rows", "emu_op_rope_kv_write", "emu_op_kv_indir_update", "emu_op_kv_reorder",
+               "emu_op_argmax_rows", "emu_op_attn_prefill_rows"]
 
 _lib = None
 
@@ -614,6 +617,81 @@ def op_attn_decode(q, k_cache, v_cache, pos, start, scale, max_len):
     rc = lib.emu_op_attn_decode(_ptr(q), _ptr(k_cache), _ptr(v_cache), B, H, D, T, _ptr(pos), _ptr(start),
                                 C.c_float(scale), _ptr(out), max_len, _stream())
     check(rc)
+    return out
+
+
+# ---- the decode-step kernels (include/emu_b200_ops.h) ----
+def _i32(t, name):
+    if t is not None and (t.dtype != torch.int32 or not t.is_contiguous()):
+        raise ValueError("%s must be a contiguous int32 tensor" % name)
+    return _ptr(t)
+
+
+def op_attn_decode_rows(q, k_cache, v_cache, pos, start, scale, max_len_hint, indir=None):
+    """q [B, H*D] (B <= 32); caches [rows, H, T, D]; pos / start int32 [B] (start may be None); indir int32 [rows, T] or None
+    (row b) -> [B, H*D]"""
+    require_cuda()
+    _, H, T, D = k_cache.shape
+    B = q.shape[0]
+    out = torch.empty(B, H * D, dtype=torch.bfloat16, device=q.device)
+    check(load().emu_op_attn_decode_rows(_ptr(q), _ptr(k_cache), _ptr(v_cache), B, H, D, T, _i32(pos, "pos"),
+                                         _i32(start, "start"), _i32(indir, "indir"), C.c_float(scale), _ptr(out),
+                                         int(max_len_hint), _stream()))
+    return out
+
+
+def op_rope_kv_write(qkv, H, D, rope_cos, rope_sin, k_cache, v_cache, pos_off=None, pos0=0, pos_dev=None, q_out=None,
+                     kv_row=None):
+    """qkv [B, N, 3*H*D] (q rotated in place unless q_out [B*N, H*D] is given); caches [rows, H, T, D] written in place"""
+    require_cuda()
+    B, N, _ = qkv.shape
+    assert qkv.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
+    check(load().emu_op_rope_kv_write(_ptr(qkv), B, N, H, D, _ptr(rope_cos), _ptr(rope_sin), _i32(pos_off, "pos_off"),
+                                      int(pos0), _i32(pos_dev, "pos_dev"), _ptr(q_out), _i32(kv_row, "kv_row"), _ptr(k_cache),
+                                      _ptr(v_cache), k_cache.shape[2], _stream()))
+
+
+def op_kv_indir_update(indir, src_idx, n_tok, row_len=None):
+    """indir int32 [rows, T] in place: indir[b, t] <- indir[src_idx[b], t] for b < len(src_idx), t < n_tok (and < row_len[b])"""
+    require_cuda()
+    check(load().emu_op_kv_indir_update(_i32(indir, "indir"), _i32(src_idx, "src_idx"), _i32(row_len, "row_len"),
+                                        src_idx.numel(), indir.shape[1], int(n_tok), _stream()))
+
+
+def op_kv_reorder(cache, src_idx, n_used_tokens, B=None):
+    """cache [outer, Bcap, H, T, D] in place: row b <- row src_idx[b] for b < B, slots t < n_used_tokens"""
+    require_cuda()
+    outer, Bcap, H, T, D = cache.shape
+    assert cache.is_contiguous()
+    B = src_idx.numel() if B is None else B
+    check(load().emu_op_kv_reorder(_ptr(cache), Bcap, _i32(src_idx, "src_idx"), int(B), outer, int(n_used_tokens), H, D, T,
+                                   _stream()))
+
+
+def op_argmax_rows(logits):
+    """logits fp32 [rows, cols] (contiguous, any base alignment) -> int32 [rows], first index of the maximum"""
+    require_cuda()
+    assert logits.dtype == torch.float32 and logits.is_contiguous()
+    out = torch.empty(logits.shape[0], dtype=torch.int32, device=logits.device)
+    check(load().emu_op_argmax_rows(_ptr(logits), logits.shape[0], logits.shape[1], _ptr(out), _stream()))
+    return out
+
+
+def op_attn_prefill_rows(q, k, v, scale, causal=False, kv_start=None, kv_row=None):
+    """q [B,Nq,H,D]; k/v [rows,Nk,H,D] views (any strides with contiguous D) of which query batch b reads batch kv_row[b]
+    (kv_row None: k/v have B entries and b reads b) -> [B,Nq,H,D]"""
+    require_cuda()
+    B, Nq, H, D = q.shape
+    Nk = k.shape[1]
+    out = torch.empty(B, Nq, H, D, dtype=torch.bfloat16, device=q.device)
+    st = []
+    for t in (q, k, v, out):
+        assert t.stride(3) == 1
+        st += [t.stride(0), t.stride(1), t.stride(2)]
+    st12 = (C.c_int64 * 12)(*st)
+    check(load().emu_op_attn_prefill_rows(_ptr(q), _ptr(k), _ptr(v), _ptr(out), B, H, Nq, Nk, D, st12, C.c_float(scale),
+                                          1 if causal else 0, _i32(kv_start, "kv_start"), _i32(kv_row, "kv_row"),
+                                          k.shape[0] if kv_row is not None else 0, _stream()))
     return out
 
 

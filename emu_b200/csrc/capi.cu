@@ -2,6 +2,7 @@
 // These expose exactly the kernels the engine launches, so the parity tests exercise the product path.
 #include "common.cuh"
 #include "engine.h"
+#include "../../include/emu_b200_ops.h"
 
 using namespace emu;
 
@@ -130,6 +131,91 @@ extern "C" int emu_op_attn_decode(const void* q, const void* k_cache, const void
   count_launch();
   return attn_decode((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, B, H, D, t_max, pos, start, scale,
                      (bf16*)out, ws, counters, max_len, 0, (cudaStream_t)s);
+}
+
+// ---- the decode-step kernels (include/emu_b200_ops.h): the engine's launchers at any shape, arguments checked first ----
+static bool llm_head_dim_ok(int D) { return D == 64 || D == 128; }
+
+extern "C" int emu_op_attn_decode_rows(const void* q, const void* k_cache, const void* v_cache, int B, int H, int D,
+                                       int t_max, const int32_t* pos, const int32_t* start, const int32_t* indir, float scale,
+                                       void* out, int max_len_hint, emu_stream_t s) {
+  if (!q || !k_cache || !v_cache || !pos || !out) return EMU_ERR_INVALID;
+  if (B < 1 || B > kLlmMaxRows || H < 1 || !llm_head_dim_ok(D) || t_max < 1) return EMU_ERR_INVALID;
+  if (max_len_hint < 1 || max_len_hint > t_max) return EMU_ERR_INVALID;
+  // split workspace and combine counters for kLlmMaxRows x H (re)allocated when a wider head set arrives; the kernel
+  // resets every counter it uses, so they are zeroed once per allocation
+  static float* ws = nullptr;
+  static int* counters = nullptr;
+  static int cap_h = 0, cap_d = 0;
+  if (H > cap_h || D > cap_d) {
+    const int h = H > cap_h ? H : cap_h, d = D > cap_d ? D : cap_d;
+    if (ws) cudaFree(ws);
+    if (counters) cudaFree(counters);
+    ws = nullptr;
+    counters = nullptr;
+    cap_h = cap_d = 0;
+    const size_t n_ctr = (size_t)kLlmMaxRows * h * sizeof(int);
+    if (cudaMalloc((void**)&ws, attn_decode_workspace_bytes(kLlmMaxRows, h, d)) != cudaSuccess) return EMU_ERR_NOMEM;
+    if (cudaMalloc((void**)&counters, n_ctr) != cudaSuccess) return EMU_ERR_NOMEM;
+    if (cudaMemset(counters, 0, n_ctr) != cudaSuccess) return EMU_ERR_CUDA;
+    cap_h = h;
+    cap_d = d;
+  }
+  count_launch();
+  return attn_decode((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, B, H, D, t_max, pos, start, scale,
+                     (bf16*)out, ws, counters, max_len_hint, 0, (cudaStream_t)s, indir);
+}
+
+extern "C" int emu_op_rope_kv_write(void* qkv, int B, int N, int H, int D, const void* rope_cos, const void* rope_sin,
+                                    const int32_t* pos_off, int pos0, const int32_t* pos_dev, void* q_out,
+                                    const int32_t* kv_row, void* k_cache, void* v_cache, int t_max, emu_stream_t s) {
+  if (!qkv || !rope_cos || !rope_sin || !k_cache || !v_cache) return EMU_ERR_INVALID;
+  if (B < 1 || B > kLlmMaxRows || N < 1 || H < 1 || !llm_head_dim_ok(D) || t_max < 1 || pos0 < 0) return EMU_ERR_INVALID;
+  if (!pos_dev && pos0 + N > t_max) return EMU_ERR_INVALID;
+  count_launch();
+  return rope_kv_write((bf16*)qkv, B, N, H, D, (const bf16*)rope_cos, (const bf16*)rope_sin, pos_off, pos0, (bf16*)k_cache,
+                       (bf16*)v_cache, t_max, (cudaStream_t)s, pos_dev, (bf16*)q_out, kv_row);
+}
+
+extern "C" int emu_op_kv_indir_update(int32_t* indir, const int32_t* src_idx, const int32_t* row_len, int B, int t_max,
+                                      int n_tok, emu_stream_t s) {
+  if (!indir || !src_idx) return EMU_ERR_INVALID;
+  if (B < 1 || B > kLlmMaxRows || t_max < 1 || n_tok < 1 || n_tok > t_max) return EMU_ERR_INVALID;
+  count_launch();
+  return kv_indir_update(indir, src_idx, B, t_max, n_tok, (cudaStream_t)s, row_len);
+}
+
+extern "C" int emu_op_kv_reorder(void* cache, int Bcap, const int32_t* src_idx, int B, int outer, int n_used_tokens, int H,
+                                 int D, int t_max, emu_stream_t s) {
+  if (!cache || !src_idx) return EMU_ERR_INVALID;
+  if (B < 1 || B > kLlmMaxRows || Bcap < B || outer < 1 || H < 1 || !llm_head_dim_ok(D) || t_max < 1) return EMU_ERR_INVALID;
+  if (n_used_tokens < 1 || n_used_tokens > t_max) return EMU_ERR_INVALID;
+  count_launch();
+  return kv_reorder((bf16*)cache, Bcap, src_idx, B, outer, n_used_tokens, H, D, t_max, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_argmax_rows(const float* logits, int rows, int cols, int32_t* out, emu_stream_t s) {
+  if (!logits || !out || rows < 1 || cols < 1) return EMU_ERR_INVALID;
+  count_launch();
+  return argmax_rows(logits, rows, cols, out, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_attn_prefill_rows(const void* q, const void* k, const void* v, void* out, int B, int H, int Nq, int Nk,
+                                        int D, const int64_t* st12, float scale, int causal, const int32_t* kv_start,
+                                        const int32_t* kv_row, int kv_rows, emu_stream_t s) {
+  if (!q || !k || !v || !out || !st12) return EMU_ERR_INVALID;
+  if (B < 1 || B > kLlmMaxRows || H < 1 || Nq < 1 || Nk < 1 || D < 8 || D > 160 || D % 8) return EMU_ERR_INVALID;
+  if (kv_row && (kv_rows < 1 || kv_rows > kLlmMaxRows)) return EMU_ERR_INVALID;
+  AttnArgs a;
+  a.q = (const bf16*)q; a.k = (const bf16*)k; a.v = (const bf16*)v; a.out = (bf16*)out;
+  a.q_bs = st12[0]; a.q_ts = st12[1]; a.q_hs = st12[2];
+  a.k_bs = st12[3]; a.k_ts = st12[4]; a.k_hs = st12[5];
+  a.v_bs = st12[6]; a.v_ts = st12[7]; a.v_hs = st12[8];
+  a.o_bs = st12[9]; a.o_ts = st12[10]; a.o_hs = st12[11];
+  a.B = B; a.H = H; a.Nq = Nq; a.Nk = Nk; a.D = D; a.scale = scale; a.causal = causal; a.kv_start = kv_start;
+  a.kv_row = kv_row; a.kv_rows = kv_row ? kv_rows : 0;
+  count_launch();
+  return attn_prefill(a, (cudaStream_t)s);
 }
 
 extern "C" int emu_op_rmsnorm(const void* x, const void* w, void* y, int rows, int cols, float eps, emu_stream_t s) {

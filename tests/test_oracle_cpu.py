@@ -1,6 +1,9 @@
 """CPU: the oracle restatement (oracle/emu_oracle.py) against the golden outputs of the UNMODIFIED reference
 (tests/golden/emu2_tiny.pt, made by tests/golden/gen_golden.py, and tests/golden/live_reference.pt, made by
 tests/golden/gen_golden_live.py)."""
+import functools
+import importlib.util
+import json
 import os
 
 import numpy as np
@@ -14,6 +17,33 @@ from oracle import emu_oracle as O
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "emu2_tiny.pt")
 LIVE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live_reference.pt")
 L, NH = TINY_LLAMA["num_hidden_layers"], TINY_LLAMA["num_attention_heads"]
+CANARY = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gen_cpu_kernel_canary.py")
+FP32_BOUND = 1e-5    # the fp32 oracle-vs-reference bound of the tests above
+
+
+@functools.lru_cache(maxsize=None)
+def golden_cpu():
+    """True when this CPU's torch kernels are the ones that computed the reference goldens (tests/golden/
+    gen_cpu_kernel_canary.py): MKL, oneDNN and ATen choose their vector code by instruction set and vendor, and another choice sums
+    in another order."""
+    spec = importlib.util.spec_from_file_location("gen_cpu_kernel_canary", CANARY)
+    G = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(G)
+    with open(G.OUT) as f:
+        return G.digests() == json.load(f)
+
+
+def assert_reference(out, want, want_fp32=None):
+    """Bit equality with the reference's output where the CPU reproduces the goldens' kernels.  Elsewhere the summation
+    order differs: fp32 results must then agree within FP32_BOUND, and a bf16 result (want_fp32 = the reference's fp32
+    output for the same input) may be no farther from the reference's bf16 output than 1.5 x what bf16 rounding moves the
+    reference itself — the parity ratio of every bf16 comparison in this suite."""
+    if golden_cpu():
+        assert torch.equal(out, want)
+    elif want_fp32 is None:
+        assert O.rel_err(out, want) <= FP32_BOUND, O.rel_err(out, want)
+    else:
+        assert O.rel_err(out, want) <= 1.5 * O.rel_err(want, want_fp32), (O.rel_err(out, want), O.rel_err(want, want_fp32))
 
 
 @pytest.fixture(scope="module")
@@ -110,10 +140,10 @@ def test_t5_oracle_vs_reference_golden():
     from oracle import t5_oracle as T
     g, sd = _cformer_golden()
     out = T.causal_former(sd, g["img_embeds"], g["cfg"])
-    assert torch.equal(out, g["out_fp32"])
+    assert_reference(out, g["out_fp32"])
     sd16 = {k: v.to(torch.bfloat16) for k, v in sd.items()}
     out16 = T.causal_former(sd16, g["img_embeds"].to(torch.bfloat16), g["cfg"]).float()
-    assert torch.equal(out16, g["out_bf16"])
+    assert_reference(out16, g["out_bf16"], g["out_fp32"])
 
 
 def test_t5_oracle_vs_reference_t5_base():
@@ -128,7 +158,8 @@ def test_t5_oracle_vs_reference_t5_base():
     x = torch.randn(1, 257, 1408, generator=torch.Generator().manual_seed(ref["seed"] + 1))
     for name, dt in (("fp32", torch.float32), ("bf16", torch.bfloat16)):
         sdt = {k: v.to(dt) for k, v in sd.items()}
-        assert torch.equal(T.causal_former(sdt, x.to(dt)), ref["out_" + name])
+        assert_reference(T.causal_former(sdt, x.to(dt)).float(), ref["out_" + name].float(),
+                         None if dt == torch.float32 else ref["out_fp32"])
 
 
 def test_emu1_oracle_vs_reference_golden():
@@ -143,8 +174,8 @@ def test_emu1_oracle_vs_reference_golden():
         feats = O.vit_forward_features(sd, g["image"], patch=14, num_heads=vis["width"] // vis["head_width"], layers=2,
                                        postnorm=False)
         feats = F.layer_norm(feats, (vis["width"],), sd["ln_visual.weight"], sd["ln_visual.bias"], 1e-6)
-        assert torch.equal(feats, g["ln_visual_features"])
-        assert torch.equal(T.causal_former(sd, feats, emu1_t5_cfg()), g["cformer_out"])
+        assert_reference(feats, g["ln_visual_features"])
+        assert_reference(T.causal_former(sd, feats, emu1_t5_cfg()), g["cformer_out"])
 
 
 def test_emu1_vit_oracle_vs_reference():
@@ -153,7 +184,7 @@ def test_emu1_vit_oracle_vs_reference():
     ref = torch.load(LIVE)["emu1_vit"]
     sd = {"visual." + k: v for k, v in D.random_state_dict(ref["shapes"], seed=ref["seed"]).items()}
     img = torch.randn(2, 3, 56, 56, generator=torch.Generator().manual_seed(9))
-    assert torch.equal(ref["features"], O.vit_forward_features(sd, img, patch=14, num_heads=2, layers=2, postnorm=False))
+    assert_reference(O.vit_forward_features(sd, img, patch=14, num_heads=2, layers=2, postnorm=False), ref["features"])
 
 
 def _emu1_generate_image_oracle(sd, ids, image, vis):
