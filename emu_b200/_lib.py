@@ -80,6 +80,8 @@ SLOT_SYMBOLS = ["emu_llm_slots_begin", "emu_llm_join", "emu_llm_fork", "emu_llm_
 # ... and in include/emu_b200_ops.h (the decode-step kernels as stand-alone operators)
 OPS_SYMBOLS = ["emu_op_attn_decode_rows", "emu_op_rope_kv_write", "emu_op_kv_indir_update", "emu_op_kv_reorder",
                "emu_op_argmax_rows", "emu_op_attn_prefill_rows"]
+# ... and in include/emu_b200_gen_slots.h (latent slots: continuous batching for image generation)
+GEN_SLOT_SYMBOLS = ["emu_denoise_step_slots", "emu_op_denoise_prepare", "emu_op_denoise_euler"]
 
 _lib = None
 
@@ -367,6 +369,22 @@ class Engine:
         check(self.lib.emu_denoise_step(self.h, _ptr(latents_f32), C.c_float(float(sigma)), C.c_float(float(sigma_next)),
                                         C.c_float(float(timestep)), C.c_float(float(guidance)), _ptr(ctx), ctx.shape[1],
                                         _ptr(text_embeds), _ptr(time_ids), B, h, w, _stream()), self.h)
+
+    def denoise_step_slots(self, latents_f32, params, live, ctx, text_embeds, time_ids, B):
+        """One iteration over latent slots 0..B-1 (include/emu_b200_gen_slots.h): latents [>=B,4,h,w] fp32 in place, params
+        fp32 [>=B, 4] {sigma, sigma_next, timestep, guidance} and live int32 [>=B] on the device, read when the step runs.
+        ctx [>=2B, L, Cc], text_embeds [>=2B, Cc], time_ids [>=2B, 6]: rows 2b / 2b+1 are slot b's cond / uncond."""
+        _, _, h, w = latents_f32.shape
+        for name, t, dt, rows in (("latents", latents_f32, torch.float32, B), ("params", params, torch.float32, B),
+                                  ("live", live, torch.int32, B), ("ctx", ctx, torch.bfloat16, 2 * B),
+                                  ("text_embeds", text_embeds, torch.bfloat16, 2 * B), ("time_ids", time_ids, torch.int32, 2 * B)):
+            if t.dtype != dt or not t.is_contiguous() or t.shape[0] < rows:
+                raise ValueError("denoise_step_slots: %s must be a contiguous %s tensor of at least %d rows, got %s %s"
+                                 % (name, dt, rows, tuple(t.shape), t.dtype))
+        if params.shape[1:] != (4,) or time_ids.shape[1:] != (6,):
+            raise ValueError("denoise_step_slots: params must be [B, 4] and time_ids [2B, 6]")
+        check(self.lib.emu_denoise_step_slots(self.h, _ptr(latents_f32), _ptr(params), _ptr(live), _ptr(ctx), ctx.shape[1],
+                                              _ptr(text_embeds), _ptr(time_ids), int(B), h, w, _stream()), self.h)
 
     def denoise_step_multistep(self, latents_f32, state_f32, coef8, timestep, guidance, ctx):
         """One PNDM / PLMS iteration (emu_denoise_step_multistep): latents [B,4,h,w] fp32 in place, state [4,B,4,h,w] fp32."""
@@ -693,6 +711,39 @@ def op_attn_prefill_rows(q, k, v, scale, causal=False, kv_start=None, kv_row=Non
                                           1 if causal else 0, _i32(kv_start, "kv_start"), _i32(kv_row, "kv_row"),
                                           k.shape[0] if kv_row is not None else 0, _stream()))
     return out
+
+
+# ---- the denoise-step glue (include/emu_b200_gen_slots.h) ----
+def _rows_layout(B, slots_adjacent):
+    return (2, 1) if slots_adjacent else (1, B)
+
+
+def op_denoise_prepare(latents, params, Cp, copies=2, slots_adjacent=False):
+    """latents [B, C, h, w] fp32, params fp32 [B, 4] (or [4]: one set for every slot) -> (UNet input NHWC bf16
+    [copies*B, h, w, Cp], per-row timesteps fp32 [copies*B]); slot b's rows are b and B + b, or 2b and 2b + 1 (copies = 2)"""
+    require_cuda()
+    B, Cc, h, w = latents.shape
+    assert latents.dtype == torch.float32 and latents.is_contiguous()
+    assert params.dtype == torch.float32 and params.is_contiguous()
+    cs, ub = _rows_layout(B, slots_adjacent)
+    xin = torch.empty(copies * B, h, w, Cp, dtype=torch.bfloat16, device=latents.device)
+    t_rows = torch.empty(copies * B, dtype=torch.float32, device=latents.device)
+    check(load().emu_op_denoise_prepare(_ptr(latents), _ptr(xin), _ptr(t_rows), B, Cc, h * w, int(Cp), _ptr(params),
+                                        4 if params.dim() == 2 else 0, int(copies), cs, ub, _stream()))
+    return xin, t_rows
+
+
+def op_denoise_euler(latents, eps_nhwc, params, live=None, slots_adjacent=False):
+    """latents [B, C, h, w] fp32 updated in place from the noise prediction eps NHWC bf16 [rows, h, w, ld] (rows as
+    op_denoise_prepare's); params fp32 [B, 4] or [4]; live int32 [B] or None"""
+    require_cuda()
+    B, Cc, h, w = latents.shape
+    assert latents.dtype == torch.float32 and latents.is_contiguous()
+    assert eps_nhwc.dtype == torch.bfloat16 and eps_nhwc.is_contiguous()
+    assert params.dtype == torch.float32 and params.is_contiguous()
+    cs, ub = _rows_layout(B, slots_adjacent)
+    check(load().emu_op_denoise_euler(_ptr(latents), _ptr(eps_nhwc), _i32(live, "live"), B, Cc, h * w, eps_nhwc.shape[-1],
+                                      _ptr(params), 4 if params.dim() == 2 else 0, cs, ub, _stream()))
 
 
 def op_rmsnorm(x, w, eps):

@@ -413,3 +413,225 @@ def chat_request(chat, inputs, is_grounding=False, skip_special_tokens=True, **k
     knobs.pop("synced_gpus", None)
     return SlotRequest(input_ids, mask, image=image, video=video, image_token_id=IMAGE, video_token_id=VIDEO,
                        finish=lambda ids: tok.batch_decode(ids, skip_special_tokens=skip_special_tokens)[0], **knobs)
+
+
+# ---- continuous batching for image generation ----
+class ImageRequest:
+    """One EmuVisualGeneration.forward call's worth of work: `inputs` (the interleaved prompt) or precomputed
+    `prompt_embeds` ([2, L, Cc] = [cond; uncond] with guidance > 1, [1, L, Cc] without, as _prepare_and_encode_inputs returns
+    them), with forward's knobs and defaults; height / width None take the scheduler's size.  `result` (an EmuVisualGenerationPipelineOutput, or the final latents
+    [1, C, h, w] fp32 with output_type="latent") or `error` is set when it is finished, then `done` is set and
+    `on_done(request)` is called."""
+
+    def __init__(self, inputs=None, prompt_embeds=None, height=None, width=None, num_inference_steps=50, guidance_scale=3.,
+                 crop_info=(0, 0), original_size=(1024, 1024), generator=None, latents=None, output_type="pil",
+                 on_done=None, tag=None):
+        if (inputs is None) == (prompt_embeds is None):
+            raise ValueError("an image request carries either inputs or prompt_embeds")
+        self.inputs = inputs if inputs is None or isinstance(inputs, list) else [inputs]
+        self.prompt_embeds = prompt_embeds
+        self.height, self.width = height, width
+        self.steps = int(num_inference_steps)
+        self.guidance = float(guidance_scale)
+        self.crop_info, self.original_size = list(crop_info), list(original_size)
+        self.generator, self.latents, self.output_type = generator, latents, output_type
+        self.on_done, self.tag = on_done, tag
+        self.done = threading.Event()
+        self.result = self.error = None
+        if self.steps < 1:
+            raise ValueError("num_inference_steps has to be >= 1")
+        if output_type not in ("pil", "latent"):
+            raise ValueError("output_type must be 'pil' or 'latent', got %r" % (output_type,))
+        # set at admission
+        self.slot = None
+        self.step = 0
+
+
+class DenoiseSlotScheduler:
+    """Continuous batching of EmuVisualGeneration requests over `n_slots` latent slots (include/emu_b200_gen_slots.h): each
+    slot holds one request at its own denoise step, with its own step count, guidance, time ids and latents.  One `step()`:
+
+      1. admit: waiting requests take the lowest free slots.  Each is encoded alone through _prepare_and_encode_inputs (so
+         the cached unconditional branch is reused) unless it carries prompt_embeds; its conditioning rows and initial
+         latents are written into its slot.  Encoding stalls the live slots;
+      2. step: the [n_slots][4] step parameters and the live mask go to the device from a pinned staging buffer, and ONE
+         emu_denoise_step_slots over B = highest live slot + 1 moves every live request one step along its own schedule;
+      3. retire: a request that has run all its steps is decoded (VAE, uint8, safety stage), answered and leaves its slot.
+
+    A request that fails answers with its own error and frees its slot; the others continue.  Each request's latents are the
+    ones `denoise` gives it alone (bitwise while the UNet's row count 2B stays within the GEMV path of its small linears, 8).
+    height / width are fixed per scheduler: the buffers, and the CUDA graph of each B, are made for one latent size.
+    Owns the pipeline's engine while it lives.  Single-threaded: `submit` may be called from any thread, `step` from one."""
+
+    def __init__(self, pipeline, n_slots=4, height=1024, width=1024, n_tokens=None):
+        self.pipe, self.engine = pipeline, pipeline.engine
+        self.n_slots = int(n_slots)
+        if not 1 <= self.n_slots <= 32:
+            raise ValueError("n_slots = %d must be in [1, 32]" % self.n_slots)
+        self.height, self.width = int(height), int(width)
+        f = pipeline.vae_scale_factor
+        if self.height % f or self.width % f:
+            raise ValueError("height and width must be multiples of %d" % f)
+        ucfg = pipeline.unet_config
+        self.L = int(n_tokens or pipeline.multimodal_encoder.n_query)
+        self.device = torch.device(pipeline.device_)
+        n, dev = self.n_slots, self.device
+        self.latents = torch.zeros(n, ucfg["in_channels"], self.height // f, self.width // f, dtype=torch.float32, device=dev)
+        self.ctx = torch.zeros(2 * n, self.L, ucfg["cross_attention_dim"], dtype=torch.bfloat16, device=dev)
+        self.text_embeds = torch.zeros(2 * n, ucfg["cross_attention_dim"], dtype=torch.bfloat16, device=dev)
+        self.time_ids = torch.zeros(2 * n, 6, dtype=torch.int32, device=dev)
+        # params [n][4] fp32 and live [n] int32 travel in ONE copy: both are views of one byte buffer on each side
+        nbytes = n * 4 * 4 + n * 4
+        self._stage = torch.zeros(nbytes, dtype=torch.uint8, pin_memory=dev.type == "cuda")
+        self._dev = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+        self.params, self.live = self._dev[:n * 16].view(torch.float32).view(n, 4), self._dev[n * 16:].view(torch.int32)
+        self._stage_params = self._stage[:n * 16].view(torch.float32).view(n, 4)
+        self._stage_live = self._stage[n * 16:].view(torch.int32)
+        self._copied = None                                  # event: the last staging copy has run
+        self.waiting = collections.deque()
+        self.owner = [None] * n
+        self.steps = 0
+        self.batch_sizes = collections.deque(maxlen=1024)   # B of the recent UNet steps (observability; the tests read it)
+        self._lock = threading.Lock()
+        # every workspace at its largest size now: a later growth would drop every captured graph
+        with _on_device(dev):
+            self._unet_step(n)
+
+    # ---- producer side ----
+    def submit(self, request: ImageRequest):
+        if request.height is None and request.width is None:
+            request.height, request.width = self.height, self.width
+        if (request.height, request.width) != (self.height, self.width):
+            raise ValueError("this scheduler generates %dx%d images; a %dx%d request needs a scheduler of its own size"
+                             % (self.width, self.height, request.width, request.height))
+        with self._lock:
+            self.waiting.append(request)
+        return request
+
+    def busy(self):
+        return any(self.owner) or bool(self.waiting)
+
+    def load(self):
+        """requests admitted or waiting"""
+        return sum(r is not None for r in self.owner) + len(self.waiting)
+
+    def abort(self, ex):
+        """fail every live and waiting request with `ex` (the scheduler itself stays usable)"""
+        for r in self._live():
+            self._fail(r, ex)
+        with self._lock:
+            waiting, self.waiting = list(self.waiting), collections.deque()
+        for r in waiting:
+            self._fail(r, ex)
+
+    def run_until_idle(self):
+        out = []
+        while self.busy():
+            out += self.step()
+        return out
+
+    def _live(self):
+        return [r for r in self.owner if r is not None]
+
+    # ---- one iteration ----
+    @torch.no_grad()
+    def step(self):
+        """admit -> step -> retire (class docstring); returns the requests finished in this step"""
+        with _on_device(self.device):
+            self._admit()
+            live = self._live()
+            if not live:
+                return []
+            try:
+                self._unet_step(max(r.slot for r in live) + 1)
+            except Exception as ex:       # an engine-level failure: every live request fails, the scheduler stays usable
+                for r in live:
+                    self._fail(r, ex)
+                return live
+            self.steps += 1
+            self.batch_sizes.append(max(r.slot for r in live) + 1)
+            finished = []
+            for r in live:
+                r.step += 1
+                if r.step == r.steps:
+                    self._retire(r)
+                    finished.append(r)
+            return finished
+
+    def _admit(self):
+        while True:
+            with self._lock:
+                if not self.waiting or None not in self.owner:
+                    return
+                r = self.waiting.popleft()
+                r.slot = self.owner.index(None)
+                self.owner[r.slot] = r
+            try:
+                self._fill_slot(r)
+            except Exception as ex:         # a prompt that cannot be encoded fails on its own
+                self._fail(r, ex)
+
+    def _fill_slot(self, r):
+        pipe, s = self.pipe, r.slot
+        cfg = r.guidance > 1.0
+        pe = r.prompt_embeds
+        if pe is None:
+            pe = pipe._prepare_and_encode_inputs(r.inputs, cfg)
+        pe = pe.to(self.device, torch.bfloat16)
+        if pe.dim() != 3 or pe.shape[0] != (2 if cfg else 1) or tuple(pe.shape[1:]) != tuple(self.ctx.shape[1:]):
+            raise ValueError("prompt embeddings of shape %s do not fit a slot: expected [%d, %d, %d]"
+                             % (tuple(pe.shape), 2 if cfg else 1, self.L, self.ctx.shape[2]))
+        ctx, te, tid = pipe.conditioning(pe, self.height, self.width, r.crop_info, r.original_size)
+        ts, sig, init_noise_sigma = pipe.schedule(r.steps)
+        lat = pipe.initial_latents(1, self.height, self.width, init_noise_sigma, generator=r.generator, latents=r.latents)
+        u = 1 if cfg else 0                  # without guidance the unconditional row repeats the conditional one (ignored)
+        self.ctx[2 * s], self.ctx[2 * s + 1] = ctx[0], ctx[u]
+        self.text_embeds[2 * s], self.text_embeds[2 * s + 1] = te[0], te[u]
+        self.time_ids[2 * s], self.time_ids[2 * s + 1] = tid[0], tid[u]
+        self.latents[s] = lat[0]
+        r.timesteps, r.sigmas = [float(t) for t in ts], [float(v) for v in sig]
+
+    def _unet_step(self, B):
+        if self._copied is not None:
+            self._copied.synchronize()       # the staging buffer is rewritten only after its last copy has run
+        self._stage.zero_()
+        for r in self._live():
+            i = r.step
+            self._stage_params[r.slot] = torch.tensor([r.sigmas[i], r.sigmas[i + 1], r.timesteps[i], r.guidance])
+            self._stage_live[r.slot] = 1
+        self._dev.copy_(self._stage, non_blocking=True)
+        if self.device.type == "cuda":
+            self._copied = torch.cuda.Event()
+            self._copied.record()
+        self.engine.denoise_step_slots(self.latents, self.params, self.live, self.ctx, self.text_embeds, self.time_ids, B)
+
+    # ---- retirement ----
+    def _retire(self, r):
+        try:
+            lat = self.latents[r.slot:r.slot + 1].clone()
+            if r.output_type == "latent":
+                r.result = lat
+            else:
+                from PIL import Image
+                from .emu2.diffusion import EmuVisualGenerationPipelineOutput
+                u8, flags = self.pipe.decode_and_check(lat)
+                r.result = EmuVisualGenerationPipelineOutput(image=Image.fromarray(u8[0]),
+                                                             nsfw_content_detected=None if flags is None else flags[0])
+        except Exception as ex:
+            r.error = ex
+        self._release(r)
+        self._answer(r)
+
+    def _release(self, r):
+        if r.slot is not None and self.owner[r.slot] is r:
+            self.owner[r.slot] = None
+
+    def _answer(self, r):
+        r.done.set()
+        if r.on_done is not None:
+            r.on_done(r)
+
+    def _fail(self, r, ex):
+        r.error = ex
+        self._release(r)
+        self._answer(r)

@@ -26,7 +26,8 @@ def sources():
 def _digest():
     h = hashlib.sha256()
     for f in sorted(os.listdir(CSRC)) + ["../../include/emu_b200.h", "../../include/emu_b200_safety.h",
-                                        "../../include/emu_b200_slots.h", "../../include/emu_b200_ops.h"]:
+                                        "../../include/emu_b200_slots.h", "../../include/emu_b200_ops.h",
+                                        "../../include/emu_b200_gen_slots.h"]:
         p = os.path.join(CSRC, f)
         if os.path.isfile(p):
             h.update(f.encode())

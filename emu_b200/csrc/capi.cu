@@ -3,6 +3,8 @@
 #include "common.cuh"
 #include "engine.h"
 #include "../../include/emu_b200_ops.h"
+#include "../../include/emu_b200_gen_slots.h"
+#include "diffusion_common.h"
 
 using namespace emu;
 
@@ -230,4 +232,28 @@ extern "C" int emu_op_layernorm(const void* x, const void* w, const void* b, con
   count_launch();
   return layernorm((const bf16*)x, (const bf16*)w, (const bf16*)b, (const bf16*)residual, (bf16*)y, rows, cols, eps,
                    (cudaStream_t)s);
+}
+
+// ---- the denoise-step glue of include/emu_b200_gen_slots.h ----
+static bool denoise_glue_args_ok(int B, int C, int HW, int ps, int cs, int ub) {
+  if (B < 1 || B > kMaxLatentSlots || C < 1 || HW < 1) return false;
+  if (ps != 0 && ps != 4) return false;
+  return (cs == 1 && ub == B) || (cs == 2 && ub == 1);  // the two row layouts; anything else could alias two slots' rows
+}
+
+extern "C" int emu_op_denoise_prepare(const float* latents, void* xin, float* t_rows, int B, int C, int HW, int Cp,
+                                      const float* params, int ps, int copies, int cs, int ub, emu_stream_t s) {
+  if (!latents || !xin || !t_rows || !params) return EMU_ERR_INVALID;
+  if (!denoise_glue_args_ok(B, C, HW, ps, cs, ub) || Cp < C || (copies != 1 && copies != 2)) return EMU_ERR_INVALID;
+  if (cs == 2 && copies != 2) return EMU_ERR_INVALID;  // adjacent rows: every slot owns two, the output holds 2B
+  count_launch();
+  return slot_prepare(latents, (bf16*)xin, t_rows, B, C, HW, Cp, params, ps, copies, cs, ub, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_denoise_euler(float* latents, const void* eps, const int32_t* live, int B, int C, int HW, int ld,
+                                    const float* params, int ps, int cs, int ub, emu_stream_t s) {
+  if (!latents || !eps || !params) return EMU_ERR_INVALID;
+  if (!denoise_glue_args_ok(B, C, HW, ps, cs, ub) || ld < C) return EMU_ERR_INVALID;
+  count_launch();
+  return slot_cfg_euler(latents, (const bf16*)eps, live, B, C, HW, ld, params, ps, cs, ub, (cudaStream_t)s);
 }

@@ -17,6 +17,8 @@
 
 namespace emu {
 
+constexpr int kMaxLatentSlots = 32;  // include/emu_b200_gen_slots.h: B of a latent-slot step
+
 // diffusion_ops.cu
 int groupnorm_nhwc(const bf16* x, const bf16* w, const bf16* b, bf16* y, float* scratch, int NB, int HW, int C,
                    int groups, float eps, int do_silu, cudaStream_t st);
@@ -28,14 +30,13 @@ int upsample2x_nhwc(const bf16* x, bf16* y, int NB, int H, int W, int C, cudaStr
 int im2col3x3(const bf16* x, bf16* out, int NB, int H, int W, int C, int stride, cudaStream_t st);
 int nchw_to_nhwc(const bf16* x, bf16* y, int NB, int C, int HW, int Cp, float scale, cudaStream_t st);
 int nhwc_to_nchw(const bf16* x, bf16* y, int NB, int C, int HW, int ldx, cudaStream_t st);
-int cfg_prepare(const float* lat, bf16* xin, int B, int C, int HW, int Cp, const float* params, int copies,
-                cudaStream_t st);
-int cfg_euler(float* lat, const bf16* eps_nhwc, int B, int C, int HW, int ld, const float* params, int cfg,
-              cudaStream_t st);
+int slot_prepare(const float* lat, bf16* xin, float* t_rows, int B, int C, int HW, int Cp, const float* params, int ps,
+                 int copies, int cs, int ub, cudaStream_t st);
+int slot_cfg_euler(float* lat, const bf16* eps_nhwc, const int* live, int B, int C, int HW, int ld, const float* params, int ps,
+                   int cs, int ub, cudaStream_t st);
 int cfg_multistep(float* lat, const bf16* eps_nhwc, float* hist, float* saved, int B, int C, int HW, int ld,
                   const float* params, int cfg, cudaStream_t st);
 int int_to_float(const int* x, float* y, int n, cudaStream_t st);
-int fill_float(float* y, int n, const float* src_scalar, cudaStream_t st);
 
 #define EMU_TRY(x)                 \
   do {                             \

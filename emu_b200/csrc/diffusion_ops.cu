@@ -203,13 +203,6 @@ int int_to_float(const int* x, float* y, int n, cudaStream_t st) {
   int_to_float_kernel<<<(n + 255) / 256, 256, 0, st>>>(x, y, n);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
-__global__ void fill_float_kernel(float* y, int n, const float* __restrict__ src) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) y[i] = src[0];
-}
-int fill_float(float* y, int n, const float* src_scalar, cudaStream_t st) {
-  fill_float_kernel<<<(n + 255) / 256, 256, 0, st>>>(y, n, src_scalar);
-  return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
-}
 
 __global__ void silu_kernel(const bf16* __restrict__ x, bf16* y, long n) {
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
@@ -320,48 +313,62 @@ int nhwc_to_nchw(const bf16* x, bf16* y, int NB, int C, int HW, int ldx, cudaStr
 // ----------------------------------------------------------------------------------------------
 // denoise-step glue (Emu2/emu/diffusion.py:131-149)
 // ----------------------------------------------------------------------------------------------
-// params (device): [0] sigma, [1] sigma_next, [2] guidance scale — read on the device so the graph is reusable
-// latent_model_input = cat([latents]*2) / sqrt(sigma^2+1), written straight as NHWC (Cp channels, zero padded)
-__global__ void cfg_prepare_kernel(const float* __restrict__ lat, bf16* xin, int B, int C, int HW, int Cp,
-                                   const float* __restrict__ params, int copies) {
-  const float sigma = params[0];
-  const float inv = 1.0f / sqrtf(sigma * sigma + 1.0f);
-  const long total = (long)copies * B * HW * Cp;
-  for (long idx = blockIdx.x * (long)blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
+// The Euler glue serves B latent slots, each at its own step: slot b reads {sigma, sigma_next, timestep, guidance} at
+// params + b * ps on the device (ps = 0: one set for all slots), so one captured graph serves every step.  Slot b's conditional
+// UNet row is b * cs and its unconditional row ub + b * cs: [cond_1..B; uncond_1..B] is cs = 1, ub = B; slots whose two rows
+// are adjacent are cs = 2, ub = 1.
+//
+// latent_model_input = cat([latents]*2) / sqrt(sigma^2+1), written straight as NHWC (Cp channels, zero padded) into the
+// `copies` rows of every slot, and the slot's timestep into t_rows at the same rows
+__global__ void slot_prepare_kernel(const float* __restrict__ lat, bf16* xin, float* t_rows, int B, int C, int HW, int Cp,
+                                    const float* __restrict__ params, int ps, int copies, int cs, int ub) {
+  const long first = blockIdx.x * (long)blockDim.x + threadIdx.x;
+  if (first < (long)copies * B) {
+    const int k = (int)first / B, b = (int)first % B;
+    t_rows[k * ub + b * cs] = params[b * ps + 2];
+  }
+  const long per_row = (long)HW * Cp, total = (long)copies * B * per_row;
+  for (long idx = first; idx < total; idx += (long)gridDim.x * blockDim.x) {
     const int c = idx % Cp;
     const long p = (idx / Cp) % HW;
-    const int b2 = idx / ((long)Cp * HW);
-    const int b = b2 % B;
+    const int kb = idx / per_row, k = kb / B, b = kb % B;
+    const float sigma = params[b * ps];
+    const float inv = 1.0f / sqrtf(sigma * sigma + 1.0f);
     // the reference scales in the activation dtype: bf16(latent) / sqrt(sigma^2+1) -> bf16
-    xin[idx] = c < C ? __float2bfloat16_rn(round_bf16(lat[((long)b * C + c) * HW + p]) * inv) : __float2bfloat16(0.f);
+    xin[((long)(k * ub + b * cs) * HW + p) * Cp + c] =
+        c < C ? __float2bfloat16_rn(round_bf16(lat[((long)b * C + c) * HW + p]) * inv) : __float2bfloat16(0.f);
   }
 }
-int cfg_prepare(const float* lat, bf16* xin, int B, int C, int HW, int Cp, const float* params, int copies,
-                cudaStream_t st) {
-  cfg_prepare_kernel<<<2 * kNumSMs, 256, 0, st>>>(lat, xin, B, C, HW, Cp, params, copies);
+int slot_prepare(const float* lat, bf16* xin, float* t_rows, int B, int C, int HW, int Cp, const float* params, int ps,
+                 int copies, int cs, int ub, cudaStream_t st) {
+  slot_prepare_kernel<<<2 * kNumSMs, 256, 0, st>>>(lat, xin, t_rows, B, C, HW, Cp, params, ps, copies, cs, ub);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
-// noise = uncond + g*(cond - uncond) (cond first, :145-146); latents += noise * (sigma_next - sigma)  (Euler, eps-pred)
-__global__ void cfg_euler_kernel(float* lat, const bf16* __restrict__ eps_nhwc, int B, int C, int HW, int ld,
-                                 const float* __restrict__ params, int cfg) {
-  const float dt = params[1] - params[0], g = params[2];
+// noise = uncond + g*(cond - uncond) (cond first, :145-146); latents += noise * (sigma_next - sigma)  (Euler, eps-pred).
+// A slot with g <= 1 takes its conditional prediction as it is (forward without CFG has no unconditional row); a slot with
+// live[b] == 0 (live NULL: every slot is live) is not written.
+__global__ void slot_cfg_euler_kernel(float* lat, const bf16* __restrict__ eps_nhwc, const int* __restrict__ live, int B, int C,
+                                      int HW, int ld, const float* __restrict__ params, int ps, int cs, int ub) {
   const long total = (long)B * C * HW;
   for (long idx = blockIdx.x * (long)blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
     const long p = idx % HW;
     const int c = (idx / HW) % C;
     const int b = idx / ((long)HW * C);
-    const float ec = __bfloat162float(eps_nhwc[((long)b * HW + p) * ld + c]);
+    if (live && !live[b]) continue;
+    const float* pr = params + b * ps;
+    const float dt = pr[1] - pr[0], g = pr[3];
+    const float ec = __bfloat162float(eps_nhwc[((long)(b * cs) * HW + p) * ld + c]);
     float e = ec;
-    if (cfg) {
-      const float eu = __bfloat162float(eps_nhwc[((long)(B + b) * HW + p) * ld + c]);
+    if (g > 1.0f) {
+      const float eu = __bfloat162float(eps_nhwc[((long)(ub + b * cs) * HW + p) * ld + c]);
       e = round_bf16(eu + round_bf16(g * round_bf16(ec - eu)));  // bf16 rounding points of the reference expression
     }
     lat[idx] += e * dt;
   }
 }
-int cfg_euler(float* lat, const bf16* eps_nhwc, int B, int C, int HW, int ld, const float* params, int cfg,
-              cudaStream_t st) {
-  cfg_euler_kernel<<<2 * kNumSMs, 256, 0, st>>>(lat, eps_nhwc, B, C, HW, ld, params, cfg);
+int slot_cfg_euler(float* lat, const bf16* eps_nhwc, const int* live, int B, int C, int HW, int ld, const float* params, int ps,
+                   int cs, int ub, cudaStream_t st) {
+  slot_cfg_euler_kernel<<<2 * kNumSMs, 256, 0, st>>>(lat, eps_nhwc, live, B, C, HW, ld, params, ps, cs, ub);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
@@ -383,7 +390,7 @@ __global__ void cfg_multistep_kernel(float* lat, const bf16* __restrict__ eps_nh
     float e = ec;
     if (cfg) {
       const float eu = __bfloat162float(eps_nhwc[((long)(B + bb) * HW + p) * ld + c]);
-      e = round_bf16(eu + round_bf16(g * round_bf16(ec - eu)));  // same rounding points as cfg_euler_kernel
+      e = round_bf16(eu + round_bf16(g * round_bf16(ec - eu)));  // same rounding points as slot_cfg_euler_kernel
     }
     const float h0 = hist[idx], h1 = hist[total + idx], h2 = hist[2 * total + idx];
     const float m = wc * e + w0 * h0 + w1 * h1 + w2 * h2;

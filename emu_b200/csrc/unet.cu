@@ -16,6 +16,7 @@
 #include <string.h>
 
 #include "diffusion_common.h"
+#include "../../include/emu_b200_gen_slots.h"
 
 namespace emu {
 
@@ -34,10 +35,10 @@ struct UNetModel {
   std::map<std::string, DevBuf> bufs;
   bool grew = false;
   // denoise-step graph
-  typedef std::tuple<const void*, const void*, const void*, const void*, int, int, int, int> StepKey;
+  typedef std::tuple<const void*, const void*, const void*, const void*, const void*, const void*, int, int, int, int> StepKey;
   std::map<StepKey, cudaGraphExec_t> graphs;
   std::map<StepKey, int> warmed;
-  float* step_params = nullptr;  // device [4]: sigma, sigma_next, guidance, timestep
+  float* step_params = nullptr;  // device [12]: sigma, sigma_next, timestep, guidance, then the multistep scalars
   int n_launch = 0;
   // all cross-attention to_k / to_v weights stacked row-wise: the context is the same for every block, so ONE
   // [B2*L, sum 2C] GEMM at the top of the forward replaces 70 tiny per-block launches (same arithmetic per element)
@@ -278,7 +279,7 @@ int unet_load_tensor(EmuEngine* e, const std::string& key, const bf16* src, cons
 // Each CTA owns a contiguous slice of the NHWC noise prediction (ld = 8 channels -> one 16-byte word per latent pixel):
 //   1. pushes its slice of THIS rank's prediction into the peer's receive slot (16-byte NVLink stores),
 //   2. publishes a sequence flag with a system-scope release and spins (acquire) on the flag the peer wrote into OUR memory,
-//   3. combines cond (rank 0's prediction) and uncond (rank 1's) exactly like cfg_euler_kernel and applies the Euler step.
+//   3. combines cond (rank 0's prediction) and uncond (rank 1's) exactly like slot_cfg_euler_kernel and applies the Euler step.
 // Both ranks hold the same fp32 latents and perform the same arithmetic in the same order, so their latents stay bitwise
 // identical — and identical to the single-GPU path.  Two receive slots (sequence parity): a rank can run at most one
 // exchange ahead of its peer.  All state is on the device, so the kernel is captured in the denoise CUDA graph.
@@ -317,7 +318,7 @@ __global__ void __launch_bounds__(256) cfg_exchange_euler_kernel(float* lat, con
   }
   __syncthreads();
   const uint4* theirs = reinterpret_cast<const uint4*>(xch_local + parity * kXchSlot);
-  const float dt = params[1] - params[0], g = params[2];
+  const float dt = params[1] - params[0], g = params[3];
   for (long i = p0 + threadIdx.x; i < p1; i += blockDim.x) {
     const uint4 a = mine[i];
     uint4 o;
@@ -328,7 +329,7 @@ __global__ void __launch_bounds__(256) cfg_exchange_euler_kernel(float* lat, con
     for (int c = 0; c < C && c < 8; ++c) {
       const float ec = (c & 1) ? bf16_hi(cw[c >> 1]) : bf16_lo(cw[c >> 1]);
       const float eu = (c & 1) ? bf16_hi(uw[c >> 1]) : bf16_lo(uw[c >> 1]);
-      const float e = round_bf16(eu + round_bf16(g * round_bf16(ec - eu)));  // same rounding points as cfg_euler_kernel
+      const float e = round_bf16(eu + round_bf16(g * round_bf16(ec - eu)));  // same rounding points as slot_cfg_euler_kernel
       lat[((long)b * C + c) * HW + p] += e * dt;
     }
   }
@@ -729,17 +730,23 @@ extern "C" int emu_unet_forward(EmuEngine* e, const void* latents_nchw, float ti
 }
 
 // One denoise iteration.  ms == nullptr: Euler (Emu2-Gen); otherwise the 8 linear-multistep scalars of cfg_multistep_kernel
-// (PNDM, Emu1) with `state` = [4][B*C*h*w] fp32 (3 history planes + the saved sample).
+// (PNDM, Emu1) with `state` = [4][B*C*h*w] fp32 (3 history planes + the saved sample).  slot_params != nullptr: latent slots
+// (include/emu_b200_gen_slots.h), each at its own step with the caller's device params [B][4] and live mask [B].
 static int denoise_step_impl(EmuEngine* e, float* latents, float sigma, float sigma_next, float timestep, float guidance,
-                             const float* ms, float* state, const void* ctxv, int L, const void* text_embeds,
-                             const int32_t* time_ids, int B, int h, int w, emu_stream_t stream) {
+                             const float* ms, float* state, const float* slot_params, const int32_t* slot_live,
+                             const void* ctxv, int L, const void* text_embeds, const int32_t* time_ids, int B, int h, int w,
+                             emu_stream_t stream) {
   if (!e || !latents || !ctxv || B < 1) return EMU_ERR_INVALID;
   EMU_TRY(unet_ready(e));
   UNetModel* m = e->unet;
   cudaStream_t st = (cudaStream_t)stream;
-  const int cfg = guidance > 1.0f ? 1 : 0;  // do_classifier_free_guidance (Emu2/emu/diffusion.py:97)
+  const bool slots = slot_params != nullptr;
+  const bool exchange = m->xch && m->xch_peer && e->tp_size == 2;
+  if (slots && exchange) return e->fail(EMU_ERR_UNSUPPORTED, "latent slots on a CFG-parallel pair");
+  // slots: two UNet rows per slot whatever its guidance (a slot with guidance <= 1 ignores its unconditional row)
+  const int cfg = (slots || guidance > 1.0f) ? 1 : 0;  // do_classifier_free_guidance (Emu2/emu/diffusion.py:97)
   // CFG-parallel pair: this rank runs only its half of the [cond; uncond] UNet batch (SURVEY.md §8e "UNet, batch 1")
-  const int split = (cfg && m->xch && m->xch_peer && e->tp_size == 2) ? 1 : 0;
+  const int split = (cfg && exchange) ? 1 : 0;
   if (split && (size_t)B * h * w * 16 > kXchSlot) return e->fail(EMU_ERR_INVALID, "batch too large for the CFG-parallel exchange");
   if (split && (m->cfg.out_channels > 8)) return e->fail(EMU_ERR_UNSUPPORTED, "CFG-parallel exchange: out_channels > 8");
   const int B2 = (cfg && !split) ? 2 * B : B;
@@ -750,46 +757,52 @@ static int denoise_step_impl(EmuEngine* e, float* latents, float sigma, float si
     if (text_embeds) text_embeds = (const bf16*)text_embeds + (size_t)e->tp_rank * B * cd;
     if (time_ids) time_ids = time_ids + (size_t)e->tp_rank * B * 6;
   }
-  // per-step scalars go through device memory so the captured graph is step-independent
-  float hp[12] = {sigma, sigma_next, guidance, timestep, 0, 0, 0, 0, 0, 0, 0, 0};
-  if (ms) {
-    for (int i = 0; i < 6; ++i) hp[4 + i] = ms[i];
-    hp[10] = guidance;
-    hp[11] = ms[7];
+  // the glue reads its step from device memory, so the captured graph is step-independent: the slots' own params, or one
+  // set for every row uploaded here
+  const float* params = slot_params;
+  if (!slots) {
+    float hp[12] = {sigma, sigma_next, timestep, guidance, 0, 0, 0, 0, 0, 0, 0, 0};
+    if (ms) {
+      for (int i = 0; i < 6; ++i) hp[4 + i] = ms[i];
+      hp[10] = guidance;
+      hp[11] = ms[7];
+    }
+    if (ms && split) return e->fail(EMU_ERR_UNSUPPORTED, "CFG-parallel exchange with the multistep scheduler");
+    if (cudaMemcpyAsync(m->step_params, hp, sizeof(hp), cudaMemcpyHostToDevice, st) != cudaSuccess)
+      return e->fail(EMU_ERR_CUDA, "step params copy");
+    cudaStreamSynchronize(st);  // hp is a stack buffer
+    params = m->step_params;
   }
-  if (ms && split) return e->fail(EMU_ERR_UNSUPPORTED, "CFG-parallel exchange with the multistep scheduler");
-  if (cudaMemcpyAsync(m->step_params, hp, sizeof(hp), cudaMemcpyHostToDevice, st) != cudaSuccess)
-    return e->fail(EMU_ERR_CUDA, "step params copy");
-  cudaStreamSynchronize(st);  // hp is a stack buffer
+  const int ps = slots ? 4 : 0, cs = slots ? 2 : 1, ub = slots ? 1 : B;
 
   auto body = [&](cudaStream_t s, int* nl) -> int {
     Ctx c{e, &m->bufs, &m->grew, s, B2, m->cfg.norm_groups, m->cfg.norm_eps};
     BUF(xin, "x_in", (size_t)B2 * h * w * Cp);
     BUF(eps, "eps", (size_t)B2 * h * w * 8);
     BUF(tdev, "t_dev_big", (size_t)B2 * 2 + 8);
-    EMU_TRY(fill_float((float*)tdev, B2, m->step_params + 3, s));
-    EMU_TRY(cfg_prepare(latents, xin, B, Cin, h * w, Cp, m->step_params, (cfg && !split) ? 2 : 1, s));
+    EMU_TRY(slot_prepare(latents, xin, (float*)tdev, B, Cin, h * w, Cp, params, ps, (cfg && !split) ? 2 : 1, cs, ub, s));
     EMU_TRY(unet_core(c, m, xin, (const float*)tdev, (const bf16*)ctxv, L, (const bf16*)text_embeds, time_ids, h, w, eps));
     if (split) {
       const long n_pix = (long)B * h * w;
       int grid = (int)((n_pix + 2047) / 2048);
       if (grid > kXchCtas) grid = kXchCtas;
       cfg_exchange_euler_kernel<<<grid, 256, 0, s>>>(latents, eps, m->xch, m->xch_peer, e->tp_rank, B, m->cfg.out_channels,
-                                                     h * w, m->step_params);
+                                                     h * w, params);
       if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "CFG-parallel exchange launch failed");
     } else if (ms) {
       const long n = (long)B * m->cfg.out_channels * h * w;
-      EMU_TRY(cfg_multistep(latents, eps, state, state + 3 * n, B, m->cfg.out_channels, h * w, 8, m->step_params + 4, cfg, s));
+      EMU_TRY(cfg_multistep(latents, eps, state, state + 3 * n, B, m->cfg.out_channels, h * w, 8, params + 4, cfg, s));
     } else {
-      EMU_TRY(cfg_euler(latents, eps, B, m->cfg.out_channels, h * w, 8, m->step_params, cfg, s));
+      EMU_TRY(slot_cfg_euler(latents, eps, slot_live, B, m->cfg.out_channels, h * w, 8, params, ps, cs, ub, s));
     }
-    *nl = c.nl + 3;
+    *nl = c.nl + 2;
     return EMU_OK;
   };
   const char* no_graph = getenv("EMU_NO_GRAPH");
   const bool use_graph = e->use_graphs && !(no_graph && no_graph[0] == '1');
   auto key = std::make_tuple((const void*)latents, (const void*)ctxv, (const void*)text_embeds,
-                             ms ? (const void*)state : (const void*)time_ids, B, h, w * 4 + cfg + 2 * split, L);
+                             ms ? (const void*)state : (const void*)time_ids, (const void*)slot_params, (const void*)slot_live,
+                             B, h, w * 4 + cfg + 2 * split, L);
   auto it = m->graphs.find(key);
   if (use_graph && it != m->graphs.end()) {
     if (cudaGraphLaunch(it->second, st) != cudaSuccess) return e->fail(EMU_ERR_CUDA, "denoise graph launch failed");
@@ -836,13 +849,23 @@ static int denoise_step_impl(EmuEngine* e, float* latents, float sigma, float si
 extern "C" int emu_denoise_step(EmuEngine* e, float* latents, float sigma, float sigma_next, float timestep,
                                 float guidance, const void* ctxv, int L, const void* text_embeds,
                                 const int32_t* time_ids, int B, int h, int w, emu_stream_t stream) {
-  return denoise_step_impl(e, latents, sigma, sigma_next, timestep, guidance, nullptr, nullptr, ctxv, L, text_embeds, time_ids,
-                           B, h, w, stream);
+  return denoise_step_impl(e, latents, sigma, sigma_next, timestep, guidance, nullptr, nullptr, nullptr, nullptr, ctxv, L,
+                           text_embeds, time_ids, B, h, w, stream);
 }
 
 extern "C" int emu_denoise_step_multistep(EmuEngine* e, float* latents, float* state, const float* host_coef8, float timestep,
                                           float guidance, const void* ctxv, int L, int B, int h, int w, emu_stream_t stream) {
   if (!state || !host_coef8) return EMU_ERR_INVALID;
-  return denoise_step_impl(e, latents, 0.f, 0.f, timestep, guidance, host_coef8, state, ctxv, L, nullptr, nullptr, B, h, w,
-                           stream);
+  return denoise_step_impl(e, latents, 0.f, 0.f, timestep, guidance, host_coef8, state, nullptr, nullptr, ctxv, L, nullptr,
+                           nullptr, B, h, w, stream);
+}
+
+extern "C" int emu_denoise_step_slots(EmuEngine* e, float* latents, const float* params, const int32_t* live, const void* ctxv,
+                                      int L, const void* text_embeds, const int32_t* time_ids, int B, int h, int w,
+                                      emu_stream_t stream) {
+  // every argument before the engine is touched
+  if (!e || !latents || !params || !live || !ctxv || !text_embeds || !time_ids) return EMU_ERR_INVALID;
+  if (B < 1 || B > kMaxLatentSlots || L < 1 || h < 1 || w < 1) return EMU_ERR_INVALID;
+  return denoise_step_impl(e, latents, 0.f, 0.f, 0.f, 0.f, nullptr, nullptr, params, live, ctxv, L, text_embeds, time_ids, B,
+                           h, w, stream);
 }

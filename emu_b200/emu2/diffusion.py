@@ -220,24 +220,39 @@ class EmuVisualGeneration:
     def denoise(self, prompt_embeds, batch_size, height=1024, width=1024, num_inference_steps=50, guidance_scale=3.,
                 crop_info=(0, 0), original_size=(1024, 1024), generator=None, latents=None):
         """Steps 2-4 of the reference forward (time ids, pooled text embedding, timesteps, latents, denoise loop)."""
-        dev = self.device_
-        do_cfg = guidance_scale > 1.0
-        B2 = prompt_embeds.shape[0]
-        time_ids = torch.tensor(list(original_size) + list(crop_info) + [height, width], dtype=torch.int32, device=dev)
-        time_ids = time_ids[None].expand(B2, -1).contiguous()
-        text_embeds = prompt_embeds.float().mean(dim=1).to(torch.bfloat16).contiguous()  # diffusion.py:113
+        ctx, text_embeds, time_ids = self.conditioning(prompt_embeds, height, width, crop_info, original_size)
+        ts, sig, init_noise_sigma = self.schedule(num_inference_steps)
+        latents = self.initial_latents(batch_size, height, width, init_noise_sigma, generator=generator, latents=latents)
+        for i in range(num_inference_steps):
+            self.engine.denoise_step(latents, float(sig[i]), float(sig[i + 1]), float(ts[i]), guidance_scale,
+                                     ctx, text_embeds, time_ids)
+        return latents
+
+    # ---- the per-request pieces of `denoise`, shared with emu_b200.batching.DenoiseSlotScheduler ----
+    def schedule(self, num_inference_steps):
+        """this request's Euler schedule: (timesteps [n], sigmas [n + 1], init_noise_sigma)"""
         self.scheduler.set_timesteps(num_inference_steps)
-        ts, sig = self.scheduler.timesteps, self.scheduler.sigmas
+        return self.scheduler.timesteps, self.scheduler.sigmas, self.scheduler.init_noise_sigma
+
+    def conditioning(self, prompt_embeds, height, width, crop_info=(0, 0), original_size=(1024, 1024)):
+        """the UNet conditioning of the rows of prompt_embeds [rows, L, Cc]: (ctx bf16, text_embeds = the mean over tokens
+        (diffusion.py:113), time_ids int32 [rows, 6] from original_size, crop_info and the output size)"""
+        ctx = prompt_embeds.to(torch.bfloat16).contiguous()
+        time_ids = torch.tensor(list(original_size) + list(crop_info) + [height, width], dtype=torch.int32, device=self.device_)
+        time_ids = time_ids[None].expand(ctx.shape[0], -1).contiguous()
+        text_embeds = ctx.float().mean(dim=1).to(torch.bfloat16).contiguous()
+        return ctx, text_embeds, time_ids
+
+    def initial_latents(self, batch_size, height, width, init_noise_sigma, generator=None, latents=None):
+        """the starting latents [batch_size, C, h, w] fp32: drawn (or given), rounded through bf16 and scaled by
+        init_noise_sigma"""
+        dev = self.device_
         h, w = height // self.vae_scale_factor, width // self.vae_scale_factor
         if latents is None:
             latents = torch.randn((batch_size, self.unet_config["in_channels"], h, w), generator=generator,
                                   device=dev if generator is None or generator.device.type == "cuda" else "cpu",
                                   dtype=torch.float32).to(dev)
-        latents = (latents.to(torch.bfloat16).float() * self.scheduler.init_noise_sigma).contiguous()
-        for i in range(num_inference_steps):
-            self.engine.denoise_step(latents, float(sig[i]), float(sig[i + 1]), float(ts[i]), guidance_scale,
-                                     prompt_embeds, text_embeds, time_ids)
-        return latents
+        return (latents.to(torch.bfloat16).float() * init_noise_sigma).contiguous()
 
     # ---- boundary: Emu2/emu/diffusion.py:168-212 (same inputs, same two modes, same cache keys) ----
     def _split_prompt(self, inputs, placeholder):

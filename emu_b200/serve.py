@@ -20,7 +20,9 @@ cache rows in lock-step (one `cur_len`), so a request cannot join a batch that i
 
 Opt-in continuous batching for chat (`EmuServer(chat_scheduler="continuous")`, `--continuous-batching`): a ContinuousWorker
 runs the pipeline's model under emu_b200/batching.py's SlotScheduler instead — requests join the decode batch between two
-steps and leave it as soon as they are finished, each with its own knobs.  Single GPU only.
+steps and leave it as soon as they are finished, each with its own knobs.  Single GPU only.  The same for image generation
+(`EmuServer(generate_scheduler="continuous")`, `--continuous-generation`): a ContinuousWorker drives a DenoiseSlotScheduler,
+whose latent slots join and leave between UNet steps, each request with its own step count and guidance.
 
 With tensor parallelism (launched under torchrun, one process per GPU) rank 0 serves HTTP and broadcasts every admitted batch;
 the other ranks run `follow()` and execute the same calls, which is what the engine's collectives need.
@@ -165,31 +167,53 @@ class BatchingWorker(threading.Thread):
                 r.done.set()
 
 
-class ContinuousWorker(threading.Thread):
-    """One chat pipeline (an EmuChatGeneration) under continuous batching: its thread owns the pipeline's engine and loops
-    SlotScheduler.step() while anything is live or queued, and blocks on the queue when idle.  Same submit / stop surface as
-    BatchingWorker.  A request that fails (prompt assembly, embedding, selection) answers with its own error and frees its
-    slots; the others continue.  `n_slots`: KV-cache slots (default: the engine's llm_max_batch).  `make_request(pipeline,
-    inputs, knobs) -> SlotRequest` turns a submitted request into scheduler work (default: batching.chat_request)."""
+def chat_scheduler(pipeline, n_slots):
+    from .batching import SlotScheduler
+    return SlotScheduler(pipeline.emu_model, n_slots)
 
-    def __init__(self, pipeline, n_slots=None, name=None, make_request=None):
-        super().__init__(daemon=True, name=name or "emu-chat-continuous")
+
+def chat_slot_request(pipeline, inputs, knobs):
+    from .batching import chat_request
+    return chat_request(pipeline, inputs, **knobs)
+
+
+def generate_scheduler_for(pipeline, n_slots):
+    """latent slots at the size the demo form always gets: forward's default 1024x1024"""
+    from .batching import DenoiseSlotScheduler
+    return DenoiseSlotScheduler(pipeline, n_slots or 4)
+
+
+def generate_slot_request(pipeline, inputs, knobs):
+    from .batching import ImageRequest
+    return ImageRequest(inputs=inputs, **knobs)
+
+
+class ContinuousWorker(threading.Thread):
+    """One pipeline under continuous batching: its thread owns the pipeline's engine and loops the scheduler's step() while
+    anything is live or queued, and blocks on the queue when idle.  Same submit / stop surface as BatchingWorker.  A request
+    that fails (prompt assembly, encoding, selection) answers with its own error and frees its slots; the others continue.
+    `make_scheduler(pipeline, n_slots)` builds the scheduler it drives (default: chat's SlotScheduler; generate_scheduler
+    for image generation) and `make_request(pipeline, inputs, knobs)` turns a submitted request into that scheduler's work
+    (default: batching.chat_request).  `n_slots`: the scheduler's slots (chat default: the engine's llm_max_batch)."""
+
+    def __init__(self, pipeline, n_slots=None, name=None, make_request=None, make_scheduler=None, kind="chat"):
+        super().__init__(daemon=True, name=name or "emu-%s-continuous" % kind)
         self.pipeline, self.n_slots = pipeline, n_slots
-        self.make_request = make_request
-        self.kind = "chat"
+        self.make_request = make_request or chat_slot_request
+        self.make_scheduler = make_scheduler or chat_scheduler
+        self.kind = kind
         self.q = queue.Queue()
         self.scheduler = None
         self._halt = threading.Event()
 
     def start(self):
-        """enter slot mode before the thread starts: an engine that cannot (EMU_KV_COPY=1, tensor parallel) fails here, in
-        the caller, instead of leaving a dead worker behind a queue"""
-        from .batching import SlotScheduler
-        self.scheduler = SlotScheduler(self.pipeline.emu_model, self.n_slots)
+        """build the scheduler before the thread starts: an engine that cannot run it (EMU_KV_COPY=1, tensor parallel) fails
+        here, in the caller, instead of leaving a dead worker behind a queue"""
+        self.scheduler = self.make_scheduler(self.pipeline, self.n_slots)
         super().start()
 
     def load(self):
-        """queued + waiting for slots + decoding"""
+        """queued + waiting for slots + running"""
         return self.q.qsize() + (self.scheduler.load() if self.scheduler is not None else 0)
 
     def submit(self, inputs, knobs, log_id="", timeout=None):
@@ -206,19 +230,16 @@ class ContinuousWorker(threading.Thread):
         self.q.put(None)
 
     def _admit(self, r):
-        from .batching import chat_request
-        make = self.make_request or (lambda pipe, inputs, knobs: chat_request(pipe, inputs, **knobs))
-
         def answer(sr, r=r):
             r.result, r.error = sr.result, sr.error
-            log.info("%s: chat done in %.1f ms", r.log_id, (time.time() - r.t_in) * 1e3)
+            log.info("%s: %s done in %.1f ms", r.log_id, self.kind, (time.time() - r.t_in) * 1e3)
             r.done.set()
         try:
-            sr = make(self.pipeline, r.inputs, r.knobs)
+            sr = self.make_request(self.pipeline, r.inputs, r.knobs)
             sr.on_done, sr.tag = answer, r.log_id
             self.scheduler.submit(sr)
         except Exception as ex:  # the request fails, the server lives
-            log.error("%s: chat request refused: %s\n%s", r.log_id, ex, traceback.format_exc())
+            log.error("%s: %s request refused: %s\n%s", r.log_id, self.kind, ex, traceback.format_exc())
             r.error = ex
             r.done.set()
 
@@ -306,11 +327,14 @@ def image_to_webp_b64(image):
 
 
 class EmuServer:
-    """HTTP front + one BatchingWorker per pipeline.  `chat` / `generate`: a pipeline or a list of pipelines (the reference's
-    --chat-concurrency / --generate-concurrency instances); requests go to the worker with the shortest queue."""
+    """HTTP front + one worker per pipeline.  `chat` / `generate`: a pipeline or a list of pipelines (the reference's
+    --chat-concurrency / --generate-concurrency instances); requests go to the worker with the shortest queue.
+    `chat_scheduler` / `generate_scheduler`: "batching" (BatchingWorker, the default) or "continuous" (ContinuousWorker; for
+    generation with max_images_per_batch latent slots)."""
 
     def __init__(self, chat=None, generate=None, host="0.0.0.0", port=9000, max_wait_ms=0.0, max_images_per_batch=4,
-                 cache_dir=None, announce=None, max_body_bytes=256 << 20, chat_scheduler="batching"):
+                 cache_dir=None, announce=None, max_body_bytes=256 << 20, chat_scheduler="batching",
+                 generate_scheduler="batching"):
         self.cache_dir = cache_dir
         self.max_body_bytes = int(max_body_bytes)
         if cache_dir:
@@ -332,9 +356,16 @@ class EmuServer:
         else:
             raise ValueError("chat_scheduler must be 'batching' or 'continuous', got %r" % (chat_scheduler,))
         # (no announce for generation: the UNet is not tensor parallel, follower ranks hold no generation pipeline)
-        self.gen_workers = [BatchingWorker(p, "generate", (lambda knobs: max_images_per_batch)
-                                           if hasattr(p, "forward_batch") else None, max_wait_ms, None, "emu-gen-%d" % i)
-                            for i, p in enumerate(as_list(generate))]
+        if generate_scheduler == "continuous":
+            self.gen_workers = [ContinuousWorker(p, max_images_per_batch, "emu-gen-%d" % i, generate_slot_request,
+                                                 generate_scheduler_for, "generate")
+                                for i, p in enumerate(as_list(generate))]
+        elif generate_scheduler == "batching":
+            self.gen_workers = [BatchingWorker(p, "generate", (lambda knobs: max_images_per_batch)
+                                               if hasattr(p, "forward_batch") else None, max_wait_ms, None, "emu-gen-%d" % i)
+                                for i, p in enumerate(as_list(generate))]
+        else:
+            raise ValueError("generate_scheduler must be 'batching' or 'continuous', got %r" % (generate_scheduler,))
         server = self
 
         class Handler(BaseHTTPRequestHandler):
@@ -474,6 +505,9 @@ def main(argv=None):
     ap.add_argument("--max-images-per-batch", type=int, default=4)
     ap.add_argument("--continuous-batching", action="store_true",
                     help="chat requests join and leave the decode batch between steps (one GPU per chat instance)")
+    ap.add_argument("--continuous-generation", action="store_true",
+                    help="image requests join and leave the denoise batch between UNet steps, in --max-images-per-batch "
+                         "latent slots")
     ap.add_argument("--cache-dir", type=str, default="", help="keep request pictures / results here (the reference always does)")
     ap.add_argument("--safety-checker", action="store_true",
                     help="run the built-in NSFW safety checker (the checkpoint's safety_checker.* weights) on every generated "
@@ -531,7 +565,8 @@ def main(argv=None):
     srv = EmuServer(chat=chat, generate=gen, host=args.host, port=args.port, max_wait_ms=args.max_wait_ms,
                     max_images_per_batch=args.max_images_per_batch, cache_dir=args.cache_dir or None,
                     announce=make_announce() if world > 1 else None,
-                    chat_scheduler="continuous" if args.continuous_batching else "batching")
+                    chat_scheduler="continuous" if args.continuous_batching else "batching",
+                    generate_scheduler="continuous" if args.continuous_generation else "batching")
     log.info("serving on %s:%d (chat x%d, generate x%d)", args.host, srv.port, len(chat), len(gen))
     try:
         srv.serve_forever()
