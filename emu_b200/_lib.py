@@ -82,6 +82,10 @@ OPS_SYMBOLS = ["emu_op_attn_decode_rows", "emu_op_rope_kv_write", "emu_op_kv_ind
                "emu_op_argmax_rows", "emu_op_attn_prefill_rows"]
 # ... and in include/emu_b200_gen_slots.h (latent slots: continuous batching for image generation)
 GEN_SLOT_SYMBOLS = ["emu_denoise_step_slots", "emu_op_denoise_prepare", "emu_op_denoise_euler"]
+# ... and in include/emu_b200_diffusion_ops.h (the diffusion kernels as stand-alone operators)
+DIFFUSION_OPS_SYMBOLS = ["emu_op_groupnorm", "emu_op_timestep_embedding", "emu_op_upsample2x", "emu_op_im2col3x3",
+                         "emu_op_copy_cols", "emu_op_nchw_to_nhwc", "emu_op_nhwc_to_nchw", "emu_op_mean_tokens",
+                         "emu_op_vae_post", "emu_op_denoise_multistep", "emu_op_vae_attention"]
 
 _lib = None
 
@@ -744,6 +748,124 @@ def op_denoise_euler(latents, eps_nhwc, params, live=None, slots_adjacent=False)
     cs, ub = _rows_layout(B, slots_adjacent)
     check(load().emu_op_denoise_euler(_ptr(latents), _ptr(eps_nhwc), _i32(live, "live"), B, Cc, h * w, eps_nhwc.shape[-1],
                                       _ptr(params), 4 if params.dim() == 2 else 0, cs, ub, _stream()))
+
+
+# ---- the diffusion kernels (include/emu_b200_diffusion_ops.h) ----
+def _c_float(v):
+    return C.c_float(float(v))
+
+
+def _bf16c(t, name):
+    if t.dtype != torch.bfloat16 or not t.is_contiguous():
+        raise ValueError("%s must be a contiguous bf16 tensor" % name)
+    return _ptr(t)
+
+
+def op_groupnorm(x, w, b, groups, eps, silu=False, out=None):
+    """x [NB, HW, C] (or [NB, H, W, C]) NHWC bf16; w, b [C] bf16 -> GroupNorm (+SiLU), same shape (written into out if given)"""
+    require_cuda()
+    NB, Cc = x.shape[0], x.shape[-1]
+    HW = x.numel() // (NB * Cc)
+    y = torch.empty_like(x) if out is None else out
+    check(load().emu_op_groupnorm(_bf16c(x, "x"), _bf16c(w, "w"), _bf16c(b, "b"), _bf16c(y, "out"), NB, HW, Cc, int(groups),
+                                  _c_float(eps), 1 if silu else 0, _stream()))
+    return y
+
+
+def op_timestep_embedding(t, out, dim, col_off=0, grp=1):
+    """t fp32 [rows] -> [cos | sin] embeddings of width dim written into out bf16 [rows / grp, ld] at columns
+    col_off + (r % grp) * dim of output row r / grp"""
+    require_cuda()
+    assert t.dtype == torch.float32 and t.is_contiguous()
+    check(load().emu_op_timestep_embedding(_ptr(t), _bf16c(out, "out"), t.numel(), int(dim), out.stride(0), int(col_off),
+                                           int(grp), _stream()))
+    return out
+
+
+def op_upsample2x(x, out=None):
+    """x [NB, H, W, C] bf16 -> [NB, 2H, 2W, C], nearest"""
+    require_cuda()
+    NB, H, W, Cc = x.shape
+    y = torch.empty(NB, 2 * H, 2 * W, Cc, dtype=x.dtype, device=x.device) if out is None else out
+    check(load().emu_op_upsample2x(_bf16c(x, "x"), _ptr(y), NB, H, W, Cc, _stream()))
+    return y
+
+
+def op_im2col3x3(x, stride, out=None):
+    """x [NB, H, W, C] bf16 -> [NB, Ho, Wo, 9 C] (3x3 taps, pad 1)"""
+    require_cuda()
+    NB, H, W, Cc = x.shape
+    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+    y = torch.empty(NB, Ho, Wo, 9 * Cc, dtype=x.dtype, device=x.device) if out is None else out
+    check(load().emu_op_im2col3x3(_bf16c(x, "x"), _ptr(y), NB, H, W, Cc, int(stride), _stream()))
+    return y
+
+
+def op_copy_cols(src, dst, col_off):
+    """dst[:, col_off:col_off + src.shape[1]] = src (2-D bf16 views with unit column stride) in place"""
+    require_cuda()
+    assert src.dtype == dst.dtype == torch.bfloat16 and src.stride(1) == 1 and dst.stride(1) == 1
+    check(load().emu_op_copy_cols(_ptr(src), _ptr(dst), C.c_int64(src.shape[0]), src.shape[1], src.stride(0), dst.stride(0),
+                                  int(col_off), _stream()))
+
+
+def op_nchw_to_nhwc(x, Cp, scale=1.0, out=None):
+    """x [NB, C, H, W] bf16 -> [NB, H, W, Cp] bf16(x * scale), zero channels past C"""
+    require_cuda()
+    NB, Cc, H, W = x.shape
+    y = torch.empty(NB, H, W, Cp, dtype=x.dtype, device=x.device) if out is None else out
+    check(load().emu_op_nchw_to_nhwc(_bf16c(x, "x"), _ptr(y), NB, Cc, H * W, int(Cp), _c_float(scale), _stream()))
+    return y
+
+
+def op_nhwc_to_nchw(x, Cc, out=None):
+    """x [NB, H, W, ld] bf16 -> its first Cc channels as [NB, Cc, H, W]"""
+    require_cuda()
+    NB, H, W, ld = x.shape
+    y = torch.empty(NB, Cc, H, W, dtype=x.dtype, device=x.device) if out is None else out
+    check(load().emu_op_nhwc_to_nchw(_bf16c(x, "x"), _ptr(y), NB, int(Cc), H * W, ld, _stream()))
+    return y
+
+
+def op_mean_tokens(x, out=None):
+    """x [B, L, C] bf16 -> [B, C], the mean over L"""
+    require_cuda()
+    B, L, Cc = x.shape
+    y = torch.empty(B, Cc, dtype=x.dtype, device=x.device) if out is None else out
+    check(load().emu_op_mean_tokens(_bf16c(x, "x"), _ptr(y), B, L, Cc, _stream()))
+    return y
+
+
+def op_vae_post(x, Cc, out=None):
+    """x [..., ld] bf16 -> fp32 [..., Cc] = clamp(x / 2 + 0.5, 0, 1) of the first Cc channels"""
+    require_cuda()
+    ld = x.shape[-1]
+    n_pix = x.numel() // ld
+    y = torch.empty(*x.shape[:-1], Cc, dtype=torch.float32, device=x.device) if out is None else out
+    check(load().emu_op_vae_post(_bf16c(x, "x"), _ptr(y), C.c_int64(n_pix), int(Cc), ld, _stream()))
+    return y
+
+
+def op_denoise_multistep(latents, eps_nhwc, hist, saved, params, cfg):
+    """latents, saved [B, C, h, w] fp32 and hist [3, B, C, h, w] fp32 updated in place from eps NHWC bf16 [B or 2B, h, w, ld];
+    params fp32 [8] on the device (layout at emu_op_denoise_multistep)"""
+    require_cuda()
+    B, Cc, h, w = latents.shape
+    for t, n in ((latents, "latents"), (hist, "hist"), (saved, "saved"), (params, "params")):
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError("%s must be a contiguous fp32 tensor" % n)
+    check(load().emu_op_denoise_multistep(_ptr(latents), _bf16c(eps_nhwc, "eps"), _ptr(hist), _ptr(saved), B, Cc, h * w,
+                                          eps_nhwc.shape[-1], _ptr(params), 1 if cfg else 0, _stream()))
+
+
+def op_vae_attention(q, k, v, out=None):
+    """q, k, v [B, T, C] bf16 -> softmax(q k^T / sqrt(C)) v, [B, T, C]"""
+    require_cuda()
+    B, T, Cc = q.shape
+    assert k.shape == v.shape == q.shape
+    out = torch.empty_like(q) if out is None else out
+    check(load().emu_op_vae_attention(_bf16c(q, "q"), _bf16c(k, "k"), _bf16c(v, "v"), _ptr(out), B, T, Cc, _stream()))
+    return out
 
 
 def op_rmsnorm(x, w, eps):

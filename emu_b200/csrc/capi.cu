@@ -4,6 +4,7 @@
 #include "engine.h"
 #include "../../include/emu_b200_ops.h"
 #include "../../include/emu_b200_gen_slots.h"
+#include "../../include/emu_b200_diffusion_ops.h"
 #include "diffusion_common.h"
 
 using namespace emu;
@@ -256,4 +257,102 @@ extern "C" int emu_op_denoise_euler(float* latents, const void* eps, const int32
   if (!denoise_glue_args_ok(B, C, HW, ps, cs, ub) || ld < C) return EMU_ERR_INVALID;
   count_launch();
   return slot_cfg_euler(latents, (const bf16*)eps, live, B, C, HW, ld, params, ps, cs, ub, (cudaStream_t)s);
+}
+
+// ---- the diffusion kernels (include/emu_b200_diffusion_ops.h): the engine's launchers at any shape, arguments checked first ----
+// a device workspace owned by one entry point, grown on demand (cudaFree waits for the work that still uses the old one)
+static int grow_workspace(void** buf, size_t* cap, size_t need) {
+  if (need <= *cap) return EMU_OK;
+  if (*buf) cudaFree(*buf);
+  *buf = nullptr;
+  *cap = 0;
+  if (cudaMalloc(buf, need) != cudaSuccess) return EMU_ERR_NOMEM;
+  *cap = need;
+  return EMU_OK;
+}
+
+extern "C" int emu_op_groupnorm(const void* x, const void* w, const void* b, void* y, int NB, int HW, int C, int groups,
+                                float eps, int silu, emu_stream_t s) {
+  if (!x || !w || !b || !y) return EMU_ERR_INVALID;
+  if (NB < 1 || HW < 1 || C < 1 || groups < 1 || C % 8 || C % groups || C > 4096) return EMU_ERR_INVALID;
+  static void* scratch = nullptr;
+  static size_t cap = 0;
+  EMU_TRY(grow_workspace(&scratch, &cap, groupnorm_scratch_bytes(NB, groups)));
+  count_launch(2);
+  return groupnorm_nhwc((const bf16*)x, (const bf16*)w, (const bf16*)b, (bf16*)y, (float*)scratch, NB, HW, C, groups, eps,
+                        silu ? 1 : 0, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_timestep_embedding(const float* t, void* out, int rows, int dim, int ld, int col_off, int grp,
+                                         emu_stream_t s) {
+  if (!t || !out) return EMU_ERR_INVALID;
+  if (rows < 1 || dim < 2 || dim % 2 || grp < 1 || col_off < 0 || (long)ld < (long)col_off + (long)grp * dim)
+    return EMU_ERR_INVALID;
+  count_launch();
+  return timestep_embedding(t, (bf16*)out, rows, dim, ld, col_off, grp, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_upsample2x(const void* x, void* y, int NB, int H, int W, int C, emu_stream_t s) {
+  if (!x || !y || NB < 1 || H < 1 || W < 1 || C < 1 || C % 8) return EMU_ERR_INVALID;
+  count_launch();
+  return upsample2x_nhwc((const bf16*)x, (bf16*)y, NB, H, W, C, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_im2col3x3(const void* x, void* out, int NB, int H, int W, int C, int stride, emu_stream_t s) {
+  if (!x || !out || NB < 1 || H < 1 || W < 1 || C < 1 || C % 8) return EMU_ERR_INVALID;
+  if (stride != 1 && stride != 2) return EMU_ERR_INVALID;
+  count_launch();
+  return im2col3x3((const bf16*)x, (bf16*)out, NB, H, W, C, stride, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_copy_cols(const void* src, void* dst, int64_t rows, int cols, int lds, int ldd, int col_off,
+                                emu_stream_t s) {
+  if (!src || !dst || rows < 1 || cols < 1 || col_off < 0 || (cols | lds | ldd | col_off) % 8) return EMU_ERR_INVALID;
+  if (lds < cols || (long)ldd < (long)col_off + cols) return EMU_ERR_INVALID;
+  count_launch();
+  return copy_cols((const bf16*)src, (bf16*)dst, rows, cols, lds, ldd, col_off, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_nchw_to_nhwc(const void* x, void* y, int NB, int C, int HW, int Cp, float scale, emu_stream_t s) {
+  if (!x || !y || NB < 1 || C < 1 || HW < 1 || Cp < C) return EMU_ERR_INVALID;
+  count_launch();
+  return nchw_to_nhwc((const bf16*)x, (bf16*)y, NB, C, HW, Cp, scale, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_nhwc_to_nchw(const void* x, void* y, int NB, int C, int HW, int ldx, emu_stream_t s) {
+  if (!x || !y || NB < 1 || C < 1 || HW < 1 || ldx < C) return EMU_ERR_INVALID;
+  count_launch();
+  return nhwc_to_nchw((const bf16*)x, (bf16*)y, NB, C, HW, ldx, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_mean_tokens(const void* x, void* y, int B, int L, int C, emu_stream_t s) {
+  if (!x || !y || B < 1 || L < 1 || C < 1) return EMU_ERR_INVALID;
+  count_launch();
+  return mean_tokens((const bf16*)x, (bf16*)y, B, L, C, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_vae_post(const void* x, float* y, int64_t n_pix, int C, int ldx, emu_stream_t s) {
+  if (!x || !y || n_pix < 1 || C < 1 || ldx < C) return EMU_ERR_INVALID;
+  count_launch();
+  return vae_post((const bf16*)x, y, n_pix, C, ldx, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_denoise_multistep(float* lat, const void* eps, float* hist, float* saved, int B, int C, int HW, int ld,
+                                        const float* params, int cfg, emu_stream_t s) {
+  if (!lat || !eps || !hist || !saved || !params) return EMU_ERR_INVALID;
+  if (B < 1 || C < 1 || HW < 1 || ld < C || (cfg != 0 && cfg != 1)) return EMU_ERR_INVALID;
+  count_launch();
+  return cfg_multistep(lat, (const bf16*)eps, hist, saved, B, C, HW, ld, params, cfg, (cudaStream_t)s);
+}
+
+extern "C" int emu_op_vae_attention(const void* q, const void* k, const void* v, void* out, int B, int T, int C,
+                                    emu_stream_t s) {
+  if (!q || !k || !v || !out || B < 1 || T < 1 || C < 1 || T % 8 || C % 8) return EMU_ERR_INVALID;
+  static void* ws = nullptr;
+  static size_t cap = 0;
+  EMU_TRY(grow_workspace(&ws, &cap, vae_attention_workspace_bytes(T, C)));
+  int nl = 0;
+  const int rc = vae_attention((const bf16*)q, (const bf16*)k, (const bf16*)v, (bf16*)out, B, T, C, ws, (cudaStream_t)s, &nl);
+  count_launch(nl);
+  return rc;
 }

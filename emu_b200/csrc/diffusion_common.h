@@ -94,8 +94,17 @@ int lin_rows(Ctx& c, const bf16* x, int M, const Lin& l, bf16* y, const bf16* re
 int conv3(Ctx& c, const bf16* x, int NB, int H, int W, const Conv& cv, int stride, bf16* y, const bf16* bias2,
           const bf16* residual, int ldy = 0);
 int gnorm(Ctx& c, const bf16* x, const Norm& n, bf16* y, int NB, int HW, float eps, int do_silu);
-int softmax_rows(bf16* s, long rows, int cols, float scale, cudaStream_t st);
+int softmax_rows(const float* s, bf16* p, long rows, int cols, float scale, cudaStream_t st);
 int transpose_2d(const bf16* x, bf16* y, int rows, int cols, cudaStream_t st);
 int vae_post(const bf16* x, float* y, long n_pix, int C, int ldx, cudaStream_t st);
+int mean_tokens(const bf16* x, bf16* y, int B, int L, int C, cudaStream_t st);
+
+// vae.cu: the VAE mid-block attention core, o[b] = softmax(q[b] k[b]^T / sqrt(C)) v[b] for q / k / v / o [B, T, C] bf16
+// (T % 8 == 0, C % 8 == 0), in query-row chunks of vae_attention_chunk_rows(T) over a workspace of
+// vae_attention_workspace_bytes(T, C) (16-byte aligned).  *launches (optional) receives the kernel count.
+int vae_attention_chunk_rows(int T);
+size_t vae_attention_workspace_bytes(int T, int C);
+int vae_attention(const bf16* q, const bf16* k, const bf16* v, bf16* o, int B, int T, int C, void* ws, cudaStream_t st,
+                  int* launches = nullptr);
 
 }  // namespace emu

@@ -14,9 +14,17 @@ namespace emu {
 // ----------------------------------------------------------------------------------------------
 constexpr int kGnChunks = 128;  // partial-sum slots per image (x NB CTAs of 512 threads: ~2 CTAs per SM in flight)
 
+// The sums are taken of x - pivot, the pivot being the first element of the (image, group) plane.  Without the shift,
+// var = E[x^2] - mean^2 in fp32 cancels: its relative error grows as 2^-24 (mean/std)^2 times the summation length, which
+// reaches the bf16 output's own rounding once |mean| is a few hundred standard deviations.  Shifted, mean/std is that of
+// one sample's distance from the mean, so the cancellation is gone while the summation order (and determinism) is kept.
+__device__ __forceinline__ float gn_pivot(const bf16* x_img, int c, int cpg) {
+  return __bfloat162float(x_img[c / cpg * cpg]);
+}
+
 __global__ void __launch_bounds__(512) gn_partial_kernel(const bf16* __restrict__ x, float* __restrict__ part, int HW,
                                                          int C, int groups, int pdl) {
-  // grid (kGnChunks, NB); part[((b*kGnChunks + chunk)*groups + g)*2 + {0,1}] = {sum, sumsq}
+  // grid (kGnChunks, NB); part[((b*kGnChunks + chunk)*groups + g)*2 + {0,1}] = {sum, sumsq} of x - pivot
   __shared__ float stage[512 * 16];  // per-thread {sum[8], sumsq[8]}
   if (pdl) {
     pdl_launch_dependents();
@@ -32,9 +40,12 @@ __global__ void __launch_bounds__(512) gn_partial_kernel(const bf16* __restrict_
     const int cv = threadIdx.x % vecC;
     const long total = (long)(p1 - p0) * vecC;
     const bf16* base = x + ((long)b * HW + p0) * C;
-    float s[8], s2[8];
+    float s[8], s2[8], piv[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) s[j] = s2[j] = 0.f;
+    for (int j = 0; j < 8; ++j) {
+      s[j] = s2[j] = 0.f;
+      piv[j] = gn_pivot(x + (long)b * HW * C, cv * 8 + j, cpg);
+    }
 #pragma unroll 4
     for (long idx = threadIdx.x; idx < total; idx += stride) {
       const long pix = idx / vecC;
@@ -42,7 +53,7 @@ __global__ void __launch_bounds__(512) gn_partial_kernel(const bf16* __restrict_
       const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const float lo = bf16_lo(w[j]), hi = bf16_hi(w[j]);
+        const float lo = bf16_lo(w[j]) - piv[2 * j], hi = bf16_hi(w[j]) - piv[2 * j + 1];
         s[2 * j] += lo; s2[2 * j] += lo * lo;
         s[2 * j + 1] += hi; s2[2 * j + 1] += hi * hi;
       }
@@ -107,9 +118,9 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const bf16* __restrict__ 
         a2 += ps[(q * gw + (int)threadIdx.x) * 2 + 1];
       }
       const float n = (float)HW * cpg;
-      const float mean = a / n;
-      const float var = fmaxf(a2 / n - mean * mean, 0.f);
-      st[g * 2] = mean;
+      const float dmean = a / n;  // mean of x - pivot
+      const float var = fmaxf(a2 / n - dmean * dmean, 0.f);
+      st[g * 2] = gn_pivot(x + (long)b * HW * C, g * cpg, cpg) + dmean;
       st[g * 2 + 1] = rsqrtf(var + eps);
     }
     __syncthreads();
@@ -425,12 +436,14 @@ int mean_tokens(const bf16* x, bf16* y, int B, int L, int C, cudaStream_t st) {
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
-// row softmax over fp32-scaled bf16 scores (VAE mid-block single-head attention, D = 512 > flash tile)
-__global__ void __launch_bounds__(256) softmax_rows_kernel(bf16* s, int cols, float scale) {
+// row softmax of fp32 scores times `scale` -> bf16 probabilities (VAE mid-block single-head attention, D = 512 > flash tile)
+__global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ s, bf16* __restrict__ p, int cols,
+                                                           float scale) {
   __shared__ float red[33];
-  bf16* row = s + (long)blockIdx.x * cols;
+  const float* row = s + (long)blockIdx.x * cols;
+  bf16* prow = p + (long)blockIdx.x * cols;
   float m = -INFINITY;
-  for (int i = threadIdx.x; i < cols; i += blockDim.x) m = fmaxf(m, __bfloat162float(row[i]) * scale);
+  for (int i = threadIdx.x; i < cols; i += blockDim.x) m = fmaxf(m, row[i] * scale);
   m = warp_max(m);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
   __syncthreads();
@@ -438,14 +451,13 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(bf16* s, int cols, fl
   for (int w = 1; w < 8; ++w) m = fmaxf(m, red[w]);
   __syncthreads();
   float l = 0.f;
-  for (int i = threadIdx.x; i < cols; i += blockDim.x) l += __expf(__bfloat162float(row[i]) * scale - m);
+  for (int i = threadIdx.x; i < cols; i += blockDim.x) l += __expf(row[i] * scale - m);
   l = block_sum(l, red);
   const float inv = 1.f / l;
-  for (int i = threadIdx.x; i < cols; i += blockDim.x)
-    row[i] = __float2bfloat16_rn(__expf(__bfloat162float(row[i]) * scale - m) * inv);
+  for (int i = threadIdx.x; i < cols; i += blockDim.x) prow[i] = __float2bfloat16_rn(__expf(row[i] * scale - m) * inv);
 }
-int softmax_rows(bf16* s, long rows, int cols, float scale, cudaStream_t st) {
-  softmax_rows_kernel<<<(unsigned)rows, 256, 0, st>>>(s, cols, scale);
+int softmax_rows(const float* s, bf16* p, long rows, int cols, float scale, cudaStream_t st) {
+  softmax_rows_kernel<<<(unsigned)rows, 256, 0, st>>>(s, p, cols, scale);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 

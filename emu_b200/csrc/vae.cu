@@ -6,8 +6,8 @@
 // ("parity unpinned").  The pipeline runs the VAE in bf16 (force_upcast is not honoured by the reference pipeline).
 //
 // Same building blocks as the UNet: NHWC bf16, wgmma implicit-GEMM 3x3 convs, 2-kernel GroupNorm+SiLU.  The
-// mid-block attention is single-head with head_dim = 512 (> the flash tile), so it is three GEMMs on wgmma
-// (S = Q K^T, O = P V with V transposed once) around a row-softmax kernel; it runs once per image.
+// mid-block attention is single-head with head_dim = 512 (> the flash tile), so it is two GEMMs on wgmma
+// (S = Q K^T in fp32, O = P V with V transposed once) around a row-softmax kernel (vae_attention below).
 #include <math.h>
 
 #include "diffusion_common.h"
@@ -64,6 +64,48 @@ static int vae_resnet(Ctx& c, const VaeResnet& r, const bf16* x, bf16* y, int NB
     shortcut = sc;
   }
   return conv3(c, g, NB, H, W, r.c2, 1, y, nullptr, shortcut);
+}
+
+// The mid-block attention core.  The scores stay fp32, as torch SDPA keeps them: the S GEMM writes fp32 and softmax_rows
+// scales them and writes bf16 P.  Rounding S to bf16 first moves every logit by up to 2^-9 of its size before the
+// exponential, which at logit spreads of a few units costs several times bf16's own error in the output.  Query rows run
+// in chunks so the fp32 scores take at most 256 MB (T = 16384: 4 chunks of 4096 rows).
+static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+int vae_attention_chunk_rows(int T) {
+  const long r = (1L << 26) / T;
+  return (int)(r < 1 ? 1 : r > T ? T : r);
+}
+size_t vae_attention_workspace_bytes(int T, int C) {
+  const size_t rows = (size_t)vae_attention_chunk_rows(T);
+  return align256((size_t)C * T * sizeof(bf16)) + align256(rows * T * sizeof(float)) + rows * T * sizeof(bf16);
+}
+int vae_attention(const bf16* q, const bf16* k, const bf16* v, bf16* o, int B, int T, int C, void* ws, cudaStream_t st,
+                  int* launches) {
+  const int rows = vae_attention_chunk_rows(T);
+  bf16* vt = (bf16*)ws;                                                                  // V^T [C, T]
+  float* s = (float*)((char*)ws + align256((size_t)C * T * sizeof(bf16)));                // S [rows, T] fp32
+  bf16* p = (bf16*)((char*)s + align256((size_t)rows * T * sizeof(float)));              // P [rows, T]
+  const float scale = 1.0f / sqrtf((float)C);
+  int nl = 0;
+  for (int bi = 0; bi < B; ++bi) {
+    const bf16* qb = q + (size_t)bi * T * C;
+    const bf16* kb = k + (size_t)bi * T * C;
+    EMU_TRY(transpose_2d(v + (size_t)bi * T * C, vt, T, C, st));  // K-major V for the P V GEMM
+    ++nl;
+    for (int r0 = 0; r0 < T; r0 += rows) {
+      const int n = T - r0 < rows ? T - r0 : rows;
+      GemmEpilogue es;
+      es.C = s; es.ldc = T; es.out_fp32 = 1;
+      EMU_TRY(gemm_bf16(qb + (size_t)r0 * C, C, kb, C, n, T, C, es, st));  // S = Q K^T
+      EMU_TRY(softmax_rows(s, p, n, T, scale, st));                       // P = softmax(S / sqrt(C))
+      GemmEpilogue eo;
+      eo.C = o + ((size_t)bi * T + r0) * C; eo.ldc = C;
+      EMU_TRY(gemm_bf16(p, T, vt, T, n, C, T, eo, st));                   // O = P V
+      nl += 3;
+    }
+  }
+  if (launches) *launches = nl;
+  return EMU_OK;
 }
 
 }  // namespace emu
@@ -141,30 +183,20 @@ extern "C" int emu_vae_decode(EmuEngine* e, const void* latents_nchw, int B, int
     BUF(q, "v_q", M0 * C);
     BUF(k, "v_k", M0 * C);
     BUF(v, "v_v", M0 * C);
-    BUF(vt, "v_vt", (size_t)C * T);
-    BUF(s, "v_s", (size_t)T * T);
-    BUF(o, "v_o", (size_t)T * C);
+    BUF(o, "v_o", M0 * C);
+    BUF(ws, "v_attn_ws", (vae_attention_workspace_bytes(T, C) + 1) / 2);
     EMU_TRY(gnorm(c, b, m->attn_gn, n, B, T, 1e-6f, 0));
     EMU_TRY(lin_rows(c, n, (int)M0, m->aq, q));
     EMU_TRY(lin_rows(c, n, (int)M0, m->ak, k));
     EMU_TRY(lin_rows(c, n, (int)M0, m->av, v));
-    for (int bi = 0; bi < B; ++bi) {
-      const bf16* qb = q + (size_t)bi * T * C;
-      const bf16* kb = k + (size_t)bi * T * C;
-      const bf16* vb = v + (size_t)bi * T * C;
-      GemmEpilogue es;
-      es.C = s; es.ldc = T;
-      EMU_TRY(gemm_bf16(qb, C, kb, C, T, T, C, es, st));          // S = Q K^T
-      EMU_TRY(softmax_rows(s, T, T, 1.0f / sqrtf((float)C), st));  // P = softmax(S / sqrt(C))
-      EMU_TRY(transpose_2d(vb, vt, T, C, st));                     // V^T [C, T] (K-major for the second GEMM)
-      GemmEpilogue eo;
-      eo.C = o; eo.ldc = C;
-      EMU_TRY(gemm_bf16(s, T, vt, T, T, C, T, eo, st));            // O = P V
-      // to_out + residual (b) -> a
+    int nl = 0;
+    EMU_TRY(vae_attention(q, k, v, o, B, T, C, ws, st, &nl));
+    c.nl += nl;
+    for (int bi = 0; bi < B; ++bi) {  // to_out + residual (b) -> a
       GemmEpilogue ef;
       ef.C = a + (size_t)bi * T * C; ef.ldc = C; ef.bias = m->ao.b; ef.residual = b + (size_t)bi * T * C; ef.ldr = C;
-      EMU_TRY(gemm_bf16(o, C, m->ao.w, C, T, C, C, ef, st));
-      c.nl += 5;
+      EMU_TRY(gemm_bf16(o + (size_t)bi * T * C, C, m->ao.w, C, T, C, C, ef, st));
+      ++c.nl;
     }
   }
   EMU_TRY(vae_resnet(c, m->mid1, a, b, B, H, W));

@@ -392,11 +392,13 @@ def vae_resnet(sd, p, x, groups):
 
 
 def vae_mid_attention(sd, p, x, groups):
-    """diffusers Attention inside UNetMidBlock2D of the VAE: single head over C, GroupNorm, q/k/v/out WITH bias."""
+    """diffusers Attention inside UNetMidBlock2D of the VAE: single head over C, GroupNorm, q/k/v/out WITH bias.  diffusers
+    runs it through torch SDPA (AttnProcessor2_0), whose kernels keep the scores and the softmax in fp32 for bf16 inputs, so
+    the bf16 policy here does the same: fp32 scores, probabilities rounded to the activation dtype before P V."""
     B, C, H, W = x.shape
     h = group_norm(sd, p + "group_norm", x, groups, 1e-6).view(B, C, H * W).transpose(1, 2)
     q, k, v = linear(sd, p + "to_q", h), linear(sd, p + "to_k", h), linear(sd, p + "to_v", h)
-    w = torch.softmax((q @ k.transpose(-1, -2)) * C ** -0.5, dim=-1)
+    w = torch.softmax((q.float() @ k.float().transpose(-1, -2)) * C ** -0.5, dim=-1).to(v.dtype)
     o = linear(sd, p + "to_out.0", w @ v)
     return o.transpose(1, 2).reshape(B, C, H, W) + x
 

@@ -166,3 +166,42 @@ def test_unet_stages_c640_c1280(cuda):
     out = eng.unet_forward(x.cuda(), 981.0, ctx.cuda(), te.cuda(), tid.cuda()).float().cpu()
     report("unet stages C=640/1280", out, ref32, ref16)
     eng.close()
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# SDXL VAE decoder at its published width (Emu2/emu/conf/diffusion_config/vae/config.json: 128/256/512/512, 2 layers per
+# block, 32 groups) on 128x128 latents -> one 1024x1024 image: GroupNorm on planes up to 1024^2 and the mid-block attention
+# over 16384 tokens of width 512.  The oracle runs on the GPU here (the CPU would take minutes at this size).
+# ------------------------------------------------------------------------------------------------------------------
+VAE_FULL = dict(latent_channels=4, out_channels=3, block_out_channels=(128, 256, 512, 512), layers_per_block=2,
+                norm_num_groups=32)
+
+
+def test_vae_decoder_real_width_128_latents(cuda):
+    from emu_b200 import _lib
+    cfg = VAE_FULL
+    sd = D.random_state_dict(D.vae_decoder_param_shapes(cfg), seed=51)
+    eng = _lib.Engine(_lib.EmuConfig())
+    v = _lib.EmuVAEConfig()
+    v.latent_channels, v.out_channels, v.n_blocks = 4, 3, len(cfg["block_out_channels"])
+    for i, c in enumerate(cfg["block_out_channels"]):
+        v.block_out_channels[i] = c
+    v.layers_per_block, v.norm_groups = cfg["layers_per_block"], cfg["norm_num_groups"]
+    eng.vae_configure(v)
+    eng.load_state_dict({"vae." + k: t for k, t in sd.items()})
+    z = torch.randn(1, 4, 128, 128, generator=torch.Generator().manual_seed(52)).to(torch.bfloat16)
+    post = lambda x: (x.float() / 2 + 0.5).clamp(0, 1).permute(0, 2, 3, 1).cpu()
+    tf32 = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
+    try:
+        torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+        with torch.no_grad():
+            ref32 = post(D.vae_decode({k: t.cuda() for k, t in sd.items()}, cfg, z.float().cuda()))
+    finally:
+        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = tf32
+    with torch.no_grad():
+        ref16 = post(D.vae_decode({k: t.to(torch.bfloat16).cuda() for k, t in sd.items()}, cfg, z.cuda()))
+    torch.cuda.empty_cache()
+    out = eng.vae_decode(z.cuda()).cpu()
+    assert out.shape == ref32.shape == (1, 1024, 1024, 3)
+    report("vae decoder 128^2 latents", out, ref32, ref16)
+    eng.close()
