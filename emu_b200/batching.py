@@ -7,9 +7,9 @@ its own length.  One `step()` is one iteration:
      pictures go through the ViT, their prompts are embedded and spliced, and ONE emu_llm_join prefills all of them
      (left-padded to the longest) while the live slots keep their cache.  A beam request joins into its first slot and is
      forked to the others.  The join stalls the live requests for one ViT + prefill;
-  2. select: every live request picks its next tokens from ITS OWN rows of the logits with ITS OWN knobs, through the same
-     kernels generation.py uses on a batch of one (beam_topk / sample_tokens / beam_step on the request's contiguous slice),
-     so a request's tokens are the ones it would get alone;
+  2. select: every live request picks its next tokens from ITS OWN rows of the logits with ITS OWN knobs, through the
+     selector generation.generate runs for those knobs (generation.selector, one prompt: num_beams rows), so a request's
+     tokens are the ones it would get alone;
   3. retire: finished requests leave (their slots are freed) and are answered;
   4. decode: ONE emu_llm_decode over B = highest occupied slot + 1 advances every live request by one token (free slots
      below B are computed and ignored).
@@ -50,42 +50,94 @@ class SlotRequest:
                                else torch.as_tensor(attention_mask).view(1, -1))
         self.image, self.video = image, video
         self.image_token_id, self.video_token_id = image_token_id, video_token_id
-        self.num_beams = int(num_beams or 1)
-        self.max_new_tokens, self.min_len = int(max_new_tokens), int(min_len or 0)
-        self.do_sample = bool(do_sample)
-        self.temperature, self.top_k, self.top_p = temperature, top_k, top_p
-        self.length_penalty, self.early_stopping = length_penalty, early_stopping
-        self.repetition_penalty = 1.0 if repetition_penalty is None else float(repetition_penalty)
-        self.ngram = int(no_repeat_ngram_size or 0)
-        self.generator = generator
+        self.num_beams, rp, ngram, n_ret = generation.decoding_knobs(num_beams, repetition_penalty, no_repeat_ngram_size,
+                                                                     num_return_sequences)
+        self.max_new_tokens = int(max_new_tokens)
+        self.knobs = dict(do_sample=bool(do_sample), min_length=int(min_len or 0), length_penalty=length_penalty,
+                          early_stopping=early_stopping, repetition_penalty=rp, no_repeat_ngram_size=ngram,
+                          temperature=temperature, top_k=top_k, top_p=top_p, generator=generator)
         self.eos, self.pad = eos_token_id, pad_token_id
         self.finish, self.on_done, self.tag = finish, on_done, tag
         self.done = threading.Event()
         self.result = self.error = None
-        if self.num_beams < 1:
-            raise ValueError("num_beams has to be an integer >= 1")
         if self.max_new_tokens < 1:
             raise ValueError("max_new_tokens has to be >= 1")
-        if self.num_beams == 1 and not self.do_sample and penalty_alpha is not None and penalty_alpha > 0 \
+        if self.num_beams == 1 and not do_sample and penalty_alpha is not None and penalty_alpha > 0 \
                 and top_k is not None and top_k > 1:
             raise ValueError("continuous batching does not run contrastive search (penalty_alpha with top_k > 1)")
         if prefix_allowed_tokens_fn is not None:
             raise ValueError("continuous batching does not take prefix_allowed_tokens_fn")
-        if int(num_return_sequences or 1) != 1:
+        if n_ret != 1:
             raise ValueError("continuous batching returns one sequence per request (num_return_sequences = 1)")
         # set at admission
         self.slots = []
         self.engine_slots = []      # the slots the engine holds for this request (joined / forked): they must leave
         self.step = 0
         self.logits = None
+        self.selector = None        # generation's token selector for this request
 
 
-class SlotScheduler:
+class _RequestQueue:
+    """The request life cycle both slot schedulers share.  `submit` (from any thread) queues a request; the subclass's
+    `step` (from one thread) admits, advances and retires.  A request is answered once: with `_result(r)` when it retires,
+    or with an error; either way it leaves its slots first (`_release`).  `_live()` lists the admitted requests."""
+
+    def __init__(self):
+        self.waiting = collections.deque()
+        self._lock = threading.Lock()
+
+    def submit(self, request):
+        with self._lock:
+            self.waiting.append(request)
+        return request
+
+    def busy(self):
+        return bool(self._live()) or bool(self.waiting)
+
+    def load(self):
+        """requests admitted or waiting"""
+        return len(self._live()) + len(self.waiting)
+
+    def abort(self, ex):
+        """fail every live and waiting request with `ex` (the scheduler itself stays usable)"""
+        for r in self._live():
+            self._fail(r, ex)
+        with self._lock:
+            waiting, self.waiting = list(self.waiting), collections.deque()
+        for r in waiting:
+            self._fail(r, ex)
+
+    def run_until_idle(self):
+        out = []
+        while self.busy():
+            out += self.step()
+        return out
+
+    def _retire(self, r):
+        try:
+            r.result = self._result(r)
+        except Exception as ex:
+            r.error = ex
+        self._answer(r)
+
+    def _fail(self, r, ex):
+        r.error = ex
+        self._answer(r)
+
+    def _answer(self, r):
+        self._release(r)
+        r.done.set()
+        if r.on_done is not None:
+            r.on_done(r)
+
+
+class SlotScheduler(_RequestQueue):
     """Continuous batching over `emu_model` (an EmuModel: its engine, tokenizer ids, ViT and projection) with `n_slots`
     KV-cache slots (at most the engine's llm_max_batch).  Owns the engine while it lives: nothing else may use the engine's
     LLM between steps.  Single-threaded: `submit` may be called from any thread, `step` from one."""
 
     def __init__(self, emu_model, n_slots=None):
+        super().__init__()
         self.model = emu_model
         self.engine = emu_model.engine
         cfg = self.engine.cfg
@@ -98,12 +150,10 @@ class SlotScheduler:
         tok = getattr(getattr(emu_model, "decoder", None), "tokenizer", None)
         self.eos = getattr(tok, "eos_token_id", None)
         self.pad = getattr(tok, "pad_token_id", None)
-        self.waiting = collections.deque()
         self.live = []                                      # admitted requests, in admission order
         self.owner = [None] * self.n_slots                  # slot -> request
         self.steps = 0
         self.batch_sizes = collections.deque(maxlen=1024)   # B of the recent decode steps (observability; the tests read it)
-        self._lock = threading.Lock()
         i32 = dict(dtype=torch.int32, device=self.device)
         self.tok_buf = torch.zeros(self.n_slots, **i32)      # fixed buffers: the decode graphs are keyed by their pointers
         self.ident = torch.arange(self.n_slots, **i32)
@@ -123,16 +173,10 @@ class SlotScheduler:
         n_prompt = request.input_ids.shape[1]
         if self.max_seq and n_prompt > self.max_seq:
             raise ValueError("prompt of %d tokens exceeds llm_max_seq = %d" % (n_prompt, self.max_seq))
-        with self._lock:
-            self.waiting.append(request)
-        return request
+        return super().submit(request)
 
-    def busy(self):
-        return bool(self.live) or bool(self.waiting)
-
-    def load(self):
-        """requests admitted or waiting"""
-        return len(self.live) + len(self.waiting)
+    def _live(self):
+        return list(self.live)
 
     # ---- one iteration ----
     @torch.no_grad()
@@ -150,21 +194,6 @@ class SlotScheduler:
             self._decode()
         self.steps += 1
         return finished
-
-    def abort(self, ex):
-        """fail every live and waiting request with `ex` (the scheduler itself stays usable)"""
-        for r in list(self.live):
-            self._fail(r, ex)
-        with self._lock:
-            waiting, self.waiting = list(self.waiting), collections.deque()
-        for r in waiting:
-            self._fail(r, ex)
-
-    def run_until_idle(self):
-        out = []
-        while self.busy():
-            out += self.step()
-        return out
 
     # ---- admission ----
     def _free_run(self, n):
@@ -253,28 +282,12 @@ class SlotScheduler:
                     self.engine.fork(r.slots[0], r.slots[1:])
                     r.engine_slots = list(r.slots)
                 r.logits = logits[i:i + 1].repeat(r.num_beams, 1).contiguous() if r.num_beams > 1 else logits[i:i + 1]
-                self._start(r)
+                r.selector = generation.selector(self.engine, 1, r.max_new_tokens, r.eos, r.pad, self.device,
+                                                 r.num_beams, **r.knobs)
             except Exception as ex:
                 self._fail(r, ex)
                 continue
             self.live.append(r)
-
-    def _start(self, r):
-        """per-request selection state, as the solo loop of its strategy sets it up (generation.py)"""
-        dev, nb = self.device, r.num_beams
-        r.processed = r.repetition_penalty != 1.0 or bool(r.ngram)
-        if nb > 1:
-            r.kind = "beam"
-            r.beams = self.engine.beam_state(1, nb, r.max_new_tokens, r.pad, dev)
-            r.zero_run = torch.zeros(1, nb, dtype=torch.float32, device=dev) if r.do_sample else None
-            return
-        r.kind = "sample" if r.do_sample else "greedy"
-        r.zero_run = torch.zeros(1, 1, dtype=torch.float32, device=dev)
-        r.prev = torch.full((1, r.max_new_tokens), r.pad, dtype=torch.int32, device=dev)
-        r.out = []
-        if r.do_sample:   # sample_search's per-call seed, drawn from the request's generator
-            g = r.generator
-            r.seed = int(torch.randint(0, 2 ** 62, (1,), generator=g, device="cpu" if g is None else g.device))
 
     # ---- selection ----
     def _select(self):
@@ -297,55 +310,17 @@ class SlotScheduler:
     def _select_one(self, r):
         """r's next tokens from r.logits ([num_beams, V]); writes them (and the beam re-parenting) into the decode inputs
         of r's slots and returns a device flag: r is finished"""
-        eng, step, first, nb = self.engine, r.step, r.slots[0], r.num_beams
-        ban = r.eos if step < r.min_len else -1
-        if r.kind == "beam":
-            st = r.beams
-            live = st.running_seq[st.live(step)]
-            need_prev = r.processed and step > 0
-            topk_lp, topk_i = eng.beam_topk(r.logits, r.zero_run if r.do_sample else st.running_scores, 1, nb, 2 * nb,
-                                            ban_id=ban, prev_tokens=live.view(nb, st.max_length) if need_prev else None,
-                                            prev_len=step, repetition_penalty=r.repetition_penalty, penalty_on_logits=False,
-                                            no_repeat_ngram=r.ngram)
-            if r.do_sample:
-                lp = generation._warp_log_probs(r.logits.view(nb, self.V), r.temperature, r.top_k, r.top_p, min_keep=2)
-                acc = (lp.view(1, nb, self.V) + st.running_scores.view(1, nb, 1)).view(1, nb * self.V)
-                pick = torch.multinomial(torch.softmax(acc, dim=-1), num_samples=2 * nb, generator=r.generator)
-                topk_lp, topk_i = torch.gather(acc, 1, pick).contiguous(), pick.to(torch.int32).contiguous()
-            eng.beam_step(st, topk_lp, topk_i, step, r.eos, r.length_penalty, r.early_stopping)
-            r.step = step + 1
-            self.tok_buf[first:first + nb] = st.next_tokens
-            self.src_buf[first:first + nb] = st.beam_src + first
-            return st.done
-        if r.kind == "greedy" and not r.processed:
-            lg = r.logits
-            if ban >= 0:
-                lg[:, ban] = float("-inf")
-            nxt = lg.argmax(-1).to(torch.int32)
-        else:
-            if r.processed:   # the processor kernels (one beam) leave the processed log-probabilities in r.logits
-                _, idx = eng.beam_topk(r.logits, r.zero_run, 1, 1, 2, ban_id=ban, prev_tokens=r.prev if step > 0 else None,
-                                       prev_len=step, repetition_penalty=r.repetition_penalty, penalty_on_logits=True,
-                                       no_repeat_ngram=r.ngram)
-            if r.kind == "greedy":
-                nxt = idx[:, 0].to(torch.int32)
-            else:
-                nxt = eng.sample_tokens(r.logits, r.temperature or 1.0, r.top_k or 0, 1.0 if r.top_p is None else r.top_p, ban,
-                                        r.seed, step).to(torch.int32)
-        r.prev[:, step] = nxt
-        r.out.append(nxt)
-        r.step = step + 1
-        self.tok_buf[first:first + 1] = nxt
-        return nxt == r.eos
+        first, nb = r.slots[0], r.num_beams
+        self.tok_buf[first:first + nb] = r.selector.select(r.logits, r.step)
+        if nb > 1:
+            self.src_buf[first:first + nb] = r.selector.beam_src + first
+        r.step += 1
+        return r.selector.done()
 
     # ---- retirement ----
-    def _output(self, r):
-        if r.kind == "beam":
-            return r.beams.result(r.step, 1).to(self.device)
-        toks = torch.stack(r.out, dim=1).to(torch.int64)
-        if r.kind == "greedy":
-            return generation._finish_rows(toks, r.eos, r.pad)
-        return toks
+    def _result(self, r):
+        ids = r.selector.output()
+        return r.finish(ids) if r.finish is not None else ids
 
     def _release(self, r):
         if r in self.live:
@@ -361,25 +336,6 @@ class SlotScheduler:
                 self.engine.leave(held)
             except Exception:
                 pass
-
-    def _answer(self, r):
-        r.done.set()
-        if r.on_done is not None:
-            r.on_done(r)
-
-    def _retire(self, r):
-        try:
-            ids = self._output(r)
-            r.result = r.finish(ids) if r.finish is not None else ids
-        except Exception as ex:
-            r.error = ex
-        self._release(r)
-        self._answer(r)
-
-    def _fail(self, r, ex):
-        r.error = ex
-        self._release(r)
-        self._answer(r)
 
     # ---- decode ----
     def _decode(self):
@@ -447,7 +403,7 @@ class ImageRequest:
         self.step = 0
 
 
-class DenoiseSlotScheduler:
+class DenoiseSlotScheduler(_RequestQueue):
     """Continuous batching of EmuVisualGeneration requests over `n_slots` latent slots (include/emu_b200_gen_slots.h): each
     slot holds one request at its own denoise step, with its own step count, guidance, time ids and latents.  One `step()`:
 
@@ -464,6 +420,7 @@ class DenoiseSlotScheduler:
     Owns the pipeline's engine while it lives.  Single-threaded: `submit` may be called from any thread, `step` from one."""
 
     def __init__(self, pipeline, n_slots=4, height=1024, width=1024, n_tokens=None):
+        super().__init__()
         self.pipe, self.engine = pipeline, pipeline.engine
         self.n_slots = int(n_slots)
         if not 1 <= self.n_slots <= 32:
@@ -488,11 +445,9 @@ class DenoiseSlotScheduler:
         self._stage_params = self._stage[:n * 16].view(torch.float32).view(n, 4)
         self._stage_live = self._stage[n * 16:].view(torch.int32)
         self._copied = None                                  # event: the last staging copy has run
-        self.waiting = collections.deque()
         self.owner = [None] * n
         self.steps = 0
         self.batch_sizes = collections.deque(maxlen=1024)   # B of the recent UNet steps (observability; the tests read it)
-        self._lock = threading.Lock()
         # every workspace at its largest size now: a later growth would drop every captured graph
         with _on_device(dev):
             self._unet_step(n)
@@ -504,31 +459,7 @@ class DenoiseSlotScheduler:
         if (request.height, request.width) != (self.height, self.width):
             raise ValueError("this scheduler generates %dx%d images; a %dx%d request needs a scheduler of its own size"
                              % (self.width, self.height, request.width, request.height))
-        with self._lock:
-            self.waiting.append(request)
-        return request
-
-    def busy(self):
-        return any(self.owner) or bool(self.waiting)
-
-    def load(self):
-        """requests admitted or waiting"""
-        return sum(r is not None for r in self.owner) + len(self.waiting)
-
-    def abort(self, ex):
-        """fail every live and waiting request with `ex` (the scheduler itself stays usable)"""
-        for r in self._live():
-            self._fail(r, ex)
-        with self._lock:
-            waiting, self.waiting = list(self.waiting), collections.deque()
-        for r in waiting:
-            self._fail(r, ex)
-
-    def run_until_idle(self):
-        out = []
-        while self.busy():
-            out += self.step()
-        return out
+        return super().submit(request)
 
     def _live(self):
         return [r for r in self.owner if r is not None]
@@ -606,32 +537,16 @@ class DenoiseSlotScheduler:
         self.engine.denoise_step_slots(self.latents, self.params, self.live, self.ctx, self.text_embeds, self.time_ids, B)
 
     # ---- retirement ----
-    def _retire(self, r):
-        try:
-            lat = self.latents[r.slot:r.slot + 1].clone()
-            if r.output_type == "latent":
-                r.result = lat
-            else:
-                from PIL import Image
-                from .emu2.diffusion import EmuVisualGenerationPipelineOutput
-                u8, flags = self.pipe.decode_and_check(lat)
-                r.result = EmuVisualGenerationPipelineOutput(image=Image.fromarray(u8[0]),
-                                                             nsfw_content_detected=None if flags is None else flags[0])
-        except Exception as ex:
-            r.error = ex
-        self._release(r)
-        self._answer(r)
+    def _result(self, r):
+        lat = self.latents[r.slot:r.slot + 1].clone()
+        if r.output_type == "latent":
+            return lat
+        from PIL import Image
+        from .emu2.diffusion import EmuVisualGenerationPipelineOutput
+        u8, flags = self.pipe.decode_and_check(lat)
+        return EmuVisualGenerationPipelineOutput(image=Image.fromarray(u8[0]),
+                                                 nsfw_content_detected=None if flags is None else flags[0])
 
     def _release(self, r):
         if r.slot is not None and self.owner[r.slot] is r:
             self.owner[r.slot] = None
-
-    def _answer(self, r):
-        r.done.set()
-        if r.on_done is not None:
-            r.on_done(r)
-
-    def _fail(self, r, ex):
-        r.error = ex
-        self._release(r)
-        self._answer(r)

@@ -18,8 +18,21 @@ Strategies (the combinations `lm.generate` picks from do_sample / num_beams / pe
   contrastive_search   penalty_alpha>0, top_k>1, 1 beam    Emu2/emu/emu.py:166,222 / Emu1 modeling_emu.py:110 forward the knob
 `num_return_sequences` (Emu1 `num_captions`, modeling_emu.py:113,177) is honoured by beam search (n best hypotheses per prompt) and
 sampling (n independent draws per prompt, one prefill).
+
+How greedy (with processors), sampling and beam search pick their tokens lives in one selector per strategy, which holds
+the per-call state (`selector` maps the knobs to one).  `select(logits, step)`, `done()` and `output()` drive the solo
+loops here and the continuous-batching scheduler (batching.py), which runs one selector per request on its own rows.
 """
 import torch
+
+
+def decoding_knobs(num_beams, repetition_penalty, no_repeat_ngram_size, num_return_sequences):
+    """the knobs callers may pass as None, normalised as `generate` takes them:
+    (num_beams, repetition_penalty, no_repeat_ngram_size, num_return_sequences)"""
+    if num_beams is None or num_beams < 1:
+        raise ValueError("num_beams has to be an integer >= 1")
+    return (int(num_beams), 1.0 if repetition_penalty is None else float(repetition_penalty), int(no_repeat_ngram_size or 0),
+            max(1, int(num_return_sequences or 1)))
 
 
 def _allowed_mask(prefix_allowed_tokens_fn, seqs, V, device):
@@ -46,18 +59,232 @@ def _finish_rows(toks, eos_token_id, pad_token_id):
     return toks
 
 
+def _prefill(engine, inputs_embeds, attention_mask, n):
+    """the prompts' last logits, each prompt's cache row mapped to n rows.  HF expands the inputs n times and prefills every
+    copy; here each prompt is prefilled ONCE (same cache contents, 1 / n of the work)."""
+    engine.llm_reset()
+    _, logits = engine.llm_prefill(inputs_embeds, attention_mask, hf_positions=True, want_logits=True)
+    if n > 1:
+        B = inputs_embeds.shape[0] * n
+        engine.llm_expand(torch.arange(B, device=inputs_embeds.device, dtype=torch.int32) // n, B)
+        logits = logits.repeat_interleave(n, dim=0).contiguous()
+    return logits
+
+
+def _decode_loop(engine, sel, logits, max_new_tokens, check_every):
+    """select -> poll the finish flag every `check_every` steps -> decode, for at most max_new_tokens steps.  The tensors
+    handed to the decode step keep their addresses for the whole call (CUDA graphs / plans are keyed by their pointers)."""
+    logits_buf = torch.empty_like(logits)
+    for step in range(max_new_tokens):
+        ids = sel.select(logits, step)
+        if step + 1 == max_new_tokens or (check_every and (step + 1) % check_every == 0 and bool(sel.done())):
+            break
+        engine.llm_decode(token_ids=ids, beam_src=sel.beam_src, logits=logits_buf, B=logits.shape[0])
+        logits = logits_buf
+    return sel.output()
+
+
+class _Selector:
+    """What the strategies share: HF's logits processors (`_topk`) and `n`, the steps selected so far."""
+
+    beam_src = None
+
+    def __init__(self, engine, eos_token_id, device, min_length, repetition_penalty, no_repeat_ngram_size,
+                 prefix_allowed_tokens_fn):
+        self.engine, self.eos, self.device, self.min_length = engine, eos_token_id, device, min_length
+        self.repetition_penalty, self.ngram, self.prefix_fn = repetition_penalty, no_repeat_ngram_size, prefix_allowed_tokens_fn
+        self.n = 0
+
+    def _topk(self, logits, running_scores, beams, step, prev, seqs, penalty_on_logits):
+        """emu_beam_topk with the processors (`prev`: the rows' tokens for the penalty and n-gram ban, or None; `seqs`
+        [prompts, beams, >= step]: the same for the prefix callback); leaves the processed log-probabilities in `logits`"""
+        allowed = None
+        if self.prefix_fn is not None:
+            allowed = _allowed_mask(self.prefix_fn, seqs[:, :, :step].to("cpu", torch.int64), self.engine.cfg.llm_vocab,
+                                    self.device)
+        return self.engine.beam_topk(logits, running_scores, logits.shape[0] // beams, beams, 2 * beams,
+                                     ban_id=self.eos if step < self.min_length else -1, prev_tokens=prev, prev_len=step,
+                                     repetition_penalty=self.repetition_penalty, penalty_on_logits=penalty_on_logits,
+                                     no_repeat_ngram=self.ngram, allowed=allowed)
+
+
+class GreedySelector(_Selector):
+    """Greedy search over `rows` rows with HF's logits processors, in `_sample`'s order: RepetitionPenalty on the RAW logits
+    -> NoRepeatNGram -> MinLength -> PrefixConstrained -> argmax; a finished row emits pad.  The processors and the selection
+    are the device kernels of emu_beam_topk run with one beam (log_softmax is monotone per row, so its top-1 is the processed
+    logits' argmax); `input_ids` for the processors is what HF sees when generation is driven by inputs_embeds: the tokens
+    generated so far, pads included.  Without processors the arg-max is taken from the logits with EOS banned below
+    min_length (what greedy_search's in-graph arg-max does)."""
+
+    def __init__(self, engine, rows, max_new_tokens, eos_token_id, pad_token_id, device, min_length=0, repetition_penalty=1.0,
+                 no_repeat_ngram_size=0, prefix_allowed_tokens_fn=None):
+        super().__init__(engine, eos_token_id, device, min_length, repetition_penalty, no_repeat_ngram_size,
+                         prefix_allowed_tokens_fn)
+        self.pad = pad_token_id
+        self.processed = repetition_penalty != 1.0 or bool(no_repeat_ngram_size) or prefix_allowed_tokens_fn is not None
+        i32 = dict(dtype=torch.int32, device=device)
+        self.prev = torch.full((rows, max_new_tokens), pad_token_id, **i32)     # the tokens so far: processor input, output
+        self.tokens = torch.empty(rows, **i32)                                  # the decode step's token_ids (fixed address)
+        self.pad_t = torch.full((rows,), pad_token_id, **i32)
+        self.finished = torch.zeros(rows, dtype=torch.bool, device=device)
+        self.zero_run = torch.zeros(rows, 1, dtype=torch.float32, device=device)
+
+    def _process(self, logits, step):
+        return self._topk(logits, self.zero_run, 1, step, self.prev if step > 0 else None, self.prev[:, None], True)[1]
+
+    def _pick(self, logits, step):
+        if self.processed:
+            return self._process(logits, step)[:, 0]                   # one beam: flat index == token id
+        if step < self.min_length:
+            logits[:, self.eos] = float("-inf")
+        return logits.argmax(-1).to(torch.int32)
+
+    def select(self, logits, step):
+        """the next token of every row from its logits [rows, V] (overwritten): int32 [rows], always the same buffer"""
+        nxt = torch.where(self.finished, self.pad_t, self._pick(logits, step), out=self.tokens)
+        self.prev[:, step] = nxt
+        self.finished |= nxt == self.eos
+        self.n = step + 1
+        return nxt
+
+    def done(self):
+        """device flag: every row has produced EOS"""
+        return self.finished.all()
+
+    def output(self):
+        return _finish_rows(self.prev[:, :self.n].to(torch.int64), self.eos, self.pad)
+
+
+class SampleSelector(GreedySelector):
+    """Multinomial sampling, HF `_sample` order: the logits processors as GreedySelector runs them (they leave the processed
+    log-probabilities in place; softmax(log_softmax(x) / T) == softmax(x / T), so the warpers see what HF's see) -> warpers
+    temperature -> top_k -> top_p -> one draw per row, all in emu_sample_tokens.  Returns every step's tokens, pads after
+    a row's EOS, untrimmed."""
+
+    def __init__(self, *args, temperature=None, top_k=None, top_p=None, generator=None, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.temperature, self.top_k, self.top_p = temperature or 1.0, top_k or 0, 1.0 if top_p is None else top_p
+        # one fresh seed per call, DRAWN from the generator so that its state advances like torch.multinomial's would:
+        # two do_sample calls with the same prompt differ, a re-seeded generator reproduces
+        g = generator
+        self.seed = int(torch.randint(0, 2 ** 62, (1,), generator=g, device="cpu" if g is None else g.device))
+
+    def _pick(self, logits, step):
+        if self.processed:
+            self._process(logits, step)
+        return self.engine.sample_tokens(logits, self.temperature, self.top_k, self.top_p,
+                                         self.eos if step < self.min_length else -1, self.seed, step)
+
+    def output(self):
+        return self.prev[:, :self.n].to(torch.int64)
+
+
+def _warp_log_probs(lp, temperature, top_k, top_p, min_keep):
+    """HF's sampling warpers on [rows, V] scores, in GenerationMixin's order (TemperatureLogitsWarper -> TopKLogitsWarper ->
+    TopPLogitsWarper); under beam search they keep at least `min_keep` = 2 tokens per row so a beam can always continue."""
+    if temperature is not None and temperature != 1.0:
+        lp = lp / temperature
+    if top_k:
+        k = min(max(int(top_k), min_keep), lp.shape[-1])
+        kth = torch.topk(lp, k)[0][..., -1, None]
+        lp = lp.masked_fill(lp < kth, float("-inf"))
+    if top_p is not None and top_p < 1.0:
+        s_sorted, s_idx = torch.sort(lp, descending=False)
+        remove = s_sorted.softmax(-1).cumsum(-1) <= (1 - top_p)
+        remove[..., -min_keep:] = False
+        lp = lp.masked_fill(remove.scatter(1, s_idx, remove), float("-inf"))
+    return lp
+
+
+class BeamSelector(_Selector):
+    """HF (transformers >= 4.50 vectorised) beam search over `batch` prompts x `num_beams` rows, decoder_prompt_len = 0
+    because generation is driven by inputs_embeds.  A step never leaves the device: engine.beam_topk (emu_beam_topk:
+    log_softmax, logits processors, running score, top 2*beams over beams x vocab) -> engine.beam_step (emu_beam_step: running
+    / finished hypothesis bookkeeping, next tokens and KV-cache reorder indices `beam_src`).  Steps made after the search
+    has finished are no-ops on the beam state.  `prefix_allowed_tokens_fn(batch_id, ids)` is a host callback by construction
+    (Emu1/mm_eval/models/emu.py:97-109): when it is given, the running sequences are read back every step to build the
+    allowed-token mask.
+
+    do_sample=True is HF's beam-sample (`_get_top_k_continuations`): the processor kernels leave the processed
+    log-probabilities in place, the sampling warpers and "+ running beam score" follow, and the 2*beams candidates are DRAWN
+    without replacement (with `generator`, every step) from softmax over beams x vocab instead of taken by top-k; the
+    bookkeeping is the same device step.  (do_sample with top_k < 2 * num_beams — the chat demo's defaults, top_k = 3 with
+    5 beams — leaves the first step fewer live candidates than the 2 * num_beams it draws: torch.multinomial then returns
+    zero-probability entries, whose accumulated score is -inf; those beams are dead from the start, exactly as in HF.)
+
+    The output is the best `num_return_sequences` finished hypotheses per prompt ([batch * n, T], best first), padded."""
+
+    def __init__(self, engine, batch, num_beams, max_new_tokens, eos_token_id, pad_token_id, device, min_length=0,
+                 length_penalty=1.0, early_stopping=False, repetition_penalty=1.0, no_repeat_ngram_size=0,
+                 prefix_allowed_tokens_fn=None, penalty_on_logits=False, num_return_sequences=1, do_sample=False,
+                 temperature=None, top_k=None, top_p=None, generator=None):
+        super().__init__(engine, eos_token_id, device, min_length, repetition_penalty, no_repeat_ngram_size,
+                         prefix_allowed_tokens_fn)
+        self.length_penalty, self.early_stopping, self.penalty_on_logits = length_penalty, early_stopping, penalty_on_logits
+        self.n_ret, self.do_sample, self.generator = num_return_sequences, do_sample, generator
+        self.temperature, self.top_k, self.top_p = temperature, top_k, top_p
+        self.st = engine.beam_state(batch, num_beams, max_new_tokens, pad_token_id, device)
+        self.need_prev = repetition_penalty != 1.0 or bool(no_repeat_ngram_size)
+        self.zero_run = torch.zeros(batch, num_beams, dtype=torch.float32, device=device) if do_sample else None
+
+    @property
+    def beam_src(self):
+        return self.st.beam_src
+
+    def select(self, logits, step):
+        """one beam-search step from the logits [batch * beams, V] (overwritten): the next tokens int32 [batch * beams]
+        (`st.next_tokens`) and their cache rows `beam_src`"""
+        st = self.st
+        Bt, nb, V = st.batch, st.beams, logits.shape[-1]
+        live = st.running_seq[st.live(step)]                       # [Bt, nb, max_length] tokens generated so far
+        topk_lp, topk_i = self._topk(logits, self.zero_run if self.do_sample else st.running_scores, nb, step,
+                                     live.view(Bt * nb, st.max_length) if self.need_prev and step > 0 else None, live,
+                                     self.penalty_on_logits)
+        if self.do_sample:
+            lp = _warp_log_probs(logits.view(Bt * nb, V), self.temperature, self.top_k, self.top_p, min_keep=2)
+            acc = (lp.view(Bt, nb, V) + st.running_scores.view(Bt, nb, 1)).view(Bt, nb * V)
+            pick = torch.multinomial(torch.softmax(acc, dim=-1), num_samples=2 * nb, generator=self.generator)
+            topk_lp, topk_i = torch.gather(acc, 1, pick).contiguous(), pick.to(torch.int32).contiguous()
+        self.engine.beam_step(st, topk_lp, topk_i, step, self.eos, self.length_penalty, self.early_stopping)
+        self.n = step + 1
+        return st.next_tokens
+
+    def done(self):
+        """device flag: the search has finished"""
+        return self.st.done
+
+    def output(self):
+        return self.st.result(self.n, self.n_ret).to(self.device)
+
+
+def selector(engine, batch, max_new_tokens, eos_token_id, pad_token_id, device, num_beams=1, do_sample=False, min_length=0,
+             length_penalty=1.0, early_stopping=False, repetition_penalty=1.0, no_repeat_ngram_size=0, temperature=None,
+             top_k=None, top_p=None, generator=None):
+    """the selector `generate` runs for these knobs (as `decoding_knobs` leaves them) on `batch` prompts, one sequence each:
+    beam search / beam-sample, sampling or greedy search (contrastive search has no selector)"""
+    common = dict(min_length=min_length, repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size)
+    if num_beams > 1:
+        return BeamSelector(engine, batch, num_beams, max_new_tokens, eos_token_id, pad_token_id, device,
+                            length_penalty=length_penalty, early_stopping=early_stopping, do_sample=do_sample,
+                            temperature=temperature, top_k=top_k, top_p=top_p, generator=generator, **common)
+    if do_sample:
+        return SampleSelector(engine, batch, max_new_tokens, eos_token_id, pad_token_id, device, temperature=temperature,
+                              top_k=top_k, top_p=top_p, generator=generator, **common)
+    return GreedySelector(engine, batch, max_new_tokens, eos_token_id, pad_token_id, device, **common)
+
+
 @torch.no_grad()
 def greedy_search(engine, inputs_embeds, attention_mask, max_new_tokens, eos_token_id, pad_token_id, min_length=0,
                   check_every=16, repetition_penalty=1.0, no_repeat_ngram_size=0, prefix_allowed_tokens_fn=None):
     """HF greedy: argmax; finished rows emit pad; stop when every row has produced EOS.  With a repetition penalty, an n-gram
-    ban or a prefix constraint the per-step argmax goes through the processor kernels (`_greedy_processed`)."""
-    if repetition_penalty != 1.0 or no_repeat_ngram_size or prefix_allowed_tokens_fn is not None:
-        return _greedy_processed(engine, inputs_embeds, attention_mask, max_new_tokens, eos_token_id, pad_token_id, min_length,
-                                 check_every, repetition_penalty, no_repeat_ngram_size or 0, prefix_allowed_tokens_fn)
+    ban or a prefix constraint the per-step argmax goes through the processor kernels (`GreedySelector`)."""
     B = inputs_embeds.shape[0]
     dev = inputs_embeds.device
-    engine.llm_reset()
-    _, logits = engine.llm_prefill(inputs_embeds, attention_mask, hf_positions=True, want_logits=True)
+    logits = _prefill(engine, inputs_embeds, attention_mask, 1)
+    if repetition_penalty != 1.0 or no_repeat_ngram_size or prefix_allowed_tokens_fn is not None:
+        sel = GreedySelector(engine, B, max_new_tokens, eos_token_id, pad_token_id, dev, min_length, repetition_penalty,
+                             no_repeat_ngram_size or 0, prefix_allowed_tokens_fn)
+        return _decode_loop(engine, sel, logits, max_new_tokens, check_every)
     if min_length > 0:
         logits[:, eos_token_id] = float("-inf")
     out = torch.empty(max_new_tokens, B, dtype=torch.int32, device=dev)
@@ -79,118 +306,22 @@ def greedy_search(engine, inputs_embeds, attention_mask, max_new_tokens, eos_tok
     return _finish_rows(out[:n_done].t().to(torch.int64), eos_token_id, pad_token_id)
 
 
-def _greedy_processed(engine, inputs_embeds, attention_mask, max_new_tokens, eos_token_id, pad_token_id, min_length,
-                      check_every, repetition_penalty, no_repeat_ngram_size, prefix_allowed_tokens_fn):
-    """Greedy search with HF's logits processors, in `_sample`'s order: RepetitionPenalty on the RAW logits -> NoRepeatNGram ->
-    MinLength -> PrefixConstrained -> argmax.  The processors and the selection are the device kernels of emu_beam_topk run
-    with one beam (log_softmax is monotone per row, so its top-1 is the processed logits' argmax); `input_ids` for the
-    processors is what HF sees when generation is driven by inputs_embeds: the tokens generated so far, pads included."""
-    B = inputs_embeds.shape[0]
-    dev = inputs_embeds.device
-    V = engine.cfg.llm_vocab
-    engine.llm_reset()
-    _, logits = engine.llm_prefill(inputs_embeds, attention_mask, hf_positions=True, want_logits=True)
-    logits_buf = torch.empty_like(logits)
-    prev = torch.full((B, max_new_tokens), pad_token_id, dtype=torch.int32, device=dev)
-    zero_run = torch.zeros(B, 1, dtype=torch.float32, device=dev)
-    finished = torch.zeros(B, dtype=torch.bool, device=dev)
-    tok = torch.empty(B, dtype=torch.int32, device=dev)
-    pad_t = torch.full((B,), pad_token_id, dtype=torch.int32, device=dev)
-    n_done = 0
-    for step in range(max_new_tokens):
-        allowed = None
-        if prefix_allowed_tokens_fn is not None:
-            allowed = _allowed_mask(prefix_allowed_tokens_fn, prev[:, None, :step].to("cpu", torch.int64), V, dev)
-        _, idx = engine.beam_topk(logits, zero_run, B, 1, 2, ban_id=eos_token_id if step < min_length else -1,
-                                  prev_tokens=prev if step > 0 else None, prev_len=step,
-                                  repetition_penalty=repetition_penalty, penalty_on_logits=True,
-                                  no_repeat_ngram=no_repeat_ngram_size, allowed=allowed)
-        nxt = torch.where(finished, pad_t, idx[:, 0].to(torch.int32))      # one beam: flat index == token id
-        prev[:, step] = nxt
-        finished |= nxt == eos_token_id
-        n_done = step + 1
-        if n_done == max_new_tokens:
-            break
-        if check_every and n_done % check_every == 0 and bool(finished.all()):
-            break
-        tok.copy_(nxt)
-        engine.llm_decode(token_ids=tok, logits=logits_buf, B=B)
-        logits = logits_buf
-    return _finish_rows(prev[:, :n_done].to(torch.int64), eos_token_id, pad_token_id)
-
-
 @torch.no_grad()
 def sample_search(engine, inputs_embeds, attention_mask, max_new_tokens, eos_token_id, pad_token_id, min_length=0,
                   temperature=None, top_k=None, top_p=None, generator=None, repetition_penalty=1.0, no_repeat_ngram_size=0,
                   prefix_allowed_tokens_fn=None, num_return_sequences=1):
-    """Multinomial sampling, HF `_sample` order: logits processors (repetition penalty on the raw logits, n-gram ban, min
-    length, prefix constraint) -> warpers temperature -> top_k -> top_p -> one draw per row.  num_return_sequences = n draws
-    n independent continuations per prompt (HF expands the inputs n times; here each prompt is prefilled once and its cache
-    row mapped to n rows); returns [B * n, T]."""
-    B0 = inputs_embeds.shape[0]
+    """Multinomial sampling (`SampleSelector`).  num_return_sequences = n draws n independent continuations per prompt (HF
+    expands the inputs n times; here each prompt is prefilled once and its cache row mapped to n rows); returns [B * n, T].
+    The host reads the finish flag every step, so T is the step at which the last row produced EOS."""
     n = max(1, int(num_return_sequences or 1))
-    B = B0 * n
-    dev = inputs_embeds.device
-    V = engine.cfg.llm_vocab
+    B = inputs_embeds.shape[0] * n
     if B > engine.cfg.llm_max_batch:
         raise ValueError("batch x num_return_sequences = %d exceeds the engine's llm_max_batch = %d" % (B, engine.cfg.llm_max_batch))
-    engine.llm_reset()
-    _, logits = engine.llm_prefill(inputs_embeds, attention_mask, hf_positions=True, want_logits=True)
-    if n > 1:
-        engine.llm_expand(torch.arange(B, device=dev, dtype=torch.int32) // n, B)
-        logits = logits.repeat_interleave(n, dim=0).contiguous()
-    processed = repetition_penalty != 1.0 or bool(no_repeat_ngram_size) or prefix_allowed_tokens_fn is not None
-    out = []
-    finished = torch.zeros(B, dtype=torch.bool, device=dev)
-    nxt32 = torch.empty(B, dtype=torch.int32, device=dev)
-    logits_buf = torch.empty_like(logits)
-    prev = torch.full((B, max_new_tokens), pad_token_id, dtype=torch.int32, device=dev) if processed else None
-    zero_run = torch.zeros(B, 1, dtype=torch.float32, device=dev)
-    # one fresh seed per call, DRAWN from the generator so that its state advances like torch.multinomial's would:
-    # two do_sample calls with the same prompt differ, a re-seeded generator reproduces
-    seed = int(torch.randint(0, 2 ** 62, (1,), generator=generator, device="cpu" if generator is None else generator.device))
-    for step in range(max_new_tokens):
-        ban = eos_token_id if step < min_length else -1
-        if processed:
-            # the processor kernels of emu_beam_topk (one beam per row) leave the processed log-probabilities in `logits`;
-            # softmax(log_softmax(x) / T) == softmax(x / T), so the warpers + draw below see what HF's see
-            allowed = None
-            if prefix_allowed_tokens_fn is not None:
-                allowed = _allowed_mask(prefix_allowed_tokens_fn, prev[:, None, :step].to("cpu", torch.int64), V, dev)
-            engine.beam_topk(logits, zero_run, B, 1, 2, ban_id=ban, prev_tokens=prev if step > 0 else None, prev_len=step,
-                             repetition_penalty=repetition_penalty, penalty_on_logits=True,
-                             no_repeat_ngram=no_repeat_ngram_size or 0, allowed=allowed)
-        # device-side step (emu_sample_tokens): warpers + multinomial draw in the library
-        nxt = engine.sample_tokens(logits, temperature or 1.0, top_k or 0, 1.0 if top_p is None else top_p, ban, seed,
-                                   step).long()
-        nxt = torch.where(finished, torch.full_like(nxt, pad_token_id), nxt)
-        out.append(nxt)
-        if processed:
-            prev[:, step] = nxt.to(torch.int32)
-        finished |= nxt == eos_token_id
-        if bool(finished.all()) or step == max_new_tokens - 1:
-            break
-        nxt32.copy_(nxt)
-        engine.llm_decode(token_ids=nxt32, logits=logits_buf, B=B)
-        logits = logits_buf
-    return torch.stack(out, dim=1)
-
-
-def _warp_log_probs(lp, temperature, top_k, top_p, min_keep):
-    """HF's sampling warpers on [rows, V] scores, in GenerationMixin's order (TemperatureLogitsWarper -> TopKLogitsWarper ->
-    TopPLogitsWarper); under beam search they keep at least `min_keep` = 2 tokens per row so a beam can always continue."""
-    if temperature is not None and temperature != 1.0:
-        lp = lp / temperature
-    if top_k:
-        k = min(max(int(top_k), min_keep), lp.shape[-1])
-        kth = torch.topk(lp, k)[0][..., -1, None]
-        lp = lp.masked_fill(lp < kth, float("-inf"))
-    if top_p is not None and top_p < 1.0:
-        s_sorted, s_idx = torch.sort(lp, descending=False)
-        remove = s_sorted.softmax(-1).cumsum(-1) <= (1 - top_p)
-        remove[..., -min_keep:] = False
-        lp = lp.masked_fill(remove.scatter(1, s_idx, remove), float("-inf"))
-    return lp
+    logits = _prefill(engine, inputs_embeds, attention_mask, n)
+    sel = SampleSelector(engine, B, max_new_tokens, eos_token_id, pad_token_id, inputs_embeds.device, min_length,
+                         repetition_penalty, no_repeat_ngram_size or 0, prefix_allowed_tokens_fn, temperature=temperature,
+                         top_k=top_k, top_p=top_p, generator=generator)
+    return _decode_loop(engine, sel, logits, max_new_tokens, check_every=1)
 
 
 @torch.no_grad()
@@ -198,72 +329,23 @@ def beam_search(engine, inputs_embeds, attention_mask, num_beams, max_new_tokens
                 min_length=0, length_penalty=1.0, early_stopping=False, repetition_penalty=1.0, no_repeat_ngram_size=0,
                 prefix_allowed_tokens_fn=None, penalty_on_logits=False, check_every=8, num_return_sequences=1,
                 do_sample=False, temperature=None, top_k=None, top_p=None, generator=None):
-    """HF (transformers >= 4.50 vectorised) beam search, decoder_prompt_len = 0 because generation is driven by
-    inputs_embeds.  Returns the best `num_return_sequences` finished hypotheses per batch row ([B * n, T], best first), new
-    tokens only, padded.
-
-    A step never leaves the device: engine.beam_topk (emu_beam_topk: log_softmax, logits processors, running score, top
-    2*beams over beams x vocab) -> engine.beam_step (emu_beam_step: running / finished hypothesis bookkeeping, next tokens and
-    KV-cache reorder indices) -> the CUDA-graphed decode step, chained through device buffers.  The host reads the `done`
-    flag every `check_every` steps only (steps launched after the search has finished are no-ops on the beam state).
-    `prefix_allowed_tokens_fn(batch_id, ids)` is a host callback by construction (Emu1/mm_eval/models/emu.py:97-109): when
-    it is given, the running sequences are read back every step to build the allowed-token mask.
-
-    do_sample=True is HF's beam-sample (`_get_top_k_continuations`): the processor kernels leave the processed
-    log-probabilities in place, the sampling warpers and "+ running beam score" follow, and the 2*beams candidates are DRAWN
-    without replacement from softmax over beams x vocab instead of taken by top-k; the bookkeeping is the same device step.
+    """HF beam search / beam-sample (`BeamSelector`).  Returns the best `num_return_sequences` finished hypotheses per batch
+    row ([B * n, T], best first), new tokens only, padded.  The step chains through device buffers into the CUDA-graphed
+    decode step; the host reads the `done` flag every `check_every` steps only.
 
     With num_beams=1, early_stopping=True and penalty_on_logits=True this is HF greedy search with logits processors."""
     Bt = inputs_embeds.shape[0]
-    dev = inputs_embeds.device
     nb = num_beams
     n_ret = max(1, int(num_return_sequences or 1))
     if n_ret > nb:
         raise ValueError("num_return_sequences = %d has to be <= num_beams = %d" % (n_ret, nb))
     if Bt * nb > engine.cfg.llm_max_batch:
         raise ValueError("batch x num_beams = %d exceeds the engine's llm_max_batch = %d" % (Bt * nb, engine.cfg.llm_max_batch))
-    V = engine.cfg.llm_vocab
-    keep = 2 * nb
-    # (do_sample with top_k < 2 * num_beams — the chat demo's defaults, top_k = 3 with 5 beams — leaves the first step fewer
-    # live candidates than the 2 * num_beams it draws: torch.multinomial then returns zero-probability entries, whose
-    # accumulated score is -inf; those beams are dead from the start, exactly as in HF)
-    max_length = max_new_tokens
-    # HF expands the inputs to batch x beams and prefills num_beams identical copies of every prompt; here each prompt is
-    # prefilled ONCE and its cache row is then mapped to num_beams rows (same cache contents, 1 / num_beams of the work)
-    engine.llm_reset()
-    _, logits = engine.llm_prefill(inputs_embeds, attention_mask, hf_positions=True, want_logits=True)
-    if nb > 1:
-        engine.llm_expand(torch.arange(Bt * nb, device=dev, dtype=torch.int32) // nb, Bt * nb)
-        logits = logits.repeat_interleave(nb, dim=0).contiguous()
-    logits_buf = torch.empty_like(logits)
-    st = engine.beam_state(Bt, nb, max_length, pad_token_id, dev)
-    need_prev = repetition_penalty != 1.0 or bool(no_repeat_ngram_size)
-    zero_run = torch.zeros(Bt, nb, dtype=torch.float32, device=dev) if do_sample else None
-    cur_len = 0
-    while True:
-        live = st.running_seq[st.live(cur_len)]                       # [Bt, nb, max_length] tokens generated so far
-        allowed = None
-        if prefix_allowed_tokens_fn is not None:
-            allowed = _allowed_mask(prefix_allowed_tokens_fn, live[:, :, :cur_len].to("cpu", torch.int64), V, dev)
-        topk_lp, topk_i = engine.beam_topk(logits, zero_run if do_sample else st.running_scores, Bt, nb, keep,
-                                           ban_id=eos_token_id if cur_len < min_length else -1,
-                                           prev_tokens=live.view(Bt * nb, max_length) if need_prev and cur_len > 0 else None,
-                                           prev_len=cur_len, repetition_penalty=repetition_penalty,
-                                           penalty_on_logits=penalty_on_logits, no_repeat_ngram=no_repeat_ngram_size or 0,
-                                           allowed=allowed)
-        if do_sample:
-            lp = _warp_log_probs(logits.view(Bt * nb, V), temperature, top_k, top_p, min_keep=2)
-            acc = (lp.view(Bt, nb, V) + st.running_scores.view(Bt, nb, 1)).view(Bt, nb * V)
-            pick = torch.multinomial(torch.softmax(acc, dim=-1), num_samples=keep, generator=generator)
-            topk_lp, topk_i = torch.gather(acc, 1, pick).contiguous(), pick.to(torch.int32).contiguous()
-        engine.beam_step(st, topk_lp, topk_i, cur_len, eos_token_id, length_penalty, early_stopping)
-        cur_len += 1
-        if cur_len >= max_length or (check_every and cur_len % check_every == 0):
-            if st.is_done():
-                break
-        engine.llm_decode(token_ids=st.next_tokens, beam_src=st.beam_src, logits=logits_buf, B=Bt * nb)
-        logits = logits_buf
-    return st.result(cur_len, n_ret).to(dev)
+    logits = _prefill(engine, inputs_embeds, attention_mask, nb)
+    sel = BeamSelector(engine, Bt, nb, max_new_tokens, eos_token_id, pad_token_id, inputs_embeds.device, min_length,
+                       length_penalty, early_stopping, repetition_penalty, no_repeat_ngram_size or 0, prefix_allowed_tokens_fn,
+                       penalty_on_logits, n_ret, do_sample, temperature, top_k, top_p, generator)
+    return _decode_loop(engine, sel, logits, max_new_tokens, check_every)
 
 
 @torch.no_grad()
@@ -354,12 +436,8 @@ def generate(engine, inputs_embeds, attention_mask, max_new_tokens, eos_token_id
         num_beams  > 1                                                 -> beam search / beam-sample (do_sample)
 
     and returns the new token ids [B * num_return_sequences, T]."""
-    n_ret = max(1, int(num_return_sequences or 1))
-    ngram = int(no_repeat_ngram_size or 0)
-    rp = 1.0 if repetition_penalty is None else float(repetition_penalty)
+    num_beams, rp, ngram, n_ret = decoding_knobs(num_beams, repetition_penalty, no_repeat_ngram_size, num_return_sequences)
     ce = {} if check_every is None else {"check_every": check_every}
-    if num_beams is None or num_beams < 1:
-        raise ValueError("num_beams has to be an integer >= 1")
     if num_beams == 1 and not do_sample:
         if n_ret != 1:
             raise ValueError("num_return_sequences has to be 1 when doing greedy / contrastive search, got %d" % n_ret)

@@ -181,6 +181,9 @@ SPECS = [
     ("beamsample5_demo", 0, dict(num_beams=5, max_new_tokens=12, min_len=1, do_sample=True, top_k=3, top_p=0.9,
                                  temperature=0.7, length_penalty=1.0, seed=9)),
     ("greedy_short", 2, dict(num_beams=1, max_new_tokens=3)),
+    ("sample_rep_ngram", 1, dict(num_beams=1, max_new_tokens=10, do_sample=True, temperature=0.8, top_k=20,
+                                 repetition_penalty=1.3, no_repeat_ngram_size=2, seed=13)),
+    ("greedy_min_len", 3, dict(num_beams=1, max_new_tokens=9, min_len=6)),
 ]
 
 
