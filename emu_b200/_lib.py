@@ -80,6 +80,9 @@ SLOT_SYMBOLS = ["emu_llm_slots_begin", "emu_llm_join", "emu_llm_fork", "emu_llm_
 # ... and in include/emu_b200_ops.h (the decode-step kernels as stand-alone operators)
 OPS_SYMBOLS = ["emu_op_attn_decode_rows", "emu_op_rope_kv_write", "emu_op_kv_indir_update", "emu_op_kv_reorder",
                "emu_op_argmax_rows", "emu_op_attn_prefill_rows"]
+# ... and in include/emu_b200_prefix.h (prefix caching: kept slots, per-slot continuation and their kernels)
+PREFIX_SYMBOLS = ["emu_llm_leave_keep", "emu_llm_slot_kept", "emu_llm_copy_prefix", "emu_llm_extend", "emu_llm_kv_cache",
+                  "emu_op_rope_kv_write_rows", "emu_op_attn_prefill_offset", "emu_op_kv_prefix_copy"]
 # ... and in include/emu_b200_gen_slots.h (latent slots: continuous batching for image generation)
 GEN_SLOT_SYMBOLS = ["emu_denoise_step_slots", "emu_op_denoise_prepare", "emu_op_denoise_euler"]
 # ... and in include/emu_b200_diffusion_ops.h (the diffusion kernels as stand-alone operators)
@@ -276,6 +279,47 @@ class Engine:
 
     def slot_len(self, slot):
         return int(self.lib.emu_llm_slot_len(self.h, int(slot)))
+
+    # ---- prefix caching (include/emu_b200_prefix.h) ----
+    def kv_cache(self):
+        """the engine's KV cache as a bf16 tensor view [layers, 2 (K, V), rows, heads, llm_max_seq, head_dim] (no copy)"""
+        ptr, dims = C.c_void_p(), (C.c_int64 * 5)()
+        check(self.lib.emu_llm_kv_cache(self.h, C.byref(ptr), dims), self.h)
+        shape = tuple(int(d) for d in dims)
+
+        class _View:
+            __cuda_array_interface__ = dict(shape=shape, typestr="<i2", data=(ptr.value, False), version=3)
+        t = torch.as_tensor(_View(), device="cuda").view(torch.bfloat16)
+        return t.view(shape[0] // 2, 2, *shape[1:])
+
+    def leave_keep(self, slots, keep):
+        """free the given live slots, slot i keeping its first keep[i] cache positions (a beam group leaves together)"""
+        if len(keep) != len(slots):
+            raise ValueError("leave_keep: %d keep lengths for %d slots" % (len(keep), len(slots)))
+        hs, cnt = self._host_slots(slots)
+        hk, _ = self._host_slots(keep)
+        check(self.lib.emu_llm_leave_keep(self.h, hs, hk, cnt, _stream()), self.h)
+
+    def slot_kept(self, slot):
+        return int(self.lib.emu_llm_slot_kept(self.h, int(slot)))
+
+    def copy_prefix(self, src_slot, dst_slot, P):
+        """positions [0, P) of src_slot's own row (live or kept) -> the free dst_slot, which becomes kept with length P"""
+        check(self.lib.emu_llm_copy_prefix(self.h, int(src_slot), int(dst_slot), int(P), _stream()), self.h)
+
+    def extend(self, slots, prefix, new, embeds, want_logits=True):
+        """the free slots continue at length prefix[i] (<= their kept length) with new[i] tokens of embeds [n, N, hidden]
+        (right-padded); returns the logits of every row's last real token [n, vocab] fp32 (or None)"""
+        n, N, H = embeds.shape
+        if not n == len(slots) == len(prefix) == len(new):
+            raise ValueError("extend: %d rows for %d slots, %d prefixes, %d counts" % (n, len(slots), len(prefix), len(new)))
+        embeds = embeds.to(torch.bfloat16).contiguous()
+        logits = torch.empty(n, self.cfg.llm_vocab, dtype=torch.float32, device=embeds.device) if want_logits else None
+        hs, cnt = self._host_slots(slots)
+        hp, _ = self._host_slots(prefix)
+        hn, _ = self._host_slots(new)
+        check(self.lib.emu_llm_extend(self.h, hs, hp, hn, cnt, _ptr(embeds), N, _ptr(logits), _stream()), self.h)
+        return logits
 
     def sample_tokens(self, logits, temperature=1.0, top_k=0, top_p=1.0, ban_id=-1, seed=0, offset=0):
         return op_sample_tokens(logits, temperature, top_k, top_p, -1 if ban_id is None else ban_id, seed, offset)
@@ -715,6 +759,45 @@ def op_attn_prefill_rows(q, k, v, scale, causal=False, kv_start=None, kv_row=Non
                                           1 if causal else 0, _i32(kv_start, "kv_start"), _i32(kv_row, "kv_row"),
                                           k.shape[0] if kv_row is not None else 0, _stream()))
     return out
+
+
+# ---- prefix caching kernels (include/emu_b200_prefix.h) ----
+def op_rope_kv_write_rows(qkv, H, D, rope_cos, rope_sin, k_cache, v_cache, pos_off, q0, n_new, kv_row=None):
+    """qkv [B, N, 3*H*D] right-padded: batch b's first n_new[b] tokens rotated in place and their k / v written at cache slots
+    q0[b] + n of row kv_row[b]; caches [rows, H, T, D] written in place"""
+    require_cuda()
+    B, N, _ = qkv.shape
+    assert qkv.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
+    check(load().emu_op_rope_kv_write_rows(_ptr(qkv), B, N, H, D, _ptr(rope_cos), _ptr(rope_sin), _i32(pos_off, "pos_off"),
+                                           _i32(q0, "q0"), _i32(n_new, "n_new"), _i32(kv_row, "kv_row"), _ptr(k_cache),
+                                           _ptr(v_cache), k_cache.shape[2], _stream()))
+
+
+def op_attn_prefill_offset(q, k, v, scale, q_off, kv_start=None, kv_row=None, q_len=None):
+    """causal attention with a per-batch query offset: q [B,Nq,H,D], query i of batch b at key position q_off[b] + i; k/v
+    [rows,Nk,H,D] views read at batch kv_row[b] (None: b) -> [B,Nq,H,D]"""
+    require_cuda()
+    B, Nq, H, D = q.shape
+    Nk = k.shape[1]
+    out = torch.empty(B, Nq, H, D, dtype=torch.bfloat16, device=q.device)
+    st = []
+    for t in (q, k, v, out):
+        assert t.stride(3) == 1
+        st += [t.stride(0), t.stride(1), t.stride(2)]
+    st12 = (C.c_int64 * 12)(*st)
+    check(load().emu_op_attn_prefill_offset(_ptr(q), _ptr(k), _ptr(v), _ptr(out), B, H, Nq, Nk, D, st12, C.c_float(scale),
+                                            _i32(q_off, "q_off"), _i32(q_len, "q_len"), _i32(kv_start, "kv_start"),
+                                            _i32(kv_row, "kv_row"),
+                                            k.shape[0] if kv_row is not None else 0, _stream()))
+    return out
+
+
+def op_kv_prefix_copy(cache, src, dst, P):
+    """cache [outer, rows, H, T, D] bf16 in place: positions [0, P) of row src -> row dst"""
+    require_cuda()
+    outer, rows, H, T, D = cache.shape
+    assert cache.is_contiguous() and cache.dtype == torch.bfloat16
+    check(load().emu_op_kv_prefix_copy(_ptr(cache), outer, rows, H, D, T, int(src), int(dst), int(P), _stream()))
 
 
 # ---- the denoise-step glue (include/emu_b200_gen_slots.h) ----

@@ -14,6 +14,13 @@ its own length.  One `step()` is one iteration:
   4. decode: ONE emu_llm_decode over B = highest occupied slot + 1 advances every live request by one token (free slots
      below B are computed and ignored).
 
+Prefix caching (`SlotScheduler(prefix_cache=True)`, opt-in): a finished request leaves with emu_llm_leave_keep, so its slot keeps
+the KV of its prompt and answer (a beam search: its prompt).  A newcomer whose key sequence (token ids; a picture slot keyed by
+the picture's digest and its index within the picture) starts like a kept or live slot's resumes from it: in place when that
+kept slot can be its first slot, else through emu_llm_copy_prefix.  Only the suffix is embedded (pictures inside the prefix do
+not go through the ViT) and ONE emu_llm_extend prefills the suffixes of all resuming newcomers.  Kept slots count as free: a
+newcomer that needs room overwrites the least recently used one, so retention never delays admission.
+
 Each step reads ONE small tensor back to the host: the finish flag of every live request (EOS of a greedy / sampled request,
 `done` of a beam search), which is what lets a request leave as soon as it is finished.
 
@@ -41,7 +48,7 @@ class SlotRequest:
                  num_beams=5, max_new_tokens=10, min_len=1, do_sample=False, temperature=None, top_k=None, top_p=None,
                  length_penalty=-1, repetition_penalty=1.0, no_repeat_ngram_size=0, early_stopping=False, penalty_alpha=None,
                  num_return_sequences=1, prefix_allowed_tokens_fn=None, generator=None, eos_token_id=None,
-                 pad_token_id=None, finish=None, on_done=None, tag=None):
+                 pad_token_id=None, finish=None, on_done=None, tag=None, image_keys=None, signature=None):
         ids = torch.as_tensor(input_ids)
         self.input_ids = ids.view(1, -1) if ids.dim() == 1 else ids
         if self.input_ids.shape[0] != 1:
@@ -58,6 +65,10 @@ class SlotRequest:
                           temperature=temperature, top_k=top_k, top_p=top_p, generator=generator)
         self.eos, self.pad = eos_token_id, pad_token_id
         self.finish, self.on_done, self.tag = finish, on_done, tag
+        # prefix caching: one digest per picture of `image` (None: a picture never matches), and the front end's view of the
+        # prompt (its elements; pictures as digests) that the serving shell routes by
+        self.image_keys = None if image_keys is None else list(image_keys)
+        self.signature = signature
         self.done = threading.Event()
         self.result = self.error = None
         if self.max_new_tokens < 1:
@@ -75,6 +86,9 @@ class SlotRequest:
         self.step = 0
         self.logits = None
         self.selector = None        # generation's token selector for this request
+        self.keys = None            # prefix caching: the prompt's key sequence
+        self.left_pad = 0           # ... its left padding in its slot's row
+        self.resume = None          # ... (prefix keys, prefix cache positions, source slot, in place) when it resumes
 
 
 class _RequestQueue:
@@ -136,8 +150,15 @@ class SlotScheduler(_RequestQueue):
     KV-cache slots (at most the engine's llm_max_batch).  Owns the engine while it lives: nothing else may use the engine's
     LLM between steps.  Single-threaded: `submit` may be called from any thread, `step` from one."""
 
-    def __init__(self, emu_model, n_slots=None):
+    def __init__(self, emu_model, n_slots=None, prefix_cache=False):
         super().__init__()
+        self.prefix_cache = bool(prefix_cache)
+        self.kept = {}                                      # kept slot -> _Kept (prefix caching)
+        self._signatures = ()                               # front-end signatures of the kept and live slots (routing)
+        self._clock = 0
+        # prefix-caching observability (the tests read them): admissions that reused a prefix, the prompt tokens they did not
+        # prefill, the prompt tokens prefilled, the pictures encoded
+        self.prefix_hits = self.prefix_tokens_reused = self.prefill_tokens = self.vit_pictures = 0
         self.model = emu_model
         self.engine = emu_model.engine
         cfg = self.engine.cfg
@@ -193,6 +214,8 @@ class SlotScheduler(_RequestQueue):
         if self.live:
             self._decode()
         self.steps += 1
+        if self.prefix_cache:                               # one assignment: readers on other threads see old or new
+            self._signatures = tuple(e.signature for e in self.kept.values()) + tuple(r.signature for r in self.live)
         return finished
 
     # ---- admission ----
@@ -210,13 +233,14 @@ class SlotScheduler(_RequestQueue):
         with self._lock:
             while self.waiting:
                 r = self.waiting[0]
-                first = self._free_run(r.num_beams)
+                first = self._place(r) if self.prefix_cache else self._free_run(r.num_beams)
                 if first is None:
                     break                                   # first come, first served: the head waits for room
                 self.waiting.popleft()
                 r.slots = list(range(first, first + r.num_beams))
                 for s in r.slots:
                     self.owner[s] = r
+                    self.kept.pop(s, None)                  # whatever a kept slot held is overwritten or resumed now
                 batch.append(r)
         if not batch:
             return
@@ -226,6 +250,8 @@ class SlotScheduler(_RequestQueue):
                 ready.append((r, self._embed(r)))
             except Exception as ex:
                 self._fail(r, ex)
+        if self.prefix_cache:
+            ready = self._resume(ready)
         for group in self._join_groups(ready):
             try:
                 self._join(group)
@@ -260,8 +286,172 @@ class SlotScheduler(_RequestQueue):
 
     def _embed(self, r):
         m = self.model
-        ids = r.input_ids.to(self.device)
-        return m.embed_prompt(ids, r.image, r.video, r.image_token_id, r.video_token_id), r.attention_mask.to(self.device)
+        ids, image = r.input_ids, r.image
+        if r.resume is not None:                            # the suffix only: pictures inside the prefix skip the ViT
+            P = r.resume[0]
+            k0 = int((ids[0, :P] == r.image_token_id).sum()) // self._per_picture(r) if image is not None else 0
+            ids, image = ids[:, P:], (image[k0:] if image is not None and k0 < image.shape[0] else None)
+        self.vit_pictures += (0 if image is None else image.shape[0]) + (0 if r.video is None else r.video.shape[0])
+        self.prefill_tokens += int(r.attention_mask[0].sum()) - (r.resume[0] if r.resume is not None else 0)
+        ids = ids.to(self.device)
+        mask = torch.ones_like(ids) if r.resume is not None else r.attention_mask.to(self.device)
+        return m.embed_prompt(ids, image, r.video, r.image_token_id, r.video_token_id), mask
+
+    # ---- prefix caching ----
+    @staticmethod
+    def _per_picture(r):
+        n_img = int((r.input_ids == r.image_token_id).sum())
+        return max(1, n_img // r.image.shape[0]) if r.image is not None and r.image.shape[0] else max(1, n_img)
+
+    def _key_sequence(self, r):
+        """token ids, with every picture slot keyed by (picture digest, index within the picture); a picture without a digest
+        (and every video frame) gets a key equal to nothing else"""
+        ids = r.input_ids[0].tolist()
+        per = self._per_picture(r)
+        keys, k = [], 0
+        for t in ids:
+            if t == r.image_token_id:
+                pic, j = divmod(k, per)
+                ok = r.image_keys is not None and r.image is not None and pic < len(r.image_keys)
+                keys.append((r.image_keys[pic], j) if ok else object())
+                k += 1
+            elif t == r.video_token_id:
+                keys.append(object())
+            else:
+                keys.append(t)
+        return keys
+
+    def _sources(self):
+        """(slot, keys, pad, kept) of every kept slot and every live request's first slot (its prompt is its own row)"""
+        out = [(s, e.keys, e.left_pad, True) for s, e in self.kept.items()]
+        out += [(r.slots[0], r.keys, r.left_pad, False) for r in self.live if r.keys is not None]
+        return out
+
+    def _match(self, r):
+        """(prefix keys, source slot, its pad, kept) of the longest usable prefix of r's keys, or (0, None, 0, False)"""
+        keys, best = r.keys, (0, None, 0, False)
+        n = len(keys)
+        for s, ks, pad, kept in self._sources():
+            P = 0
+            for a, b in zip(keys, ks):
+                if a != b:
+                    break
+                P += 1
+            P = min(P, n - 1)                               # the last prompt token is recomputed for its logits
+            if P < n and isinstance(keys[P], tuple):        # never split a picture: cut back to its first slot
+                P -= keys[P][1]
+            if P <= best[0] or (self.max_seq and pad + n > self.max_seq) or self._cap(r, pad + n) != self._cap(r, n):
+                continue
+            best = (P, s, pad, kept)
+        return best
+
+    def _place(self, r):
+        """the first slot for r (prefix caching on), or None; sets r.keys and r.resume"""
+        nb = r.num_beams
+        r.keys = self._key_sequence(r) if bool((r.attention_mask != 0).all()) else None
+        r.resume = None
+        P, src, pad, kept = self._match(r) if r.keys is not None else (0, None, 0, False)
+        if P > 0 and kept and all(t < self.n_slots and self.owner[t] is None for t in range(src, src + nb)):
+            first, in_place = src, True
+        else:
+            first, in_place = self._pick_run(nb), False      # the copy runs before anything overwrites the source
+        if first is None:
+            return None
+        if P > 0:
+            r.resume, r.left_pad = (P, pad + P, src, in_place), pad
+            if src in self.kept:
+                self._clock += 1
+                self.kept[src].used = self._clock
+        return first
+
+    def _pick_run(self, n):
+        """first slot of n contiguous unowned slots, preferring runs that hold no kept prefix, then the least recently used"""
+        best = None
+        for first in range(self.n_slots - n + 1):
+            run = range(first, first + n)
+            if any(self.owner[t] is not None for t in run):
+                continue
+            cost = max([self.kept[t].used for t in run if t in self.kept], default=-1)
+            if best is None or cost < best[0]:
+                best = (cost, first)
+        return None if best is None else best[1]
+
+    def _resume(self, ready):
+        """copy the prefixes that cannot resume in place, then ONE emu_llm_extend for every resuming newcomer; returns the
+        items that join from nothing"""
+        joins, ext = [], []
+        for item in ready:
+            r = item[0]
+            if r.resume is None:
+                joins.append(item)
+                continue
+            P, Pc, src, in_place = r.resume
+            try:
+                if not in_place:
+                    self.engine.copy_prefix(src, r.slots[0], Pc)
+            except Exception as ex:
+                self._fail(r, ex)
+                continue
+            ext.append(item)
+        if ext:
+            try:
+                self._extend(ext)
+            except Exception as ex:
+                if len(ext) == 1:
+                    self._extend_failed(ext[0][0], ex)
+                else:
+                    for item in ext:                        # a shared extend failed: one by one, only the culprit fails
+                        try:
+                            self._extend([item])
+                        except Exception as ex1:
+                            self._extend_failed(item[0], ex1)
+        return joins
+
+    def _extend_failed(self, r, ex):
+        for s in r.slots:
+            self.kept.pop(s, None)
+        self._fail(r, ex)
+
+    def _extend(self, items):
+        N = max(e.shape[1] for _, (e, _) in items)
+        embeds = torch.zeros(len(items), N, items[0][1][0].shape[-1], dtype=items[0][1][0].dtype, device=self.device)
+        for i, (_, (e, _)) in enumerate(items):            # right padding: every row continues its own slot
+            embeds[i, :e.shape[1]] = e[0]
+        logits = self.engine.extend([r.slots[0] for r, _ in items], [r.resume[1] for r, _ in items],
+                                    [e.shape[1] for _, (e, _) in items], embeds)
+        for r, _ in items:
+            self.prefix_hits += 1
+            self.prefix_tokens_reused += r.resume[0]
+        self._start(items, logits, [r.left_pad + len(r.keys) for r, _ in items])
+
+    def _keep(self, r):
+        """what r's first slot keeps when it retires: the prompt and every answer token whose KV was written (beam search:
+        the prompt, its generated positions are scattered over the group's rows), or None"""
+        if r.keys is None:
+            return None
+        keys = list(r.keys)
+        if r.num_beams == 1 and r.step > 1:
+            keys += r.selector.prev[0, :r.step - 1].tolist()
+        if self.max_seq:
+            keys = keys[:self.max_seq - 1 - r.left_pad]
+        if not keys:
+            return None
+        self._clock += 1
+        return _Kept(keys, r.left_pad, r.left_pad + len(keys), self._clock)
+
+    def cached_prefix(self, signature):
+        """how many leading elements of a prompt's front-end signature a kept or live slot of this scheduler holds (the
+        serving shell sends a request to the worker where this is longest).  Reads the snapshot `step()` publishes, so it
+        may be called from any thread."""
+        best = 0
+        for sig in self._signatures:
+            n = 0
+            for a, b in zip(signature or (), sig or ()):
+                if a != b:
+                    break
+                n += 1
+            best = max(best, n)
+        return best
 
     def _join(self, items):
         """one emu_llm_join for `items`; raises only if nothing was joined.  After the join every request is on its own: a
@@ -273,11 +463,17 @@ class SlotScheduler(_RequestQueue):
             embeds[i, N - e.shape[1]:] = e[0]
             mask[i, N - e.shape[1]:] = m[0].to(torch.int32)
         logits = self.engine.join([r.slots[0] for r, _ in items], embeds, mask)
+        for r, (e, _) in items:
+            r.left_pad = N - e.shape[1]
+        self._start(items, logits, [N] * len(items))
+
+    def _start(self, items, logits, lengths):
+        """the joined / resumed first slots (lengths: their cache lengths) become live requests: beam groups fork"""
         for r, _ in items:
             r.engine_slots = [r.slots[0]]
         for i, (r, _) in enumerate(items):
             try:
-                r.max_new_tokens = self._cap(r, N)          # the room it has alone (_join_groups)
+                r.max_new_tokens = self._cap(r, lengths[i])  # the room it has alone (_join_groups, _match)
                 if r.num_beams > 1:
                     self.engine.fork(r.slots[0], r.slots[1:])
                     r.engine_slots = list(r.slots)
@@ -332,10 +528,19 @@ class SlotScheduler(_RequestQueue):
             self.src_buf[r.slots[0]:r.slots[-1] + 1] = self.ident[r.slots[0]:r.slots[-1] + 1]
         held, r.engine_slots = r.engine_slots, []
         if held:
+            keep = self._keep(r) if self.prefix_cache and r.error is None and r.selector is not None else None
             try:
-                self.engine.leave(held)
+                if keep is None:
+                    self.engine.leave(held)
+                else:
+                    self.engine.leave_keep(held, [keep.length] + [0] * (len(held) - 1))
+                    keep.signature = r.signature
+                    self.kept[held[0]] = keep
             except Exception:
-                pass
+                try:
+                    self.engine.leave(held)
+                except Exception:
+                    pass
 
     # ---- decode ----
     def _decode(self):
@@ -352,13 +557,21 @@ class SlotScheduler(_RequestQueue):
             r.logits = self.logits_buf[r.slots[0]:r.slots[0] + r.num_beams]
 
 
+class _Kept:
+    """a kept slot of the prefix cache: its key sequence, left padding, kept length (cache positions) and last use"""
+
+    def __init__(self, keys, pad, length, used):
+        self.keys, self.left_pad, self.length, self.used = keys, pad, length, used
+        self.signature = None
+
+
 def _on_device(device):
     """the engine enqueues on the current stream of the current device: make that the scheduler's device"""
     import contextlib
     return torch.cuda.device(device) if device.type == "cuda" else contextlib.nullcontext()
 
 
-def chat_request(chat, inputs, is_grounding=False, skip_special_tokens=True, **knobs):
+def chat_request(chat, inputs, is_grounding=False, skip_special_tokens=True, prefix_keys=False, **knobs):
     """one EmuChatGeneration call (`chat(inputs, **knobs)`) as a SlotRequest whose result is the decoded answer: the same
     prompt assembly, tokenisation and picture transform as `forward`, and the same `skip_special_tokens` decoding"""
     model = chat.emu_model
@@ -367,8 +580,50 @@ def chat_request(chat, inputs, is_grounding=False, skip_special_tokens=True, **k
     tok = model.decoder.tokenizer
     knobs = dict(knobs)
     knobs.pop("synced_gpus", None)
+    keys = sig = None
+    if prefix_keys:                                         # only a prefix-caching scheduler reads them
+        pics = _pictures(inputs)
+        keys = [picture_key(p) for p in pics] if image is not None and len(pics) == image.shape[0] else None
+        sig = prompt_signature(inputs)
     return SlotRequest(input_ids, mask, image=image, video=video, image_token_id=IMAGE, video_token_id=VIDEO,
-                       finish=lambda ids: tok.batch_decode(ids, skip_special_tokens=skip_special_tokens)[0], **knobs)
+                       finish=lambda ids: tok.batch_decode(ids, skip_special_tokens=skip_special_tokens)[0],
+                       image_keys=keys, signature=sig, **knobs)
+
+
+def picture_key(picture):
+    """the prefix-cache key of a picture: a blake2b digest of its RGB pixels and their shape, taken before any transform"""
+    key = getattr(picture, "_emu_prefix_key", None)        # computed once per picture object (routing, then the request)
+    if key is not None:
+        return key
+    import hashlib
+    import numpy as np
+    a = np.ascontiguousarray(np.asarray(picture.convert("RGB"), dtype=np.uint8))
+    h = hashlib.blake2b(digest_size=32)
+    h.update(repr(a.shape).encode())
+    h.update(a.tobytes())
+    key = h.hexdigest()
+    try:
+        picture._emu_prefix_key = key
+    except AttributeError:
+        pass
+    return key
+
+
+def prompt_signature(inputs):
+    """the front end's view of a prompt: its elements in order, strings as they are and pictures as their digests"""
+    return [picture_key(x) if hasattr(x, "convert") else x for x in _flatten(inputs)]
+
+
+def _flatten(inputs):
+    for x in inputs:
+        if isinstance(x, (list, tuple)):
+            yield from _flatten(x)
+        else:
+            yield x
+
+
+def _pictures(inputs):
+    return [x for x in _flatten(inputs) if hasattr(x, "convert")]
 
 
 # ---- continuous batching for image generation ----

@@ -27,7 +27,8 @@ def _digest():
     h = hashlib.sha256()
     for f in sorted(os.listdir(CSRC)) + ["../../include/emu_b200.h", "../../include/emu_b200_safety.h",
                                         "../../include/emu_b200_slots.h", "../../include/emu_b200_ops.h",
-                                        "../../include/emu_b200_gen_slots.h", "../../include/emu_b200_diffusion_ops.h"]:
+                                        "../../include/emu_b200_gen_slots.h", "../../include/emu_b200_diffusion_ops.h",
+                                        "../../include/emu_b200_prefix.h"]:
         p = os.path.join(CSRC, f)
         if os.path.isfile(p):
             h.update(f.encode())

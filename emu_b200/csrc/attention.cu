@@ -269,7 +269,8 @@ __device__ __forceinline__ void fa_load_tile(bf16* dst, const bf16* src, long ts
   }
 }
 
-template <int DP>
+// kRowOff: the causal offset is per batch, a.q_off[b] (prefix caching)
+template <int DP, bool kRowOff>
 __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs a) {
   constexpr int LD = FaSmem<DP>::LD;
   constexpr int KS = DP / 16;  // k-steps over the head dim
@@ -289,16 +290,18 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
   const bf16* kp = a.k + (long)kvb * a.k_bs + (long)h * a.k_hs;
   const bf16* vp = a.v + (long)kvb * a.v_bs + (long)h * a.v_hs;
   const int kv_lo = a.kv_start ? a.kv_start[b] : 0;
-  const int shift = a.Nk - a.Nq;  // causal: key j visible to query i iff j <= i + shift
-  int kv_hi = a.Nk;
-  if (a.causal) kv_hi = min(a.Nk, q0 + kFaBM + shift);
+  const int shift = kRowOff ? a.q_off[b] : a.Nk - a.Nq;  // causal: key j visible to query i iff j <= i + shift
+  // keys of this batch: all Nk, or (kRowOff) up to the end of its real rows; past it the tiles load as zeros
+  const int kv_n = kRowOff ? min(a.Nk, shift + (a.q_len ? a.q_len[b] : a.Nq)) : a.Nk;
+  int kv_hi = kv_n;
+  if (a.causal) kv_hi = min(kv_n, q0 + kFaBM + shift);
   const int nb0 = kv_lo / kFaBN;
   const int nb1 = (kv_hi + kFaBN - 1) / kFaBN;
 
   fa_load_tile<DP>(sQ, qp, a.q_ts, q0, a.Nq, a.D);
   if (nb0 < nb1) {
-    fa_load_tile<DP>(sK, kp, a.k_ts, nb0 * kFaBN, a.Nk, a.D);
-    fa_load_tile<DP>(sV, vp, a.v_ts, nb0 * kFaBN, a.Nk, a.D);
+    fa_load_tile<DP>(sK, kp, a.k_ts, nb0 * kFaBN, kv_n, a.D);
+    fa_load_tile<DP>(sV, vp, a.v_ts, nb0 * kFaBN, kv_n, a.D);
   }
   cp_async_commit();
 
@@ -315,8 +318,8 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
   for (int nb = nb0; nb < nb1; ++nb) {
     const int buf = (nb - nb0) & 1;
     if (nb + 1 < nb1) {
-      fa_load_tile<DP>(sK + (buf ^ 1) * FaSmem<DP>::kTile, kp, a.k_ts, (nb + 1) * kFaBN, a.Nk, a.D);
-      fa_load_tile<DP>(sV + (buf ^ 1) * FaSmem<DP>::kTile, vp, a.v_ts, (nb + 1) * kFaBN, a.Nk, a.D);
+      fa_load_tile<DP>(sK + (buf ^ 1) * FaSmem<DP>::kTile, kp, a.k_ts, (nb + 1) * kFaBN, kv_n, a.D);
+      fa_load_tile<DP>(sV + (buf ^ 1) * FaSmem<DP>::kTile, vp, a.v_ts, (nb + 1) * kFaBN, kv_n, a.D);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -365,7 +368,7 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
         const int kj = key0 + nt * 8 + 2 * t + (j & 1);
         float x = s[nt][j] * a.scale;
         if (a.bias != nullptr && qi < a.Nq && kj < a.Nk) x += a.bias[((long)h * a.Nq + qi) * a.Nk + kj];
-        const bool vis = kj < a.Nk && kj >= kv_lo && (!a.causal || kj <= qi + shift);
+        const bool vis = kj < kv_n && kj >= kv_lo && (!a.causal || kj <= qi + shift);
         x = vis ? x : -INFINITY;
         s[nt][j] = x;
         mx[j >> 1] = fmaxf(mx[j >> 1], x);
@@ -441,17 +444,17 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
   }
 }
 
-template <int DP>
+template <int DP, bool kRowOff = false>
 static int launch_fa(const AttnArgs& a, cudaStream_t st) {
   static bool set = false;
   if (!set) {
-    if (cudaFuncSetAttribute(attn_prefill_kernel<DP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    if (cudaFuncSetAttribute(attn_prefill_kernel<DP, kRowOff>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              FaSmem<DP>::kBytes) != cudaSuccess)
       return EMU_ERR_CUDA;
     set = true;
   }
   dim3 grid((a.Nq + kFaBM - 1) / kFaBM, a.H, a.B);
-  attn_prefill_kernel<DP><<<grid, kFaThreads, FaSmem<DP>::kBytes, st>>>(a);
+  attn_prefill_kernel<DP, kRowOff><<<grid, kFaThreads, FaSmem<DP>::kBytes, st>>>(a);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
@@ -470,6 +473,12 @@ int attn_prefill(const AttnArgs& a, cudaStream_t st) {
   if (!legacy) {
     const int rc = attn_prefill_tc(a, st);
     if (rc != EMU_ERR_UNSUPPORTED) return rc;
+  }
+  if (a.q_off) {  // prefix caching: causal, the LLaMA head dims only
+    if (!a.causal || a.bias) return EMU_ERR_INVALID;
+    if (a.D == 64) return launch_fa<64, true>(a, st);
+    if (a.D == 128) return launch_fa<128, true>(a, st);
+    return EMU_ERR_INVALID;
   }
   if (a.D <= 32) return launch_fa<32>(a, st);
   if (a.D <= 64) return launch_fa<64>(a, st);

@@ -47,6 +47,8 @@ struct AtParams {
   long o_bs, o_ts, o_hs;
   const int* kv_start;
   const int* kv_row;  // [B] K/V batch coordinate of query batch b, or null = b
+  const int* q_off;   // [B] kRowOff: key position of query 0 of batch b (AttnArgs::q_off)
+  const int* q_len;   // [B] kRowOff: real query rows of batch b, or null = Nq (AttnArgs::q_len)
   int Nq, Nk, D;  // D = real head dim (<= DT)
   int causal;
   float scale_log2;  // scale * log2(e)
@@ -60,7 +62,8 @@ __device__ __forceinline__ void load_rows(void* dst, const CUtensorMap* m, uint6
   else tma_load_4d(dst, m, bar, d0, tok, head, batch);
 }
 
-template <int DT, int BN>
+// kRowOff: the causal offset is per batch (prefix caching), so each CTA bounds its key loop by its own batch's offset
+template <int DT, int BN, bool kRowOff>
 __global__ void __launch_bounds__(AtCfg<DT, BN>::kThreads, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AtParams p) {
@@ -76,8 +79,10 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128, head = blockIdx.y, batch = blockIdx.z;
-  const int off = p.Nk - p.Nq;
-  int kmax = p.Nk - 1;  // last key any query row of this CTA may see
+  const int off = kRowOff ? p.q_off[batch] : p.Nk - p.Nq;
+  // keys of this batch: all Nk, or (kRowOff) up to the end of its real rows, which is all the caller wrote
+  const int kv_n = kRowOff ? min(p.Nk, off + (p.q_len ? p.q_len[batch] : p.Nq)) : p.Nk;
+  int kmax = kv_n - 1;  // last key any query row of this CTA may see
   if (p.causal) kmax = min(kmax, min(q0 + 127, p.Nq - 1) + off);
   const int nb = kmax < 0 ? 0 : kmax / BN + 1;
 
@@ -131,7 +136,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     const int lo = p.kv_start ? p.kv_start[batch] : 0;
     int hi[2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) hi[h] = p.causal ? min(p.Nk - 1, qi[h] + off) : p.Nk - 1;
+    for (int h = 0; h < 2; ++h) hi[h] = p.causal ? min(kv_n - 1, qi[h] + off) : kv_n - 1;
     float o[DT / 2];
 #pragma unroll
     for (int i = 0; i < DT / 2; ++i) o[i] = 0.f;
@@ -193,6 +198,18 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
       for (int i = 0; i < DT / 2; ++i) o[i] *= corr[(i >> 1) & 1];
       // ---- O += P V_j : V is used in place as an MN-major B operand (64-wide d chunks BN*128 B apart, 8-key groups 1 KB) ----
       mbar_wait(&v_full[s], ph);
+      if (kRowOff && k0 + BN > kv_n) {
+        // the tile runs past this batch's last written key: zero those V rows (128 B each in every 64-wide chunk, whatever
+        // the swizzle) so a stale non-finite value cannot reach O through a zero probability.  Both consumer warpgroups
+        // write the same zeros; each makes its own writes visible to its wgmma before issuing it.
+        uint8_t* vt = smem + C::kOffV + s * C::kKVBytes;
+        const int r0 = kv_n - k0, units = (BN - r0) * 8, tid = threadIdx.x - 128 * (wg + 1);
+        for (int cc = 0; cc < C::kDC; ++cc)
+          for (int u = tid; u < units; u += 128)
+            *reinterpret_cast<uint4*>(vt + cc * (BN * 128) + r0 * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory");
+      }
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < BN / 16; ++kk)
@@ -222,12 +239,12 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   }
 }
 
-template <int DT, int BN>
+template <int DT, int BN, bool kRowOff = false>
 int launch_attn_tc(const AttnArgs& a, cudaStream_t st) {
   using C = AtCfg<DT, BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(attn_tc_kernel<DT, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem) != cudaSuccess)
+    if (cudaFuncSetAttribute(attn_tc_kernel<DT, BN, kRowOff>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem) != cudaSuccess)
       return EMU_ERR_CUDA;
     attr_set = true;
   }
@@ -238,11 +255,11 @@ int launch_attn_tc(const AttnArgs& a, cudaStream_t st) {
   if (make_tmap_bnhd(&tk, a.k, a.D, a.Nk, a.H, kvB, a.k_ts, a.k_hs, a.k_bs, BN, &p.k_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
   if (make_tmap_bnhd(&tv, a.v, a.D, a.Nk, a.H, kvB, a.v_ts, a.v_hs, a.v_bs, BN, &p.v_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
   p.out = a.out; p.o_bs = a.o_bs; p.o_ts = a.o_ts; p.o_hs = a.o_hs;
-  p.kv_start = a.kv_start; p.kv_row = a.kv_row; p.Nq = a.Nq; p.Nk = a.Nk; p.D = a.D; p.causal = a.causal;
+  p.kv_start = a.kv_start; p.kv_row = a.kv_row; p.q_off = a.q_off; p.q_len = a.q_len; p.Nq = a.Nq; p.Nk = a.Nk; p.D = a.D; p.causal = a.causal;
   p.scale_log2 = a.scale * 1.4426950408889634f;
   p.pdl = g_pdl_chain;
   dim3 grid((a.Nq + 127) / 128, a.H, a.B);
-  return launch_kernel(attn_tc_kernel<DT, BN>, grid, dim3(C::kThreads), C::kSmem, st, p.pdl, tq, tk, tv, p);
+  return launch_kernel(attn_tc_kernel<DT, BN, kRowOff>, grid, dim3(C::kThreads), C::kSmem, st, p.pdl, tq, tk, tv, p);
 }
 
 }  // namespace
@@ -256,6 +273,12 @@ int attn_prefill_tc(const AttnArgs& a, cudaStream_t st) {
   if ((reinterpret_cast<uintptr_t>(a.q) & 15) || (reinterpret_cast<uintptr_t>(a.k) & 15) || (reinterpret_cast<uintptr_t>(a.v) & 15))
     return EMU_ERR_UNSUPPORTED;
   if (a.H > 65535 || a.B > 65535) return EMU_ERR_UNSUPPORTED;
+  if (a.q_off) {  // prefix caching: the LLaMA head dims only
+    if (!a.causal) return EMU_ERR_UNSUPPORTED;
+    if (a.D == 64) return launch_attn_tc<64, 128, true>(a, st);
+    if (a.D == 128) return launch_attn_tc<128, 64, true>(a, st);
+    return EMU_ERR_UNSUPPORTED;
+  }
   if (a.D <= 64) {
     if (a.Nk <= 64) return launch_attn_tc<64, 64>(a, st);  // cross-attention: 64 keys
     return launch_attn_tc<64, 128>(a, st);

@@ -195,10 +195,13 @@ int layernorm(const bf16* x, const bf16* w, const bf16* b, const bf16* residual,
 // prefill: RoPE on q (in place) and k, append k/v to the cache.  q/k head dims are pair-interleaved
 // (element 2j = original j, 2j+1 = original j + D/2) by the weight packer, so a rotation pair is one 4-byte word.
 // ----------------------------------------------------------------------------------------------
+// kRows (prefix caching, emu_llm_extend): batch b's tokens sit at cache slots pos_dev[b] + n and only the first n_dev[b] of
+// its N tokens are real (right padding); the padding is neither rotated nor written
+template <bool kRows>
 __global__ void rope_kv_write_kernel(bf16* qkv, int B, int N, int H, int D, const bf16* __restrict__ cos_t,
                                      const bf16* __restrict__ sin_t, const int* pos_off, int pos0, bf16* k_cache,
                                      bf16* v_cache, int t_max, const int* __restrict__ pos_dev, bf16* q_out,
-                                     const int* __restrict__ kv_row) {
+                                     const int* __restrict__ kv_row, const int* __restrict__ n_dev) {
   const int half = D >> 1;
   const long total = (long)B * N * H * half;
   for (long idx = blockIdx.x * (long)blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
@@ -206,6 +209,7 @@ __global__ void rope_kv_write_kernel(bf16* qkv, int B, int N, int H, int D, cons
     const int h = (idx / half) % H;
     const int n = (idx / ((long)half * H)) % N;
     const int b = idx / ((long)half * H * N);
+    if (kRows && n >= n_dev[b]) continue;
     bf16* base = qkv + ((long)b * N + n) * 3 * H * D;
     // CUDA-graphed decode: the cache slot of every row's new token lives on the device (rows differ in slot mode)
     const int p0 = pos_dev ? pos_dev[b] : pos0;
@@ -234,8 +238,53 @@ int rope_kv_write(bf16* qkv, int B, int N, int H, int D, const bf16* cos_t, cons
                   const int* kv_row) {
   const long total = (long)B * N * H * (D / 2);
   const int grid = (int)((total + 255) / 256 < 4 * kNumSMs ? (total + 255) / 256 : 4 * kNumSMs);
-  rope_kv_write_kernel<<<grid, 256, 0, st>>>(qkv, B, N, H, D, cos_t, sin_t, pos_off, pos0, k_cache, v_cache, t_max, pos_dev, q_out,
-                                             kv_row);
+  rope_kv_write_kernel<false><<<grid, 256, 0, st>>>(qkv, B, N, H, D, cos_t, sin_t, pos_off, pos0, k_cache, v_cache, t_max, pos_dev,
+                                                    q_out, kv_row, nullptr);
+  return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
+}
+
+int rope_kv_write_rows(bf16* qkv, int B, int N, int H, int D, const bf16* cos_t, const bf16* sin_t, const int* pos_off,
+                       const int* q0, const int* n_new, bf16* k_cache, bf16* v_cache, int t_max, const int* kv_row,
+                       cudaStream_t st) {
+  const long total = (long)B * N * H * (D / 2);
+  const int grid = (int)((total + 255) / 256 < 4 * kNumSMs ? (total + 255) / 256 : 4 * kNumSMs);
+  rope_kv_write_kernel<true><<<grid, 256, 0, st>>>(qkv, B, N, H, D, cos_t, sin_t, pos_off, 0, k_cache, v_cache, t_max, q0, nullptr,
+                                                   kv_row, n_new);
+  return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
+}
+
+// prefix caching: cache positions [0, P) of row src -> row dst in every (layer, k/v, head) plane of a [outer][rows][H][t_max][D]
+// cache.  Each plane's prefix is P*D contiguous elements, moved as 16-byte words; 4 independent words in flight per thread
+// keep enough loads outstanding for a copy that is bound by HBM bandwidth.
+__global__ void kv_prefix_copy_kernel(bf16* cache, int rows, int H, int t_max, int D, int src, int dst, long per, long total) {
+  const long stride = (long)gridDim.x * blockDim.x;
+  for (long i0 = blockIdx.x * (long)blockDim.x + threadIdx.x; i0 < total; i0 += 4 * stride) {
+    uint4 v[4];
+    long off[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const long idx = i0 + u * stride;
+      off[u] = -1;
+      if (idx < total) {
+        const long w = idx % per, plane = idx / per;  // plane = o * H + h
+        const long o = plane / H, h = plane % H;
+        const long base = ((o * rows) * H + h) * t_max * D / 8 + w;
+        off[u] = base;
+        v[u] = __ldg(reinterpret_cast<const uint4*>(cache) + base + (long)src * H * t_max * D / 8);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u)
+      if (off[u] >= 0) reinterpret_cast<uint4*>(cache)[off[u] + (long)dst * H * t_max * D / 8] = v[u];
+  }
+}
+
+int kv_prefix_copy(bf16* cache, long outer, int rows, int H, int D, int t_max, int src, int dst, int P, cudaStream_t st) {
+  const long per = (long)P * D / 8;  // 16-byte words per plane
+  const long total = outer * H * per;
+  const long want = (total + 4 * 256 - 1) / (4 * 256);
+  const int grid = (int)(want < 8 * kNumSMs ? want : 8 * kNumSMs);
+  kv_prefix_copy_kernel<<<grid, 256, 0, st>>>(cache, rows, H, t_max, D, src, dst, per, total);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 

@@ -6,6 +6,7 @@
 //   LLaMA    : HF LlamaModel.forward as driven by Emu2/emu/emu.py:133-138 (prefill, hidden_states[-1]) and
 //              :213-229 (generate: prefill + one-token steps with KV cache)
 #include "engine.h"
+#include "../../include/emu_b200_prefix.h"
 #include "../../include/emu_b200_slots.h"
 
 #include <dlfcn.h>
@@ -126,6 +127,67 @@ __global__ void slot_fork_kernel(int src, SlotList dst, int* pos, int* start, in
     posoff[row] = posoff[src];
     active[row] = 1;
   }
+}
+// prefix caching: slots leave keeping their first keep.r[b] cache positions (0 = a plain leave, as slot_set_kernel).  The real
+// left-pad start / position offset move to the kept arrays, and the slot is parked at pos = start = keep: the decode step
+// computes every free slot below B and appends its junk token at pos, which then lands at position keep, past the kept
+// prefix (a resume overwrites it before anything reads it), and its attention reads that one key.
+__global__ void slot_keep_kernel(SlotList rows, SlotList keep, int* pos, int* start, int* posoff, int* active, int* kept_start,
+                                 int* kept_posoff, int* indir, int t_max) {
+  const int b = blockIdx.x, row = rows.r[b], k = keep.r[b];
+  if (threadIdx.x == 0) {
+    kept_start[row] = k > 0 ? start[row] : 0;
+    kept_posoff[row] = k > 0 ? posoff[row] : 0;
+    pos[row] = k;
+    start[row] = k;
+    posoff[row] = 0;
+    active[row] = 0;
+  }
+  for (int t = threadIdx.x; t < t_max; t += blockDim.x) indir[(long)row * t_max + t] = row;
+}
+// prefix caching: free slot dst becomes kept with P positions copied from src (live: its current start / offset; kept: its
+// saved ones).  One CTA.
+__global__ void slot_copy_state_kernel(int src, int src_kept, int dst, int P, int* pos, int* start, int* posoff, int* active,
+                                       int* kept_start, int* kept_posoff, int* indir, int t_max) {
+  if (threadIdx.x == 0) {
+    kept_start[dst] = src_kept ? kept_start[src] : start[src];
+    kept_posoff[dst] = src_kept ? kept_posoff[src] : posoff[src];
+    pos[dst] = P;
+    start[dst] = P;
+    posoff[dst] = 0;
+    active[dst] = 0;
+  }
+  for (int t = threadIdx.x; t < t_max; t += blockDim.x) indir[(long)dst * t_max + t] = dst;
+}
+// emu_llm_extend, before the layers: the join-local start / position offset of every resuming slot (its kept ones; zero for
+// a slot that starts from nothing).  One thread per slot.
+__global__ void slot_resume_begin_kernel(SlotList rows, SlotList prefix, const int* __restrict__ kept_start,
+                                         const int* __restrict__ kept_posoff, int* join_start, int* join_posoff, int n) {
+  const int b = threadIdx.x;
+  if (b >= n) return;
+  const int row = rows.r[b], p = prefix.r[b];
+  join_start[b] = p > 0 ? kept_start[row] : 0;
+  join_posoff[b] = p > 0 ? kept_posoff[row] : 0;
+}
+// ... after the layers: the slots are live at length len.r[b].  One CTA per slot.
+__global__ void slot_resume_end_kernel(SlotList rows, SlotList len, const int* __restrict__ join_start,
+                                       const int* __restrict__ join_posoff, int* pos, int* start, int* posoff, int* active,
+                                       int* indir, int t_max) {
+  const int b = blockIdx.x, row = rows.r[b];
+  if (threadIdx.x == 0) {
+    pos[row] = len.r[b];
+    start[row] = join_start[b];
+    posoff[row] = join_posoff[b];
+    active[row] = 1;
+  }
+  for (int t = threadIdx.x; t < t_max; t += blockDim.x) indir[(long)row * t_max + t] = row;
+}
+// the hidden row of every sequence's last real token: row b * N + n_new[b] - 1 -> out row b (16-byte words)
+__global__ void gather_last_rows_kernel(const bf16* __restrict__ h, int N, int Hd, const int* __restrict__ n_new, bf16* out) {
+  const int b = blockIdx.x;
+  const uint4* src = reinterpret_cast<const uint4*>(h + ((long)b * N + n_new[b] - 1) * Hd);
+  uint4* dst = reinterpret_cast<uint4*>(out + (long)b * Hd);
+  for (int i = threadIdx.x; i < Hd / 8; i += blockDim.x) dst[i] = src[i];
 }
 __global__ void argmax_ban_kernel(float* logits, int cols, int ban) {
   if (ban >= 0 && ban < cols) logits[(long)blockIdx.x * cols + ban] = -INFINITY;
@@ -333,6 +395,9 @@ extern "C" int emu_engine_create(const EmuConfig* cfg, int tp_rank, int tp_size,
     e->d_join_rows = e->d_active + kLlmMaxRows;
     e->d_join_start = e->d_active + 2 * kLlmMaxRows;
     e->d_join_posoff = e->d_active + 3 * kLlmMaxRows;
+    e->d_kept_start = (int*)e->dmalloc(5 * kLlmMaxRows * sizeof(int));
+    e->d_kept_posoff = e->d_kept_start + kLlmMaxRows;
+    e->d_ext = e->d_kept_start + 2 * kLlmMaxRows;
     if (c.llm_max_batch > 8) {  // wide decode (more than 8 cache rows: the C4 workload, 4 prompts x 5 beams) runs on the GEMM path
       e->dec_xn = (bf16*)e->dmalloc((size_t)c.llm_max_batch * c.llm_hidden * 2);
       e->dec_qkv = (bf16*)e->dmalloc((size_t)c.llm_max_batch * 3 * e->Hl * c.llm_head_dim * 2);
@@ -363,7 +428,7 @@ extern "C" int emu_engine_create(const EmuConfig* cfg, int tp_rank, int tp_size,
     e->dec_logits_shard = (float*)e->dmalloc(((size_t)Bm * e->Vl + 4) * sizeof(float));
     e->dec_part = (float*)e->dmalloc((size_t)Bm * c.llm_hidden * sizeof(float));
     e->dec_logits_gather = (float*)e->dmalloc((size_t)Bm * e->Vl * tp_size * sizeof(float));
-    if (!e->rope_cos || !e->rope_sin || !e->kv || !e->d_pos || !e->d_active || !e->dec_h || !e->dec_q || !e->dec_attn || !e->dec_act ||
+    if (!e->rope_cos || !e->rope_sin || !e->kv || !e->d_pos || !e->d_active || !e->d_kept_start || !e->dec_h || !e->dec_q || !e->dec_attn || !e->dec_act ||
         !e->dec_tmp || !e->dec_attn_ws || !e->dec_counters || !e->dec_logits_local || !e->kv_indir) {
       emu_engine_destroy(e);
       return EMU_ERR_NOMEM;
@@ -372,6 +437,7 @@ extern "C" int emu_engine_create(const EmuConfig* cfg, int tp_rank, int tp_size,
     cudaMemset(e->dec_counters, 0, (size_t)Bm * e->Hl * sizeof(int));
     cudaMemset(e->d_pos, 0, 3 * kLlmMaxRows * sizeof(int));
     cudaMemset(e->d_active, 0, 4 * kLlmMaxRows * sizeof(int));
+    cudaMemset(e->d_kept_start, 0, 5 * kLlmMaxRows * sizeof(int));
     kv_indir_identity(e->kv_indir, Bm, c.llm_max_seq, 0);
   }
   if (c.vit_layers > 0) {
@@ -763,6 +829,9 @@ extern "C" int emu_llm_reset(EmuEngine* e, emu_stream_t s) {
   e->n_slots = 0;
   e->slot_len.clear();
   e->slot_group.clear();
+  e->slot_kept.clear();
+  e->slot_own.clear();
+  e->slot_grows.clear();
   if (e->d_pos && cudaMemsetAsync(e->d_pos, 0, 3 * kLlmMaxRows * sizeof(int), (cudaStream_t)s) != cudaSuccess) return EMU_ERR_CUDA;
   if (e->kv_indir && e->kv_indir_dirty) {
     EMU_TRY(kv_indir_identity(e->kv_indir, e->cfg.llm_max_batch, e->cfg.llm_max_seq, (cudaStream_t)s));
@@ -856,9 +925,11 @@ static int prefill_stage(EmuEngine* e, const void* inputs_embeds, long M, cudaSt
 }
 
 // the decoder layers over the B x N prompt tokens in pf_h: k / v of batch b go to cache row kv_row[b] (null: row b) at
-// slots [pos0, pos0 + N), rotated at position slot - posoff[b]; the attention reads keys [start[b], pos0 + N) of that row
+// slots [pos0, pos0 + N), rotated at position slot - posoff[b]; the attention reads keys [start[b], pos0 + N) of that row.
+// With q0 (prefix caching, device [B]): batch b's tokens go to slots [q0[b], q0[b] + n_new[b]) instead (the rest of its N
+// rows are right padding) and read keys [start[b], q0[b] + i]; Nk = the key extent of the longest row.
 static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start, const int* posoff, const int* kv_row,
-                          cudaStream_t st) {
+                          cudaStream_t st, const int* q0 = nullptr, const int* n_new = nullptr, int Nk = 0) {
   const EmuConfig& c = e->cfg;
   const int Hd = c.llm_hidden, D = c.llm_head_dim, Hl = e->Hl, Fl = e->Fl;
   const long M = (long)B * N;
@@ -877,8 +948,9 @@ static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start
     GemmEpilogue ep;
     ep.C = qkv; ep.ldc = 3 * Hl * D;
     EMU_TRY(gemm_bf16(xn, Hd, L.wqkv, Hd, (int)M, 3 * Hl * D, Hd, ep, st));
-    EMU_TRY(rope_kv_write(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, pos0, kc, vc, c.llm_max_seq, st, nullptr, nullptr,
-                          kv_row));
+    if (q0) EMU_TRY(rope_kv_write_rows(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, q0, n_new, kc, vc, c.llm_max_seq, kv_row, st));
+    else EMU_TRY(rope_kv_write(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, pos0, kc, vc, c.llm_max_seq, st, nullptr, nullptr,
+                               kv_row));
     AttnArgs a;
     a.q = qkv; a.q_bs = (long)N * 3 * Hl * D; a.q_ts = 3 * Hl * D; a.q_hs = D;
     a.k = kc; a.k_bs = (long)Hl * c.llm_max_seq * D; a.k_hs = (long)c.llm_max_seq * D; a.k_ts = D;
@@ -886,6 +958,11 @@ static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start
     a.out = att; a.o_bs = (long)N * Hl * D; a.o_ts = Hl * D; a.o_hs = D;
     a.B = B; a.H = Hl; a.Nq = N; a.Nk = pos0 + N; a.D = D; a.scale = scale; a.causal = 1; a.kv_start = start;
     a.kv_row = kv_row; a.kv_rows = kv_row ? c.llm_max_batch : 0;
+    if (q0) {
+      a.q_off = q0;
+      a.q_len = n_new;
+      a.Nk = Nk;
+    }
     EMU_TRY(attn_prefill(a, st));
     if (e->tp_size == 1) {
       GemmEpilogue eo;
@@ -920,12 +997,22 @@ static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start
   return EMU_OK;
 }
 
-// final norm of every prompt token (last_hidden) and the logits of every sequence's last position (logits_last)
-static int prefill_outputs(EmuEngine* e, int B, int N, void* last_hidden, float* logits_last, cudaStream_t st) {
+// final norm of every prompt token (last_hidden) and the logits of every sequence's last position (logits_last).  With n_new
+// (device [B], right-padded rows): the logits of row b's token n_new[b] - 1, gathered to pf_last first.
+static int prefill_outputs(EmuEngine* e, int B, int N, void* last_hidden, float* logits_last, cudaStream_t st,
+                           const int* n_new = nullptr) {
   const EmuConfig& c = e->cfg;
   const int Hd = c.llm_hidden;
   const long M = (long)B * N;
   bf16* h = (bf16*)e->pf_h.p;
+  if (n_new && logits_last) {
+    EMU_TRY(e->ensure(e->pf_last, (size_t)B * Hd * 2));
+    gather_last_rows_kernel<<<B, 128, 0, st>>>(h, N, Hd, n_new, (bf16*)e->pf_last.p);
+    count_launch();
+    if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "last-token gather failed");
+    h = (bf16*)e->pf_last.p;
+    N = 1;
+  }
   if (last_hidden) {
     EMU_TRY(rmsnorm(h, e->final_norm, (bf16*)last_hidden, (int)M, Hd, c.llm_rms_eps, 0, st));
     count_launch();
@@ -934,8 +1021,8 @@ static int prefill_outputs(EmuEngine* e, int B, int N, void* last_hidden, float*
     // more rows than the skinny GEMV takes: final norm of the last position of every sequence, then the wgmma GEMM
     EMU_TRY(e->ensure(e->pf_last, (size_t)B * Hd * 2));
     bf16* last = (bf16*)e->pf_last.p;
-    if (cudaMemcpy2DAsync(last, (size_t)Hd * 2, h + (size_t)(N - 1) * Hd, (size_t)N * Hd * 2, (size_t)Hd * 2, B,
-                          cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+    if (!n_new && cudaMemcpy2DAsync(last, (size_t)Hd * 2, h + (size_t)(N - 1) * Hd, (size_t)N * Hd * 2, (size_t)Hd * 2, B,
+                                    cudaMemcpyDeviceToDevice, st) != cudaSuccess)
       return e->fail(EMU_ERR_CUDA, "last-position gather failed");
     EMU_TRY(rmsnorm(last, e->final_norm, last, B, Hd, c.llm_rms_eps, 0, st));
     GemmEpilogue el;
@@ -1317,7 +1404,10 @@ extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void
   }
   if (e->n_slots > 0) {
     for (int b = 0; b < B; ++b)
-      if (e->slot_group[b] >= 0) e->slot_len[b] += 1;
+      if (e->slot_group[b] >= 0) {
+        e->slot_len[b] += 1;
+        if (e->slot_grows[b]) e->slot_own[b] += 1;
+      }
   } else {
     e->cur_len += 1;
   }
@@ -1349,6 +1439,21 @@ static int check_slots(EmuEngine* e, const int32_t* slots, int n, bool want_free
   return EMU_OK;
 }
 
+// a beam group leaves together: its slots' table rows point into each other
+static int check_groups_leave(EmuEngine* e, const SlotList& rows, int n) {
+  for (int b = 0; b < e->n_slots; ++b) {
+    if (e->slot_group[b] < 0) continue;
+    bool named = false, group_named = false;
+    for (int i = 0; i < n; ++i) {
+      named |= rows.r[i] == b;
+      group_named |= e->slot_group[rows.r[i]] == e->slot_group[b];
+    }
+    if (group_named && !named)
+      return e->fail(EMU_ERR_STATE, "slot " + std::to_string(b) + " belongs to a leaving beam group and must leave with it");
+  }
+  return EMU_OK;
+}
+
 extern "C" int emu_llm_slots_begin(EmuEngine* e, int n_slots, emu_stream_t s) {
   if (!e) return EMU_ERR_INVALID;
   const EmuConfig& c = e->cfg;
@@ -1364,6 +1469,9 @@ extern "C" int emu_llm_slots_begin(EmuEngine* e, int n_slots, emu_stream_t s) {
   e->n_slots = n_slots;
   e->slot_len.assign(n_slots, 0);
   e->slot_group.assign(n_slots, -1);
+  e->slot_kept.assign(n_slots, 0);
+  e->slot_own.assign(n_slots, 0);
+  e->slot_grows.assign(n_slots, 0);
   e->kv_indir_dirty = true;  // joins, forks and leaves rewrite table rows: emu_llm_reset restores the identity
   return EMU_OK;
 }
@@ -1394,6 +1502,9 @@ extern "C" int emu_llm_join(EmuEngine* e, const int32_t* host_slots, int n, cons
   for (int i = 0; i < n; ++i) {
     e->slot_len[rows.r[i]] = N;
     e->slot_group[rows.r[i]] = rows.r[i];
+    e->slot_kept[rows.r[i]] = 0;
+    e->slot_own[rows.r[i]] = N;
+    e->slot_grows[rows.r[i]] = 1;
   }
   return prefill_outputs(e, n, N, nullptr, logits_last, st);
 }
@@ -1413,7 +1524,11 @@ extern "C" int emu_llm_fork(EmuEngine* e, int src_slot, const int32_t* host_dst_
   for (int i = 0; i < n; ++i) {
     e->slot_len[dst.r[i]] = e->slot_len[src_slot];
     e->slot_group[dst.r[i]] = e->slot_group[src_slot];
+    e->slot_kept[dst.r[i]] = 0;
+    e->slot_own[dst.r[i]] = 0;  // its table row points into the source's row
+    e->slot_grows[dst.r[i]] = 0;
   }
+  e->slot_grows[src_slot] = 0;  // beam re-parenting scatters the group's new positions over its rows
   return EMU_OK;
 }
 
@@ -1422,17 +1537,7 @@ extern "C" int emu_llm_leave(EmuEngine* e, const int32_t* host_slots, int n, emu
   EMU_TRY(slot_mode_ok(e));
   SlotList rows;
   EMU_TRY(check_slots(e, host_slots, n, false, &rows));
-  // a beam group leaves together: its slots' table rows point into each other
-  for (int b = 0; b < e->n_slots; ++b) {
-    if (e->slot_group[b] < 0) continue;
-    bool named = false, group_named = false;
-    for (int i = 0; i < n; ++i) {
-      named |= rows.r[i] == b;
-      group_named |= e->slot_group[rows.r[i]] == e->slot_group[b];
-    }
-    if (group_named && !named)
-      return e->fail(EMU_ERR_STATE, "slot " + std::to_string(b) + " belongs to a leaving beam group and must leave with it");
-  }
+  EMU_TRY(check_groups_leave(e, rows, n));
   const EmuConfig& c = e->cfg;
   slot_set_kernel<<<n, 256, 0, (cudaStream_t)stream>>>(rows, nullptr, nullptr, 0, e->d_pos, e->d_start, e->d_posoff, e->d_active,
                                                        e->kv_indir, c.llm_max_seq);
@@ -1441,6 +1546,9 @@ extern "C" int emu_llm_leave(EmuEngine* e, const int32_t* host_slots, int n, emu
   for (int i = 0; i < n; ++i) {
     e->slot_len[rows.r[i]] = 0;
     e->slot_group[rows.r[i]] = -1;
+    e->slot_kept[rows.r[i]] = 0;
+    e->slot_own[rows.r[i]] = 0;
+    e->slot_grows[rows.r[i]] = 0;
   }
   return EMU_OK;
 }
@@ -1448,4 +1556,143 @@ extern "C" int emu_llm_leave(EmuEngine* e, const int32_t* host_slots, int n, emu
 extern "C" int emu_llm_slot_len(EmuEngine* e, int slot) {
   if (!e || e->n_slots < 1 || slot < 0 || slot >= e->n_slots) return -1;
   return e->slot_len[slot];
+}
+
+// ================================================================================================
+// prefix caching: kept slots and per-slot continuation (include/emu_b200_prefix.h)
+// ================================================================================================
+static int prefix_mode_ok(EmuEngine* e) {
+  if (e->tp_size > 1) return e->fail(EMU_ERR_UNSUPPORTED, "prefix caching under tensor parallelism");
+  return slot_mode_ok(e);
+}
+
+extern "C" int emu_llm_leave_keep(EmuEngine* e, const int32_t* host_slots, const int32_t* host_keep, int n, emu_stream_t stream) {
+  if (!e || !host_slots || !host_keep || n < 1) return EMU_ERR_INVALID;
+  EMU_TRY(prefix_mode_ok(e));
+  SlotList rows, keep;
+  EMU_TRY(check_slots(e, host_slots, n, false, &rows));
+  EMU_TRY(check_groups_leave(e, rows, n));
+  const EmuConfig& c = e->cfg;
+  for (int i = 0; i < n; ++i) {
+    const int s = rows.r[i], k = host_keep[i];
+    const int own = e->slot_own[s];
+    if (k < 0 || k > own || k > c.llm_max_seq - 1)
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " may keep 0 .. " +
+                                          std::to_string(own < c.llm_max_seq - 1 ? own : c.llm_max_seq - 1) +
+                                          " positions (its own-row length " + std::to_string(own) + "), asked for " +
+                                          std::to_string(k));
+    keep.r[i] = k;
+  }
+  slot_keep_kernel<<<n, 256, 0, (cudaStream_t)stream>>>(rows, keep, e->d_pos, e->d_start, e->d_posoff, e->d_active, e->d_kept_start,
+                                                        e->d_kept_posoff, e->kv_indir, c.llm_max_seq);
+  count_launch();
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot leave failed");
+  for (int i = 0; i < n; ++i) {
+    const int s = rows.r[i];
+    e->slot_len[s] = 0;
+    e->slot_group[s] = -1;
+    e->slot_kept[s] = keep.r[i];
+    e->slot_own[s] = 0;
+    e->slot_grows[s] = 0;
+  }
+  return EMU_OK;
+}
+
+extern "C" int emu_llm_slot_kept(EmuEngine* e, int slot) {
+  if (!e || e->n_slots < 1 || slot < 0 || slot >= e->n_slots) return -1;
+  return e->slot_kept[slot];
+}
+
+extern "C" int emu_llm_copy_prefix(EmuEngine* e, int src_slot, int dst_slot, int P, emu_stream_t stream) {
+  if (!e) return EMU_ERR_INVALID;
+  EMU_TRY(prefix_mode_ok(e));
+  const EmuConfig& c = e->cfg;
+  if (src_slot < 0 || src_slot >= e->n_slots) return e->fail(EMU_ERR_INVALID, "source slot " + std::to_string(src_slot) + " out of range");
+  if (dst_slot < 0 || dst_slot >= e->n_slots)
+    return e->fail(EMU_ERR_INVALID, "destination slot " + std::to_string(dst_slot) + " out of range");
+  if (dst_slot == src_slot) return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(src_slot) + " copied onto itself");
+  if (e->slot_group[dst_slot] >= 0) return e->fail(EMU_ERR_STATE, "destination slot " + std::to_string(dst_slot) + " is occupied");
+  const bool live = e->slot_group[src_slot] >= 0;
+  const int avail = live ? e->slot_own[src_slot] : e->slot_kept[src_slot];
+  if (!live && avail == 0) return e->fail(EMU_ERR_STATE, "source slot " + std::to_string(src_slot) + " is free and keeps nothing");
+  if (P < 1 || P > avail || P > c.llm_max_seq - 1)
+    return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(src_slot) + " holds " + std::to_string(avail) +
+                                        " positions of its own row, asked to copy " + std::to_string(P));
+  cudaStream_t st = (cudaStream_t)stream;
+  EMU_TRY(kv_prefix_copy(e->kv, (long)c.llm_layers * 2, c.llm_max_batch, e->Hl, c.llm_head_dim, c.llm_max_seq, src_slot, dst_slot, P,
+                         st));
+  slot_copy_state_kernel<<<1, 256, 0, st>>>(src_slot, live ? 0 : 1, dst_slot, P, e->d_pos, e->d_start, e->d_posoff, e->d_active,
+                                            e->d_kept_start, e->d_kept_posoff, e->kv_indir, c.llm_max_seq);
+  count_launch(2);
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "prefix copy failed");
+  e->slot_kept[dst_slot] = P;
+  return EMU_OK;
+}
+
+extern "C" int emu_llm_extend(EmuEngine* e, const int32_t* host_slots, const int32_t* host_prefix, const int32_t* host_new, int n,
+                              const void* inputs_embeds, int N, float* logits_last, emu_stream_t stream) {
+  if (!e || !host_slots || !host_prefix || !host_new || !inputs_embeds || n < 1 || N < 1) return EMU_ERR_INVALID;
+  EMU_TRY(prefix_mode_ok(e));
+  EMU_TRY(llm_ready(e));
+  const EmuConfig& c = e->cfg;
+  if (N > c.llm_max_seq) return e->fail(EMU_ERR_INVALID, "suffix of " + std::to_string(N) + " tokens exceeds llm_max_seq");
+  SlotList rows, prefix, len;
+  EMU_TRY(check_slots(e, host_slots, n, true, &rows));
+  int host_ext[3 * kLlmMaxRows];
+  int max_prefix = 0;
+  for (int i = 0; i < n; ++i) {
+    const int s = rows.r[i], p = host_prefix[i], k = host_new[i];
+    if (p < 0 || p > e->slot_kept[s])
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " keeps " + std::to_string(e->slot_kept[s]) +
+                                          " positions, asked to resume at " + std::to_string(p));
+    if (k < 1 || k > N)
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + ": " + std::to_string(k) + " new tokens, N = " + std::to_string(N));
+    if (p + k > c.llm_max_seq)
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + ": " + std::to_string(p) + " + " + std::to_string(k) +
+                                          " positions exceed llm_max_seq");
+    prefix.r[i] = p;
+    len.r[i] = p + k;
+    host_ext[i] = s;
+    host_ext[kLlmMaxRows + i] = p;
+    host_ext[2 * kLlmMaxRows + i] = k;
+    max_prefix = p > max_prefix ? p : max_prefix;
+  }
+  const int Nk = max_prefix + N < c.llm_max_seq ? max_prefix + N : c.llm_max_seq;
+  cudaStream_t st = (cudaStream_t)stream;
+  PdlScope pdl_chain(1);
+  if (cudaMemcpyAsync(e->d_ext, host_ext, sizeof(host_ext), cudaMemcpyHostToDevice, st) != cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "slot list upload failed");
+  const int* d_rows = e->d_ext;
+  const int* d_q0 = e->d_ext + kLlmMaxRows;
+  const int* d_new = e->d_ext + 2 * kLlmMaxRows;
+  EMU_TRY(prefill_stage(e, inputs_embeds, (long)n * N, st));
+  slot_resume_begin_kernel<<<1, 32, 0, st>>>(rows, prefix, e->d_kept_start, e->d_kept_posoff, e->d_join_start, e->d_join_posoff, n);
+  count_launch();
+  EMU_TRY(prefill_layers(e, n, N, 0, e->d_join_start, e->d_join_posoff, d_rows, st, d_q0, d_new, Nk));
+  slot_resume_end_kernel<<<n, 256, 0, st>>>(rows, len, e->d_join_start, e->d_join_posoff, e->d_pos, e->d_start, e->d_posoff,
+                                            e->d_active, e->kv_indir, c.llm_max_seq);
+  count_launch();
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot extend failed");
+  for (int i = 0; i < n; ++i) {
+    const int s = rows.r[i];
+    e->slot_len[s] = len.r[i];
+    e->slot_group[s] = s;
+    e->slot_kept[s] = 0;
+    e->slot_own[s] = len.r[i];
+    e->slot_grows[s] = 1;
+  }
+  return prefill_outputs(e, n, N, nullptr, logits_last, st, d_new);
+}
+
+extern "C" int emu_llm_kv_cache(EmuEngine* e, void** kv, int64_t* dims5) {
+  if (!e || !kv || !dims5) return EMU_ERR_INVALID;
+  const EmuConfig& c = e->cfg;
+  if (c.llm_layers < 1 || !e->kv) return e->fail(EMU_ERR_STATE, "engine has no LLM");
+  *kv = e->kv;
+  dims5[0] = (int64_t)c.llm_layers * 2;
+  dims5[1] = c.llm_max_batch;
+  dims5[2] = e->Hl;
+  dims5[3] = c.llm_max_seq;
+  dims5[4] = c.llm_head_dim;
+  return EMU_OK;
 }

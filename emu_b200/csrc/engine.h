@@ -92,6 +92,13 @@ struct EmuEngine {
   int* d_active = nullptr;       // [kLlmMaxRows] 1 = live slot: the decode step advances its position
   int* d_join_rows = nullptr;    // [kLlmMaxRows] cache rows of the sequences being joined
   int *d_join_start = nullptr, *d_join_posoff = nullptr;  // [kLlmMaxRows] their left-pad starts / position offsets
+  // prefix caching (include/emu_b200_prefix.h): a slot may leave but keep the first slot_kept[s] positions of its own row.
+  // slot_own[s] = how many leading positions of a live slot's table row are its own physical row: the whole length of a
+  // slot that was never re-parented (slot_grows), the join length of a beam group's first slot, 0 for a forked slot.
+  std::vector<int> slot_kept, slot_own;
+  std::vector<char> slot_grows;
+  int *d_kept_start = nullptr, *d_kept_posoff = nullptr;  // [kLlmMaxRows] a kept slot's real left-pad start / position offset
+  int* d_ext = nullptr;  // [3][kLlmMaxRows] emu_llm_extend's cache rows, prefix lengths and new-token counts
   // decode graphs keyed by the baked-in arguments (the last int: slot mode, whose step advances live rows only)
   typedef std::tuple<int, const void*, const void*, const void*, const void*, const void*, const void*, int, int> GraphKey;
   std::map<GraphKey, cudaGraphExec_t> graphs;

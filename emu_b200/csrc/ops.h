@@ -118,6 +118,12 @@ struct AttnArgs {
   // b itself; kv_rows = how many batch entries the k / v views span (0 = B)
   const int* kv_row = nullptr;
   int kv_rows = 0;
+  // [B] causal attention with a per-batch query offset (prefix caching): query i of batch b sits at key position
+  // q_off[b] + i and sees keys [kv_start[b], q_off[b] + i]; null = the uniform offset Nk - Nq.  D of 64 or 128 only.
+  const int* q_off = nullptr;
+  // [B] with q_off: batch b's real query rows (right padding beyond them), or null = Nq.  Keys at or past q_off[b] + q_len[b]
+  // were not written by the caller: no query reads them and their V rows enter P·V as zeros.
+  const int* q_len = nullptr;
 };
 int attn_prefill(const AttnArgs& a, cudaStream_t st);
 int attn_prefill_tc(const AttnArgs& a, cudaStream_t st);  // attention_tc.cu; EMU_ERR_UNSUPPORTED -> use attn_prefill's own kernel
@@ -157,6 +163,13 @@ int rope_kv_write(bf16* qkv /*[B,N,3*H*D] pair-interleaved q,k*/, int B, int N, 
                   cudaStream_t st, const int* pos_dev = nullptr /*[B] device slot of the new token (N == 1), overrides pos0*/,
                   bf16* q_out = nullptr /*decode: the rotated q goes compact [B*N, H*D] here instead of in place*/,
                   const int* kv_row = nullptr /*[B] cache row of batch b (join into chosen rows), null = b*/);
+// prefix caching (emu_llm_extend): batch b's N tokens go to cache slots q0[b] + n of row kv_row[b] (null = b), rotated at
+// position slot - pos_off[b]; only n < n_new[b] are real (right padding): the rest are neither rotated nor written
+int rope_kv_write_rows(bf16* qkv, int B, int N, int H, int D, const bf16* cos, const bf16* sin, const int* pos_off /*[B]*/,
+                       const int* q0 /*[B]*/, const int* n_new /*[B]*/, bf16* k_cache, bf16* v_cache, int t_max,
+                       const int* kv_row, cudaStream_t st);
+// positions [0, P) of cache row src -> row dst in every plane of a [outer][rows][H][t_max][D] cache (D % 8 == 0)
+int kv_prefix_copy(bf16* cache, long outer, int rows, int H, int D, int t_max, int src, int dst, int P, cudaStream_t st);
 int embed_gather(const bf16* table, const int* ids, bf16* out, int n, int dim, cudaStream_t st);
 int argmax_rows(const float* logits, int rows, int cols, int* out_idx, cudaStream_t st);
 int vit_im2col(const bf16* img_nchw, bf16* out, int B, int C, int HW, int P, int Kpad, cudaStream_t st);

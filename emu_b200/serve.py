@@ -167,14 +167,24 @@ class BatchingWorker(threading.Thread):
                 r.done.set()
 
 
-def chat_scheduler(pipeline, n_slots):
+def chat_scheduler(pipeline, n_slots, prefix_cache=False):
     from .batching import SlotScheduler
-    return SlotScheduler(pipeline.emu_model, n_slots)
+    return SlotScheduler(pipeline.emu_model, n_slots, prefix_cache=prefix_cache)
+
+
+def chat_prefix_scheduler(pipeline, n_slots):
+    return chat_scheduler(pipeline, n_slots, prefix_cache=True)
 
 
 def chat_slot_request(pipeline, inputs, knobs):
     from .batching import chat_request
     return chat_request(pipeline, inputs, **knobs)
+
+
+def chat_prefix_request(pipeline, inputs, knobs):
+    """a chat request with the keys a prefix-caching scheduler matches on"""
+    from .batching import chat_request
+    return chat_request(pipeline, inputs, prefix_keys=True, **knobs)
 
 
 def generate_scheduler_for(pipeline, n_slots):
@@ -334,8 +344,11 @@ class EmuServer:
 
     def __init__(self, chat=None, generate=None, host="0.0.0.0", port=9000, max_wait_ms=0.0, max_images_per_batch=4,
                  cache_dir=None, announce=None, max_body_bytes=256 << 20, chat_scheduler="batching",
-                 generate_scheduler="batching"):
+                 generate_scheduler="batching", chat_prefix_cache=False):
         self.cache_dir = cache_dir
+        self.chat_prefix_cache = bool(chat_prefix_cache)
+        if self.chat_prefix_cache and chat_scheduler != "continuous":
+            raise ValueError("chat_prefix_cache keeps KV-cache slots between requests: it needs chat_scheduler='continuous'")
         self.max_body_bytes = int(max_body_bytes)
         if cache_dir:
             os.makedirs(cache_dir, exist_ok=True)
@@ -349,7 +362,10 @@ class EmuServer:
         if chat_scheduler == "continuous":
             if announce is not None:
                 raise ValueError("continuous batching runs on one GPU: it cannot follow a tensor-parallel instance")
-            self.chat_workers = [ContinuousWorker(p, name="emu-chat-%d" % i) for i, p in enumerate(as_list(chat))]
+            self.chat_workers = [ContinuousWorker(p, name="emu-chat-%d" % i,
+                                                  make_scheduler=chat_prefix_scheduler if self.chat_prefix_cache else None,
+                                                  make_request=chat_prefix_request if self.chat_prefix_cache else None)
+                                 for i, p in enumerate(as_list(chat))]
         elif chat_scheduler == "batching":
             self.chat_workers = [BatchingWorker(p, "chat", chat_cap(p), max_wait_ms, announce, "emu-chat-%d" % i)
                                  for i, p in enumerate(as_list(chat))]
@@ -396,9 +412,16 @@ class EmuServer:
         self.port = self.httpd.server_address[1]
 
     # ---- the two routes; a failing request answers code -1 with the message, like the reference ----
-    def _pick(self, workers, what):
+    def _pick(self, workers, what, inputs=None):
+        """the least loaded worker; with chat prefix caching, the worker holding the longest kept prefix of the prompt"""
         if not workers:
             raise RuntimeError("%s is disabled on this server" % what)
+        if inputs is not None and self.chat_prefix_cache and len(workers) > 1:
+            from .batching import prompt_signature
+            sig = prompt_signature(inputs)
+            held = [w.scheduler.cached_prefix(sig) if w.scheduler is not None else 0 for w in workers]
+            if max(held) > 0:
+                return min((w for w, n in zip(workers, held) if n == max(held)), key=lambda w: w.load())
         return min(workers, key=lambda w: w.load())
 
     def _save(self, log_id, name, image):
@@ -414,7 +437,8 @@ class EmuServer:
             inputs = decode_prompt(fields, files)
             knobs = knobs_of(fields)
             log.info("%s: %s with hyper-parameters %s", log_id, what, knobs)
-            res["data"] = finish(log_id, self._pick(workers, what).submit(inputs, knobs, log_id))
+            res["data"] = finish(log_id, self._pick(workers, what, inputs if workers is self.chat_workers else None)
+                                 .submit(inputs, knobs, log_id))
         except Exception as ex:
             log.error("%s: %s failed, err msg: %s\n%s", log_id, what, ex, traceback.format_exc())
             res = {"code": -1, "data": str(ex)}
@@ -508,11 +532,16 @@ def main(argv=None):
     ap.add_argument("--continuous-generation", action="store_true",
                     help="image requests join and leave the denoise batch between UNet steps, in --max-images-per-batch "
                          "latent slots")
+    ap.add_argument("--prefix-cache", action="store_true",
+                    help="with --continuous-batching: a finished chat request keeps its KV-cache slot, and a later turn of the "
+                         "same conversation resumes from it and prefills only its new tokens")
     ap.add_argument("--cache-dir", type=str, default="", help="keep request pictures / results here (the reference always does)")
     ap.add_argument("--safety-checker", action="store_true",
                     help="run the built-in NSFW safety checker (the checkpoint's safety_checker.* weights) on every generated "
                          "image: flagged images come back black, with nsfw_content_detected set")
     args = ap.parse_args(argv)
+    if args.prefix_cache and not args.continuous_batching:
+        ap.error("--prefix-cache keeps KV-cache slots between requests: it needs --continuous-batching")
     logging.basicConfig(level=logging.INFO, format="%(asctime)s %(name)s %(levelname)s %(message)s")
     import torch
     import torch.distributed as dist
@@ -566,7 +595,8 @@ def main(argv=None):
                     max_images_per_batch=args.max_images_per_batch, cache_dir=args.cache_dir or None,
                     announce=make_announce() if world > 1 else None,
                     chat_scheduler="continuous" if args.continuous_batching else "batching",
-                    generate_scheduler="continuous" if args.continuous_generation else "batching")
+                    generate_scheduler="continuous" if args.continuous_generation else "batching",
+                    chat_prefix_cache=args.prefix_cache)
     log.info("serving on %s:%d (chat x%d, generate x%d)", args.host, srv.port, len(chat), len(gen))
     try:
         srv.serve_forever()
