@@ -83,6 +83,8 @@ OPS_SYMBOLS = ["emu_op_attn_decode_rows", "emu_op_rope_kv_write", "emu_op_kv_ind
 # ... and in include/emu_b200_prefix.h (prefix caching: kept slots, per-slot continuation and their kernels)
 PREFIX_SYMBOLS = ["emu_llm_leave_keep", "emu_llm_slot_kept", "emu_llm_copy_prefix", "emu_llm_extend", "emu_llm_kv_cache",
                   "emu_op_rope_kv_write_rows", "emu_op_attn_prefill_offset", "emu_op_kv_prefix_copy"]
+# ... and in include/emu_b200_chunked.h (chunked prefill: the mixed decode + prefill step and its kernels)
+CHUNKED_SYMBOLS = ["emu_llm_step", "emu_op_rope_kv_write_packed", "emu_op_attn_prefill_packed"]
 # ... and in include/emu_b200_gen_slots.h (latent slots: continuous batching for image generation)
 GEN_SLOT_SYMBOLS = ["emu_denoise_step_slots", "emu_op_denoise_prepare", "emu_op_denoise_euler"]
 # ... and in include/emu_b200_diffusion_ops.h (the diffusion kernels as stand-alone operators)
@@ -320,6 +322,34 @@ class Engine:
         hn, _ = self._host_slots(new)
         check(self.lib.emu_llm_extend(self.h, hs, hp, hn, cnt, _ptr(embeds), N, _ptr(logits), _stream()), self.h)
         return logits
+
+    # ---- chunked prefill (include/emu_b200_chunked.h) ----
+    def step(self, slots, prefix, new, final, embeds, token_ids=None, B=0, beam_src=None, logits=None, want_logits=True):
+        """one mixed step: the decode rows of slots [0, B) (token_ids [>= B] int32, beam_src [>= B] or None, logits
+        [>= B, vocab] fp32 filled in place or None) and one packed prefill segment per free slot: slots[i] continues at
+        prefix[i] with new[i] tokens of embeds [sum(new), hidden], live afterwards if final[i] else kept; returns the logits
+        of every segment's last token [n, vocab] fp32 (or None)"""
+        n = len(slots)
+        if not n == len(prefix) == len(new) == len(final):
+            raise ValueError("step: %d slots, %d prefixes, %d counts, %d final flags" % (n, len(prefix), len(new), len(final)))
+        embeds = embeds.to(torch.bfloat16).contiguous()
+        if embeds.dim() != 2 or embeds.shape[0] != sum(int(k) for k in new):
+            raise ValueError("step: embeds must be [sum(new) = %d, hidden], got %s" % (sum(int(k) for k in new), tuple(embeds.shape)))
+        c = self.cfg
+        for name, t, need, dt in (("logits", logits, B * c.llm_vocab, torch.float32), ("token_ids", token_ids, B, torch.int32),
+                                  ("beam_src", beam_src, B, torch.int32)):
+            if t is not None and (t.dtype != dt or t.numel() < need or not t.is_contiguous()):
+                raise ValueError(f"step: {name} must be a contiguous {dt} tensor of at least {need} elements, got "
+                                 f"{tuple(t.shape)} {t.dtype}")
+        last = torch.empty(n, c.llm_vocab, dtype=torch.float32, device=embeds.device) if want_logits else None
+        hs, cnt = self._host_slots(slots)
+        hp, _ = self._host_slots(prefix)
+        hn, _ = self._host_slots(new)
+        hf, _ = self._host_slots([1 if f else 0 for f in final])
+        check(self.lib.emu_llm_step(self.h, _ptr(token_ids) if B else None, _ptr(beam_src) if B else None, int(B),
+                                    _ptr(logits) if B else None, hs, hp, hn, hf, cnt, _ptr(embeds), _ptr(last), _stream()),
+              self.h)
+        return last
 
     def sample_tokens(self, logits, temperature=1.0, top_k=0, top_p=1.0, ban_id=-1, seed=0, offset=0):
         return op_sample_tokens(logits, temperature, top_k, top_p, -1 if ban_id is None else ban_id, seed, offset)
@@ -788,6 +818,44 @@ def op_attn_prefill_offset(q, k, v, scale, q_off, kv_start=None, kv_row=None, q_
     check(load().emu_op_attn_prefill_offset(_ptr(q), _ptr(k), _ptr(v), _ptr(out), B, H, Nq, Nk, D, st12, C.c_float(scale),
                                             _i32(q_off, "q_off"), _i32(q_len, "q_len"), _i32(kv_start, "kv_start"),
                                             _i32(kv_row, "kv_row"),
+                                            k.shape[0] if kv_row is not None else 0, _stream()))
+    return out
+
+
+# ---- chunked prefill kernels (include/emu_b200_chunked.h) ----
+def op_rope_kv_write_packed(qkv, H, D, rope_cos, rope_sin, k_cache, v_cache, B=0, pos=None, pos_off=None, active=None,
+                            q_out=None, seg_row=None, seg_q0=None, seg_new=None, seg_posoff=None):
+    """qkv [M, 3*H*D] packed: rows [0, B) decode rows (q -> q_out [B, H*D], k / v at slot pos[b] of row b if active[b]), then
+    the segments (seg_new[i] rows each, q in place, k / v at slots seg_q0[i] + j of row seg_row[i]); caches [rows, H, T, D]"""
+    require_cuda()
+    M = qkv.shape[0]
+    n = 0 if seg_new is None else seg_new.numel()
+    assert qkv.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
+    check(load().emu_op_rope_kv_write_packed(_ptr(qkv), M, int(B), n, H, D, _ptr(rope_cos), _ptr(rope_sin), _i32(pos, "pos"),
+                                             _i32(pos_off, "pos_off"), _i32(active, "active"), _ptr(q_out),
+                                             _i32(seg_row, "seg_row"), _i32(seg_q0, "seg_q0"), _i32(seg_new, "seg_new"),
+                                             _i32(seg_posoff, "seg_posoff"), _ptr(k_cache), _ptr(v_cache), k_cache.shape[2],
+                                             _stream()))
+
+
+def op_attn_prefill_packed(q, k, v, scale, q_row0, q_len, q_off, kv_start=None, kv_row=None, Nq=None, out=None):
+    """causal attention over packed queries: q [rows, H, D], batch b's q_len[b] queries start at row q_row0[b] and sit at key
+    positions q_off[b] + i; k / v [kv_rows, Nk, H, D] views read at batch kv_row[b] (None: b).  Writes those rows of out
+    [rows, H, D] (a new zero tensor if None) and returns it; Nq = the longest q_len (read back if None)"""
+    require_cuda()
+    rows, H, D = q.shape
+    Nk = k.shape[1]
+    if out is None:
+        out = torch.zeros(rows, H, D, dtype=torch.bfloat16, device=q.device)
+    if Nq is None:
+        Nq = int(q_len.max())
+    for t in (q, k, v, out):
+        assert t.stride(-1) == 1
+    st10 = (C.c_int64 * 10)(q.stride(0), q.stride(1), k.stride(0), k.stride(1), k.stride(2), v.stride(0), v.stride(1),
+                            v.stride(2), out.stride(0), out.stride(1))
+    check(load().emu_op_attn_prefill_packed(_ptr(q), _ptr(k), _ptr(v), _ptr(out), rows, q_len.numel(), H, int(Nq), Nk, D, st10,
+                                            C.c_float(scale), _i32(q_row0, "q_row0"), _i32(q_len, "q_len"), _i32(q_off, "q_off"),
+                                            _i32(kv_start, "kv_start"), _i32(kv_row, "kv_row"),
                                             k.shape[0] if kv_row is not None else 0, _stream()))
     return out
 

@@ -21,6 +21,14 @@ kept slot can be its first slot, else through emu_llm_copy_prefix.  Only the suf
 not go through the ViT) and ONE emu_llm_extend prefills the suffixes of all resuming newcomers.  Kept slots count as free: a
 newcomer that needs room overwrites the least recently used one, so retention never delays admission.
 
+Chunked prefill (`SlotScheduler(prefill_chunk=C)`, opt-in): a newcomer takes its slots, has its pictures encoded and its prompt
+embedded at admission as above, but is not joined: it is queued as prefilling.  While any request is prefilling, the decode of
+step 4 becomes ONE emu_llm_step (include/emu_b200_chunked.h): the live slots' next tokens and at most C prompt tokens of the
+prefilling requests (first come, first served), packed without padding into one weight pass.  A request's last chunk makes
+its first slot live (a beam request then forks, as after a join); its earlier chunks leave that slot kept at its length, owned
+by the request, so it is never a prefix source nor evicted.  No live request waits longer than one such step for a newcomer.
+A prompt with left padding (zeros in its attention_mask) still joins whole.
+
 Each step reads ONE small tensor back to the host: the finish flag of every live request (EOS of a greedy / sampled request,
 `done` of a beam search), which is what lets a request leave as soon as it is finished.
 
@@ -150,9 +158,13 @@ class SlotScheduler(_RequestQueue):
     KV-cache slots (at most the engine's llm_max_batch).  Owns the engine while it lives: nothing else may use the engine's
     LLM between steps.  Single-threaded: `submit` may be called from any thread, `step` from one."""
 
-    def __init__(self, emu_model, n_slots=None, prefix_cache=False):
+    def __init__(self, emu_model, n_slots=None, prefix_cache=False, prefill_chunk=None):
         super().__init__()
         self.prefix_cache = bool(prefix_cache)
+        self.prefill_chunk = None if prefill_chunk is None else int(prefill_chunk)
+        if self.prefill_chunk is not None and self.prefill_chunk < 1:
+            raise ValueError("prefill_chunk must be >= 1, got %d" % self.prefill_chunk)
+        self.prefilling = []                                # chunked prefill: admitted requests not yet live, in admission order
         self.kept = {}                                      # kept slot -> _Kept (prefix caching)
         self._signatures = ()                               # front-end signatures of the kept and live slots (routing)
         self._clock = 0
@@ -175,6 +187,8 @@ class SlotScheduler(_RequestQueue):
         self.owner = [None] * self.n_slots                  # slot -> request
         self.steps = 0
         self.batch_sizes = collections.deque(maxlen=1024)   # B of the recent decode steps (observability; the tests read it)
+        self.prefill_chunks = 0                             # chunked prefill: mixed steps run, and their recent sizes
+        self.mixed_sizes = collections.deque(maxlen=1024)   # ... (decode rows B, prompt tokens prefilled)
         i32 = dict(dtype=torch.int32, device=self.device)
         self.tok_buf = torch.zeros(self.n_slots, **i32)      # fixed buffers: the decode graphs are keyed by their pointers
         self.ident = torch.arange(self.n_slots, **i32)
@@ -197,7 +211,7 @@ class SlotScheduler(_RequestQueue):
         return super().submit(request)
 
     def _live(self):
-        return list(self.live)
+        return list(self.live) + list(self.prefilling)
 
     # ---- one iteration ----
     @torch.no_grad()
@@ -211,7 +225,9 @@ class SlotScheduler(_RequestQueue):
         finished = self._select()
         for r in finished:
             self._retire(r)
-        if self.live:
+        if self.prefilling:
+            self._mixed()
+        elif self.live:
             self._decode()
         self.steps += 1
         if self.prefix_cache:                               # one assignment: readers on other threads see old or new
@@ -252,6 +268,8 @@ class SlotScheduler(_RequestQueue):
                 self._fail(r, ex)
         if self.prefix_cache:
             ready = self._resume(ready)
+        if self.prefill_chunk is not None:
+            ready = self._queue_prefill(ready)
         for group in self._join_groups(ready):
             try:
                 self._join(group)
@@ -393,7 +411,12 @@ class SlotScheduler(_RequestQueue):
                 self._fail(r, ex)
                 continue
             ext.append(item)
-        if ext:
+        if ext and self.prefill_chunk is not None:          # chunked prefill: the first chunk starts at the resumed prefix
+            for r, (e, _) in ext:
+                self.prefix_hits += 1
+                self.prefix_tokens_reused += r.resume[0]
+                self._prefilling(r, e, r.resume[1])
+        elif ext:
             try:
                 self._extend(ext)
             except Exception as ex:
@@ -423,6 +446,63 @@ class SlotScheduler(_RequestQueue):
             self.prefix_hits += 1
             self.prefix_tokens_reused += r.resume[0]
         self._start(items, logits, [r.left_pad + len(r.keys) for r, _ in items])
+
+    # ---- chunked prefill ----
+    def _queue_prefill(self, ready):
+        """queue the unpadded prompts for chunked prefill; returns the left-padded ones, which join whole"""
+        joins = []
+        for item in ready:
+            r, (e, m) = item
+            if bool((m != 0).all()):
+                r.left_pad = 0
+                self._prefilling(r, e, 0)
+            else:
+                joins.append(item)
+        return joins
+
+    def _prefilling(self, r, embeds, start):
+        """r prefills embeds [1, T, hidden] into its first slot from cache position `start` on, a chunk per step"""
+        r.pf_embeds, r.pf_start, r.pf_done = embeds[0], int(start), 0
+        self.prefilling.append(r)
+
+    def _mixed(self):
+        """ONE emu_llm_step: the live slots' decode rows and up to prefill_chunk prompt tokens of the prefilling requests"""
+        segs, budget = [], self.prefill_chunk
+        for r in self.prefilling:
+            if budget == 0:
+                break
+            T = r.pf_embeds.shape[0]
+            k = min(budget, T - r.pf_done)
+            segs.append((r, r.pf_start + r.pf_done, k, r.pf_done + k == T))
+            budget -= k
+        B = max(s for r in self.live for s in r.slots) + 1 if self.live else 0
+        beams = any(r.num_beams > 1 for r in self.live)
+        embeds = torch.cat([r.pf_embeds[r.pf_done:r.pf_done + k] for r, _, k, _ in segs])
+        try:
+            last = self.engine.step([r.slots[0] for r, _, _, _ in segs], [p for _, p, _, _ in segs], [k for _, _, k, _ in segs],
+                                    [f for _, _, _, f in segs], embeds, token_ids=self.tok_buf if B else None, B=B,
+                                    beam_src=self.src_buf if beams else None, logits=self.logits_buf if B else None)
+        except Exception as ex:       # the requests in the step fail, the scheduler stays usable
+            for r in list(self.live) + [r for r, _, _, _ in segs]:
+                self._fail(r, ex)
+            return
+        self.prefill_chunks += 1
+        self.mixed_sizes.append((B, sum(k for _, _, k, _ in segs)))
+        if B:
+            self.batch_sizes.append(B)
+        for r in self.live:
+            r.logits = self.logits_buf[r.slots[0]:r.slots[0] + r.num_beams]
+        started, rows, lengths = [], [], []
+        for i, (r, p, k, final) in enumerate(segs):
+            r.pf_done += k
+            if final:
+                self.prefilling.remove(r)
+                r.pf_embeds = None
+                started.append((r, None))
+                rows.append(i)
+                lengths.append(p + k)
+        if started:
+            self._start(started, last[rows], lengths)
 
     def _keep(self, r):
         """what r's first slot keeps when it retires: the prompt and every answer token whose KV was written (beam search:
@@ -521,6 +601,9 @@ class SlotScheduler(_RequestQueue):
     def _release(self, r):
         if r in self.live:
             self.live.remove(r)
+        if r in self.prefilling:                            # a kept slot the engine holds for it is simply overwritten later
+            self.prefilling.remove(r)
+            r.pf_embeds = None
         for s in r.slots:
             if self.owner[s] is r:
                 self.owner[s] = None

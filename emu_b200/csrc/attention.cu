@@ -269,8 +269,9 @@ __device__ __forceinline__ void fa_load_tile(bf16* dst, const bf16* src, long ts
   }
 }
 
-// kRowOff: the causal offset is per batch, a.q_off[b] (prefix caching)
-template <int DP, bool kRowOff>
+// kRowOff: the causal offset is per batch, a.q_off[b] (prefix caching).  kPacked (with kRowOff): batch b's queries are the
+// rows a.q_row0[b] .. + a.q_len[b] of one packed view (chunked prefill); rows past its q_len are neither loaded nor stored.
+template <int DP, bool kRowOff, bool kPacked = false>
 __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs a) {
   constexpr int LD = FaSmem<DP>::LD;
   constexpr int KS = DP / 16;  // k-steps over the head dim
@@ -284,8 +285,10 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int q0 = qb * kFaBM;
+  const int q_n = kPacked ? a.q_len[b] : a.Nq;  // this batch's query rows
+  if (kPacked && q0 >= q_n) return;
 
-  const bf16* qp = a.q + (long)b * a.q_bs + (long)h * a.q_hs;
+  const bf16* qp = a.q + (kPacked ? (long)a.q_row0[b] * a.q_ts : (long)b * a.q_bs) + (long)h * a.q_hs;
   const int kvb = a.kv_row ? a.kv_row[b] : b;
   const bf16* kp = a.k + (long)kvb * a.k_bs + (long)h * a.k_hs;
   const bf16* vp = a.v + (long)kvb * a.v_bs + (long)h * a.v_hs;
@@ -298,7 +301,7 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
   const int nb0 = kv_lo / kFaBN;
   const int nb1 = (kv_hi + kFaBN - 1) / kFaBN;
 
-  fa_load_tile<DP>(sQ, qp, a.q_ts, q0, a.Nq, a.D);
+  fa_load_tile<DP>(sQ, qp, a.q_ts, q0, q_n, a.D);
   if (nb0 < nb1) {
     fa_load_tile<DP>(sK, kp, a.k_ts, nb0 * kFaBN, kv_n, a.D);
     fa_load_tile<DP>(sV, vp, a.v_ts, nb0 * kFaBN, kv_n, a.D);
@@ -428,11 +431,11 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
     l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
     l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
   }
-  bf16* op = a.out + (long)b * a.o_bs + (long)h * a.o_hs;
+  bf16* op = a.out + (kPacked ? (long)a.q_row0[b] * a.o_ts : (long)b * a.o_bs) + (long)h * a.o_hs;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int qi = qrow0 + r * 8;
-    if (qi >= a.Nq) continue;
+    if (qi >= q_n) continue;
     const float inv = l_run[r] > 0.f ? 1.f / l_run[r] : 0.f;
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
@@ -444,17 +447,17 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
   }
 }
 
-template <int DP, bool kRowOff = false>
+template <int DP, bool kRowOff = false, bool kPacked = false>
 static int launch_fa(const AttnArgs& a, cudaStream_t st) {
   static bool set = false;
   if (!set) {
-    if (cudaFuncSetAttribute(attn_prefill_kernel<DP, kRowOff>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    if (cudaFuncSetAttribute(attn_prefill_kernel<DP, kRowOff, kPacked>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              FaSmem<DP>::kBytes) != cudaSuccess)
       return EMU_ERR_CUDA;
     set = true;
   }
   dim3 grid((a.Nq + kFaBM - 1) / kFaBM, a.H, a.B);
-  attn_prefill_kernel<DP, kRowOff><<<grid, kFaThreads, FaSmem<DP>::kBytes, st>>>(a);
+  attn_prefill_kernel<DP, kRowOff, kPacked><<<grid, kFaThreads, FaSmem<DP>::kBytes, st>>>(a);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
@@ -476,6 +479,12 @@ int attn_prefill(const AttnArgs& a, cudaStream_t st) {
   }
   if (a.q_off) {  // prefix caching: causal, the LLaMA head dims only
     if (!a.causal || a.bias) return EMU_ERR_INVALID;
+    if (a.q_row0) {  // chunked prefill: packed queries
+      if (!a.q_len) return EMU_ERR_INVALID;
+      if (a.D == 64) return launch_fa<64, true, true>(a, st);
+      if (a.D == 128) return launch_fa<128, true, true>(a, st);
+      return EMU_ERR_INVALID;
+    }
     if (a.D == 64) return launch_fa<64, true>(a, st);
     if (a.D == 128) return launch_fa<128, true>(a, st);
     return EMU_ERR_INVALID;

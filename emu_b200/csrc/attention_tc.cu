@@ -54,6 +54,7 @@ struct AtParams {
   float scale_log2;  // scale * log2(e)
   int pdl;
   int q_hf, k_hf, v_hf;  // tensor-map coordinate order: 1 = (d, head, token, batch), 0 = (d, token, head, batch)
+  const int* q_row0;     // [B] kPacked: first row of batch b in the one-batch q / out views (AttnArgs::q_row0)
 };
 
 __device__ __forceinline__ void load_rows(void* dst, const CUtensorMap* m, uint64_t* bar, int d0, int tok, int head, int batch,
@@ -62,8 +63,10 @@ __device__ __forceinline__ void load_rows(void* dst, const CUtensorMap* m, uint6
   else tma_load_4d(dst, m, bar, d0, tok, head, batch);
 }
 
-// kRowOff: the causal offset is per batch (prefix caching), so each CTA bounds its key loop by its own batch's offset
-template <int DT, int BN, bool kRowOff>
+// kRowOff: the causal offset is per batch (prefix caching), so each CTA bounds its key loop by its own batch's offset.
+// kPacked (with kRowOff, chunked prefill): batch b's queries are rows q_row0[b] .. + q_len[b] of ONE packed q / out view; a
+// CTA past its batch's rows does nothing, and rows past them (the next batch's, or zeros past the view) are never stored.
+template <int DT, int BN, bool kRowOff, bool kPacked = false>
 __global__ void __launch_bounds__(AtCfg<DT, BN>::kThreads, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AtParams p) {
@@ -82,9 +85,10 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   const int off = kRowOff ? p.q_off[batch] : p.Nk - p.Nq;
   // keys of this batch: all Nk, or (kRowOff) up to the end of its real rows, which is all the caller wrote
   const int kv_n = kRowOff ? min(p.Nk, off + (p.q_len ? p.q_len[batch] : p.Nq)) : p.Nk;
+  const int q_n = kPacked ? p.q_len[batch] : p.Nq;  // this batch's query rows
   int kmax = kv_n - 1;  // last key any query row of this CTA may see
-  if (p.causal) kmax = min(kmax, min(q0 + 127, p.Nq - 1) + off);
-  const int nb = kmax < 0 ? 0 : kmax / BN + 1;
+  if (p.causal) kmax = min(kmax, min(q0 + 127, q_n - 1) + off);
+  const int nb = kmax < 0 || (kPacked && q0 >= q_n) ? 0 : kmax / BN + 1;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -108,7 +112,11 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
       if (p.pdl) pdl_wait();  // Q/K/V are the predecessor's output; all stores of this kernel happen after these loads
       const int kvb = p.kv_row ? p.kv_row[batch] : batch;
       mbar_expect_tx(q_full, C::kQBytes);
-      for (int c = 0; c < C::kDC; ++c) load_rows(smem + c * (128 * 128), &tmQ, q_full, c * 64, q0, head, batch, p.q_hf);
+      if (kPacked) {
+        for (int c = 0; c < C::kDC; ++c) load_rows(smem + c * (128 * 128), &tmQ, q_full, c * 64, p.q_row0[batch] + q0, head, 0, p.q_hf);
+      } else {
+        for (int c = 0; c < C::kDC; ++c) load_rows(smem + c * (128 * 128), &tmQ, q_full, c * 64, q0, head, batch, p.q_hf);
+      }
       for (int j = 0; j < nb; ++j) {
         const int s = j % kAtStages;
         const uint32_t ph = (uint32_t)(j / kAtStages) & 1u;
@@ -227,9 +235,10 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      if (qi[h] >= p.Nq) continue;
+      if (qi[h] >= q_n) continue;
       const float inv = l_run[h] > 0.f ? 1.f / l_run[h] : 0.f;
-      bf16* dst = p.out + (long)batch * p.o_bs + (long)qi[h] * p.o_ts + (long)head * p.o_hs;
+      bf16* dst = p.out + (kPacked ? (long)(p.q_row0[batch] + qi[h]) * p.o_ts : (long)batch * p.o_bs + (long)qi[h] * p.o_ts) +
+                  (long)head * p.o_hs;
 #pragma unroll
       for (int jj = 0; jj < DT / 8; ++jj) {
         const int d = 8 * jj + 2 * t;
@@ -239,18 +248,23 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   }
 }
 
-template <int DT, int BN, bool kRowOff = false>
+template <int DT, int BN, bool kRowOff = false, bool kPacked = false>
 int launch_attn_tc(const AttnArgs& a, cudaStream_t st) {
   using C = AtCfg<DT, BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(attn_tc_kernel<DT, BN, kRowOff>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem) != cudaSuccess)
+    if (cudaFuncSetAttribute(attn_tc_kernel<DT, BN, kRowOff, kPacked>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem) !=
+        cudaSuccess)
       return EMU_ERR_CUDA;
     attr_set = true;
   }
   CUtensorMap tq, tk, tv;
   AtParams p;
-  if (make_tmap_bnhd(&tq, a.q, a.D, a.Nq, a.H, a.B, a.q_ts, a.q_hs, a.q_bs, 128, &p.q_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
+  if (kPacked) {  // one batch of q_rows rows: a tile past the last row loads zeros
+    if (make_tmap_bnhd(&tq, a.q, a.D, a.q_rows, a.H, 1, a.q_ts, a.q_hs, 0, 128, &p.q_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
+  } else if (make_tmap_bnhd(&tq, a.q, a.D, a.Nq, a.H, a.B, a.q_ts, a.q_hs, a.q_bs, 128, &p.q_hf) != EMU_OK) {
+    return EMU_ERR_UNSUPPORTED;
+  }
   const int kvB = a.kv_row && a.kv_rows > 0 ? a.kv_rows : a.B;  // a row-mapped K/V map spans every cache row
   if (make_tmap_bnhd(&tk, a.k, a.D, a.Nk, a.H, kvB, a.k_ts, a.k_hs, a.k_bs, BN, &p.k_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
   if (make_tmap_bnhd(&tv, a.v, a.D, a.Nk, a.H, kvB, a.v_ts, a.v_hs, a.v_bs, BN, &p.v_hf) != EMU_OK) return EMU_ERR_UNSUPPORTED;
@@ -258,8 +272,9 @@ int launch_attn_tc(const AttnArgs& a, cudaStream_t st) {
   p.kv_start = a.kv_start; p.kv_row = a.kv_row; p.q_off = a.q_off; p.q_len = a.q_len; p.Nq = a.Nq; p.Nk = a.Nk; p.D = a.D; p.causal = a.causal;
   p.scale_log2 = a.scale * 1.4426950408889634f;
   p.pdl = g_pdl_chain;
+  p.q_row0 = a.q_row0;
   dim3 grid((a.Nq + 127) / 128, a.H, a.B);
-  return launch_kernel(attn_tc_kernel<DT, BN, kRowOff>, grid, dim3(C::kThreads), C::kSmem, st, p.pdl, tq, tk, tv, p);
+  return launch_kernel(attn_tc_kernel<DT, BN, kRowOff, kPacked>, grid, dim3(C::kThreads), C::kSmem, st, p.pdl, tq, tk, tv, p);
 }
 
 }  // namespace
@@ -275,6 +290,12 @@ int attn_prefill_tc(const AttnArgs& a, cudaStream_t st) {
   if (a.H > 65535 || a.B > 65535) return EMU_ERR_UNSUPPORTED;
   if (a.q_off) {  // prefix caching: the LLaMA head dims only
     if (!a.causal) return EMU_ERR_UNSUPPORTED;
+    if (a.q_row0) {  // chunked prefill: packed queries
+      if (!a.q_len || a.q_rows < 1) return EMU_ERR_INVALID;
+      if (a.D == 64) return launch_attn_tc<64, 128, true, true>(a, st);
+      if (a.D == 128) return launch_attn_tc<128, 64, true, true>(a, st);
+      return EMU_ERR_UNSUPPORTED;
+    }
     if (a.D == 64) return launch_attn_tc<64, 128, true>(a, st);
     if (a.D == 128) return launch_attn_tc<128, 64, true>(a, st);
     return EMU_ERR_UNSUPPORTED;

@@ -4,6 +4,7 @@
 #include "engine.h"
 #include "../../include/emu_b200_ops.h"
 #include "../../include/emu_b200_prefix.h"
+#include "../../include/emu_b200_chunked.h"
 #include "../../include/emu_b200_gen_slots.h"
 #include "../../include/emu_b200_diffusion_ops.h"
 #include "diffusion_common.h"
@@ -257,6 +258,41 @@ extern "C" int emu_op_kv_prefix_copy(void* cache, int outer, int rows, int H, in
   if (src < 0 || src >= rows || dst < 0 || dst >= rows || src == dst || P < 1 || P > t_max) return EMU_ERR_INVALID;
   count_launch();
   return kv_prefix_copy((bf16*)cache, outer, rows, H, D, t_max, src, dst, P, (cudaStream_t)s);
+}
+
+// ---- the kernels behind emu_llm_step (include/emu_b200_chunked.h) ----
+extern "C" int emu_op_rope_kv_write_packed(void* qkv, int M, int B, int n, int H, int D, const void* rope_cos, const void* rope_sin,
+                                           const int32_t* pos, const int32_t* pos_off, const int32_t* active, void* q_out,
+                                           const int32_t* seg_row, const int32_t* seg_q0, const int32_t* seg_new,
+                                           const int32_t* seg_posoff, void* k_cache, void* v_cache, int t_max, emu_stream_t s) {
+  if (!qkv || !rope_cos || !rope_sin || !k_cache || !v_cache) return EMU_ERR_INVALID;
+  if (B > 0 && (!pos || !pos_off || !active || !q_out)) return EMU_ERR_INVALID;
+  if (n > 0 && (!seg_row || !seg_q0 || !seg_new)) return EMU_ERR_INVALID;
+  if (B < 0 || B > kLlmMaxRows || n < 0 || n > kLlmMaxRows || B + n < 1 || M < B + n) return EMU_ERR_INVALID;
+  if (H < 1 || !llm_head_dim_ok(D) || t_max < 1) return EMU_ERR_INVALID;
+  count_launch();
+  return rope_kv_write_packed((bf16*)qkv, M, B, n, H, D, (const bf16*)rope_cos, (const bf16*)rope_sin, pos, pos_off, active,
+                              (bf16*)q_out, seg_row, seg_q0, seg_new, seg_posoff, (bf16*)k_cache, (bf16*)v_cache, t_max,
+                              (cudaStream_t)s);
+}
+
+extern "C" int emu_op_attn_prefill_packed(const void* q, const void* k, const void* v, void* out, int rows, int B, int H, int Nq,
+                                          int Nk, int D, const int64_t* st10, float scale, const int32_t* q_row0,
+                                          const int32_t* q_len, const int32_t* q_off, const int32_t* kv_start, const int32_t* kv_row,
+                                          int kv_rows, emu_stream_t s) {
+  if (!q || !k || !v || !out || !st10 || !q_row0 || !q_len || !q_off) return EMU_ERR_INVALID;
+  if (rows < 1 || B < 1 || B > kLlmMaxRows || H < 1 || Nq < 1 || Nk < 1 || !llm_head_dim_ok(D)) return EMU_ERR_INVALID;
+  if (kv_row && (kv_rows < 1 || kv_rows > kLlmMaxRows)) return EMU_ERR_INVALID;
+  AttnArgs a;
+  a.q = (const bf16*)q; a.k = (const bf16*)k; a.v = (const bf16*)v; a.out = (bf16*)out;
+  a.q_ts = st10[0]; a.q_hs = st10[1];
+  a.k_bs = st10[2]; a.k_ts = st10[3]; a.k_hs = st10[4];
+  a.v_bs = st10[5]; a.v_ts = st10[6]; a.v_hs = st10[7];
+  a.o_ts = st10[8]; a.o_hs = st10[9];
+  a.B = B; a.H = H; a.Nq = Nq; a.Nk = Nk; a.D = D; a.scale = scale; a.causal = 1; a.kv_start = kv_start;
+  a.kv_row = kv_row; a.kv_rows = kv_row ? kv_rows : 0; a.q_off = q_off; a.q_len = q_len; a.q_row0 = q_row0; a.q_rows = rows;
+  count_launch();
+  return attn_prefill(a, (cudaStream_t)s);
 }
 
 extern "C" int emu_op_rmsnorm(const void* x, const void* w, void* y, int rows, int cols, float eps, emu_stream_t s) {

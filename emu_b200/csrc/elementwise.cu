@@ -253,6 +253,61 @@ int rope_kv_write_rows(bf16* qkv, int B, int N, int H, int D, const bf16* cos_t,
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
+// chunked prefill (emu_llm_step): the M packed rows of a mixed step, one CTA per row.  Row m < B is the decode token of slot m
+// (cache slot pos[m], q compact to q_out, k / v only if the slot is live); the rows after it are the segments back to back,
+// row j of segment i at cache slot seg_q0[i] + j of row seg_row[i] (q in place).  Same rotation and rounding as above.
+__global__ void rope_kv_write_packed_kernel(bf16* qkv, int B, int n, int H, int D, const bf16* __restrict__ cos_t,
+                                            const bf16* __restrict__ sin_t, const int* __restrict__ pos,
+                                            const int* __restrict__ pos_off, const int* __restrict__ active, bf16* q_out,
+                                            const int* __restrict__ seg_row, const int* __restrict__ seg_q0,
+                                            const int* __restrict__ seg_new, const int* __restrict__ seg_posoff,
+                                            bf16* k_cache, bf16* v_cache, int t_max) {
+  const int m = blockIdx.x, half = D >> 1;
+  int row, slot, off;
+  bool write_kv = true;
+  if (m < B) {
+    row = m;
+    slot = pos[m];
+    off = pos_off ? pos_off[m] : 0;
+    write_kv = active[m] != 0;
+  } else {
+    int r = m - B, i = 0;
+    while (i < n && r >= seg_new[i]) r -= seg_new[i++];
+    if (i == n) return;  // past the last segment
+    row = seg_row[i];
+    slot = seg_q0[i] + r;
+    off = seg_posoff ? seg_posoff[i] : 0;
+  }
+  bf16* base = qkv + (long)m * 3 * H * D;
+  int rp = slot - off;
+  rp = rp < 0 ? 0 : rp;
+  for (int idx = threadIdx.x; idx < H * half; idx += blockDim.x) {
+    const int j = idx % half, h = idx / half;
+    const float c = __bfloat162float(cos_t[(long)rp * half + j]);
+    const float s = __bfloat162float(sin_t[(long)rp * half + j]);
+    uint32_t* qp = reinterpret_cast<uint32_t*>(base + h * D + 2 * j);
+    const uint32_t qv = *qp;
+    const float q1 = bf16_lo(qv), q2 = bf16_hi(qv);
+    uint32_t* qd = m < B ? reinterpret_cast<uint32_t*>(q_out + (long)m * H * D + h * D + 2 * j) : qp;
+    *qd = pack_bf16(round_bf16(q1 * c) + round_bf16(-q2 * s), round_bf16(q2 * c) + round_bf16(q1 * s));
+    if (!write_kv) continue;
+    const uint32_t kv = *reinterpret_cast<const uint32_t*>(base + (H + h) * D + 2 * j);
+    const float k1 = bf16_lo(kv), k2 = bf16_hi(kv);
+    const long coff = (((long)row * H + h) * t_max + slot) * D + 2 * j;
+    *reinterpret_cast<uint32_t*>(k_cache + coff) =
+        pack_bf16(round_bf16(k1 * c) + round_bf16(-k2 * s), round_bf16(k2 * c) + round_bf16(k1 * s));
+    *reinterpret_cast<uint32_t*>(v_cache + coff) = *reinterpret_cast<const uint32_t*>(base + (2 * H + h) * D + 2 * j);
+  }
+}
+
+int rope_kv_write_packed(bf16* qkv, int M, int B, int n, int H, int D, const bf16* cos_t, const bf16* sin_t, const int* pos,
+                         const int* pos_off, const int* active, bf16* q_out, const int* seg_row, const int* seg_q0,
+                         const int* seg_new, const int* seg_posoff, bf16* k_cache, bf16* v_cache, int t_max, cudaStream_t st) {
+  rope_kv_write_packed_kernel<<<M, 256, 0, st>>>(qkv, B, n, H, D, cos_t, sin_t, pos, pos_off, active, q_out, seg_row, seg_q0,
+                                                 seg_new, seg_posoff, k_cache, v_cache, t_max);
+  return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
+}
+
 // prefix caching: cache positions [0, P) of row src -> row dst in every (layer, k/v, head) plane of a [outer][rows][H][t_max][D]
 // cache.  Each plane's prefix is P*D contiguous elements, moved as 16-byte words; 4 independent words in flight per thread
 // keep enough loads outstanding for a copy that is bound by HBM bandwidth.

@@ -6,6 +6,7 @@
 //   LLaMA    : HF LlamaModel.forward as driven by Emu2/emu/emu.py:133-138 (prefill, hidden_states[-1]) and
 //              :213-229 (generate: prefill + one-token steps with KV cache)
 #include "engine.h"
+#include "../../include/emu_b200_chunked.h"
 #include "../../include/emu_b200_prefix.h"
 #include "../../include/emu_b200_slots.h"
 
@@ -181,6 +182,34 @@ __global__ void slot_resume_end_kernel(SlotList rows, SlotList len, const int* _
     active[row] = 1;
   }
   for (int t = threadIdx.x; t < t_max; t += blockDim.x) indir[(long)row * t_max + t] = row;
+}
+// emu_llm_step, after the layers: segment b's slot becomes live at len.r[b] (final.r[b]) or is kept there, as
+// slot_keep_kernel leaves a slot (its start / position offset saved, parked at pos = start = len).  One CTA per slot.
+__global__ void slot_step_end_kernel(SlotList rows, SlotList len, SlotList final_, const int* __restrict__ join_start,
+                                     const int* __restrict__ join_posoff, int* pos, int* start, int* posoff, int* active,
+                                     int* kept_start, int* kept_posoff, int* indir, int t_max) {
+  const int b = blockIdx.x, row = rows.r[b], n = len.r[b];
+  if (threadIdx.x == 0) {
+    if (final_.r[b]) {
+      start[row] = join_start[b];
+      posoff[row] = join_posoff[b];
+    } else {
+      kept_start[row] = join_start[b];
+      kept_posoff[row] = join_posoff[b];
+      start[row] = n;
+      posoff[row] = 0;
+    }
+    pos[row] = n;
+    active[row] = final_.r[b] ? 1 : 0;
+  }
+  for (int t = threadIdx.x; t < t_max; t += blockDim.x) indir[(long)row * t_max + t] = row;
+}
+// hidden rows idx[b] -> out row b (16-byte words)
+__global__ void gather_rows_kernel(const bf16* __restrict__ h, int Hd, const int* __restrict__ idx, bf16* out) {
+  const int b = blockIdx.x;
+  const uint4* src = reinterpret_cast<const uint4*>(h + (long)idx[b] * Hd);
+  uint4* dst = reinterpret_cast<uint4*>(out + (long)b * Hd);
+  for (int i = threadIdx.x; i < Hd / 8; i += blockDim.x) dst[i] = src[i];
 }
 // the hidden row of every sequence's last real token: row b * N + n_new[b] - 1 -> out row b (16-byte words)
 __global__ void gather_last_rows_kernel(const bf16* __restrict__ h, int N, int Hd, const int* __restrict__ n_new, bf16* out) {
@@ -909,8 +938,9 @@ extern "C" int emu_project(EmuEngine* e, int which, const void* x, int M, void* 
   return gemm_bf16((const bf16*)x, in, W, in, M, out, in, ep, st);
 }
 
-// prefill workspaces for M = B x N prompt tokens; the embeddings go to pf_h
-static int prefill_stage(EmuEngine* e, const void* inputs_embeds, long M, cudaStream_t st) {
+// prefill workspaces for M = B x N prompt tokens; the embeddings go to pf_h (from row `skip` on: emu_llm_step's decode rows
+// come first)
+static int prefill_stage(EmuEngine* e, const void* inputs_embeds, long M, cudaStream_t st, long skip = 0) {
   const EmuConfig& c = e->cfg;
   const int Hd = c.llm_hidden, D = c.llm_head_dim, Hl = e->Hl, Fl = e->Fl;
   EMU_TRY(e->ensure(e->pf_h, (size_t)M * Hd * 2));
@@ -919,20 +949,53 @@ static int prefill_stage(EmuEngine* e, const void* inputs_embeds, long M, cudaSt
   EMU_TRY(e->ensure(e->pf_attn, (size_t)M * Hl * D * 2));
   EMU_TRY(e->ensure(e->pf_act, (size_t)M * Fl * 2));
   if (e->tp_size > 1) EMU_TRY(e->ensure(e->pf_tmp, (size_t)M * Hd * 2));
-  if (cudaMemcpyAsync(e->pf_h.p, inputs_embeds, (size_t)M * Hd * 2, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+  if (cudaMemcpyAsync((bf16*)e->pf_h.p + skip * Hd, inputs_embeds, (size_t)(M - skip) * Hd * 2, cudaMemcpyDeviceToDevice, st) !=
+      cudaSuccess)
     return e->fail(EMU_ERR_CUDA, "embeds copy failed");
   return EMU_OK;
+}
+
+// emu_llm_step: B decode rows, then n segments packed back to back; M rows in all.  Device [n]: the segments' cache rows,
+// prefix lengths, token counts and first packed rows.
+struct MixedRows {
+  int B, n, M, max_new, Nk;
+  const int *seg_row, *seg_q0, *seg_new, *seg_row0;
+};
+
+// one layer's RoPE / KV append and attention of a mixed step: the decode rows through the row-table decode attention, written
+// straight into the first B rows of att; the segments through the packed-query prefill attention
+static int mixed_attention(EmuEngine* e, const MixedRows& m, bf16* qkv, bf16* att, bf16* kc, bf16* vc, float scale,
+                           cudaStream_t st) {
+  const EmuConfig& c = e->cfg;
+  const int D = c.llm_head_dim, Hl = e->Hl;
+  EMU_TRY(rope_kv_write_packed(qkv, m.M, m.B, m.n, Hl, D, e->rope_cos, e->rope_sin, e->d_pos, e->d_posoff, e->d_active, e->dec_q,
+                               m.seg_row, m.seg_q0, m.seg_new, e->d_join_posoff, kc, vc, c.llm_max_seq, st));
+  if (m.B > 0)
+    EMU_TRY(attn_decode(e->dec_q, kc, vc, m.B, Hl, D, c.llm_max_seq, e->d_pos, e->d_start, scale, att, e->dec_attn_ws,
+                        e->dec_counters, c.llm_max_seq, 0, st, e->kv_indir));
+  AttnArgs a;
+  a.q = qkv; a.q_ts = 3 * Hl * D; a.q_hs = D;
+  a.k = kc; a.k_bs = (long)Hl * c.llm_max_seq * D; a.k_hs = (long)c.llm_max_seq * D; a.k_ts = D;
+  a.v = vc; a.v_bs = a.k_bs; a.v_hs = a.k_hs; a.v_ts = D;
+  a.out = att; a.o_ts = Hl * D; a.o_hs = D;
+  a.B = m.n; a.H = Hl; a.Nq = m.max_new; a.Nk = m.Nk; a.D = D; a.scale = scale; a.causal = 1; a.kv_start = e->d_join_start;
+  a.kv_row = m.seg_row; a.kv_rows = c.llm_max_batch;
+  a.q_off = m.seg_q0; a.q_len = m.seg_new; a.q_row0 = m.seg_row0; a.q_rows = m.M;
+  if (m.B > 0) count_launch();  // the layer's count has one RoPE and one attention launch
+  return attn_prefill(a, st);
 }
 
 // the decoder layers over the B x N prompt tokens in pf_h: k / v of batch b go to cache row kv_row[b] (null: row b) at
 // slots [pos0, pos0 + N), rotated at position slot - posoff[b]; the attention reads keys [start[b], pos0 + N) of that row.
 // With q0 (prefix caching, device [B]): batch b's tokens go to slots [q0[b], q0[b] + n_new[b]) instead (the rest of its N
 // rows are right padding) and read keys [start[b], q0[b] + i]; Nk = the key extent of the longest row.
+// With mix (emu_llm_step): the M = mix->M packed rows of a mixed step instead, attention by mixed_attention.
 static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start, const int* posoff, const int* kv_row,
-                          cudaStream_t st, const int* q0 = nullptr, const int* n_new = nullptr, int Nk = 0) {
+                          cudaStream_t st, const int* q0 = nullptr, const int* n_new = nullptr, int Nk = 0,
+                          const MixedRows* mix = nullptr) {
   const EmuConfig& c = e->cfg;
   const int Hd = c.llm_hidden, D = c.llm_head_dim, Hl = e->Hl, Fl = e->Fl;
-  const long M = (long)B * N;
+  const long M = mix ? (long)mix->M : (long)B * N;
   bf16* h = (bf16*)e->pf_h.p;
   bf16* xn = (bf16*)e->pf_xn.p;
   bf16* qkv = (bf16*)e->pf_qkv.p;
@@ -948,22 +1011,26 @@ static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start
     GemmEpilogue ep;
     ep.C = qkv; ep.ldc = 3 * Hl * D;
     EMU_TRY(gemm_bf16(xn, Hd, L.wqkv, Hd, (int)M, 3 * Hl * D, Hd, ep, st));
-    if (q0) EMU_TRY(rope_kv_write_rows(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, q0, n_new, kc, vc, c.llm_max_seq, kv_row, st));
-    else EMU_TRY(rope_kv_write(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, pos0, kc, vc, c.llm_max_seq, st, nullptr, nullptr,
-                               kv_row));
-    AttnArgs a;
-    a.q = qkv; a.q_bs = (long)N * 3 * Hl * D; a.q_ts = 3 * Hl * D; a.q_hs = D;
-    a.k = kc; a.k_bs = (long)Hl * c.llm_max_seq * D; a.k_hs = (long)c.llm_max_seq * D; a.k_ts = D;
-    a.v = vc; a.v_bs = a.k_bs; a.v_hs = a.k_hs; a.v_ts = D;
-    a.out = att; a.o_bs = (long)N * Hl * D; a.o_ts = Hl * D; a.o_hs = D;
-    a.B = B; a.H = Hl; a.Nq = N; a.Nk = pos0 + N; a.D = D; a.scale = scale; a.causal = 1; a.kv_start = start;
-    a.kv_row = kv_row; a.kv_rows = kv_row ? c.llm_max_batch : 0;
-    if (q0) {
-      a.q_off = q0;
-      a.q_len = n_new;
-      a.Nk = Nk;
+    if (mix) {
+      EMU_TRY(mixed_attention(e, *mix, qkv, att, kc, vc, scale, st));
+    } else {
+      if (q0) EMU_TRY(rope_kv_write_rows(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, q0, n_new, kc, vc, c.llm_max_seq, kv_row, st));
+      else EMU_TRY(rope_kv_write(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, pos0, kc, vc, c.llm_max_seq, st, nullptr, nullptr,
+                                 kv_row));
+      AttnArgs a;
+      a.q = qkv; a.q_bs = (long)N * 3 * Hl * D; a.q_ts = 3 * Hl * D; a.q_hs = D;
+      a.k = kc; a.k_bs = (long)Hl * c.llm_max_seq * D; a.k_hs = (long)c.llm_max_seq * D; a.k_ts = D;
+      a.v = vc; a.v_bs = a.k_bs; a.v_hs = a.k_hs; a.v_ts = D;
+      a.out = att; a.o_bs = (long)N * Hl * D; a.o_ts = Hl * D; a.o_hs = D;
+      a.B = B; a.H = Hl; a.Nq = N; a.Nk = pos0 + N; a.D = D; a.scale = scale; a.causal = 1; a.kv_start = start;
+      a.kv_row = kv_row; a.kv_rows = kv_row ? c.llm_max_batch : 0;
+      if (q0) {
+        a.q_off = q0;
+        a.q_len = n_new;
+        a.Nk = Nk;
+      }
+      EMU_TRY(attn_prefill(a, st));
     }
-    EMU_TRY(attn_prefill(a, st));
     if (e->tp_size == 1) {
       GemmEpilogue eo;
       eo.C = h; eo.ldc = Hd; eo.residual = h; eo.ldr = Hd;
@@ -1694,5 +1761,131 @@ extern "C" int emu_llm_kv_cache(EmuEngine* e, void** kv, int64_t* dims5) {
   dims5[2] = e->Hl;
   dims5[3] = c.llm_max_seq;
   dims5[4] = c.llm_head_dim;
+  return EMU_OK;
+}
+
+// ================================================================================================
+// chunked prefill: the mixed decode + prefill step (include/emu_b200_chunked.h)
+// ================================================================================================
+extern "C" int emu_llm_step(EmuEngine* e, const int32_t* token_ids, const int32_t* beam_src_idx, int B, float* logits,
+                            const int32_t* host_slots, const int32_t* host_prefix, const int32_t* host_new, const int32_t* host_final,
+                            int n, const void* embeds, float* logits_last, emu_stream_t stream) {
+  if (!e || !host_slots || !host_prefix || !host_new || !host_final || !embeds || n < 1 || B < 0) return EMU_ERR_INVALID;
+  if (B > 0 && !token_ids) return EMU_ERR_INVALID;
+  if (B == 0 && (beam_src_idx || logits)) return EMU_ERR_INVALID;
+  EMU_TRY(prefix_mode_ok(e));
+  if (e->kv_copy) return e->fail(EMU_ERR_UNSUPPORTED, "chunked prefill with EMU_KV_COPY=1");
+  EMU_TRY(llm_ready(e));
+  const EmuConfig& c = e->cfg;
+  // the decode part: as emu_llm_decode in slot mode
+  if (B > 0) {
+    int hi = -1;
+    for (int b = 0; b < e->n_slots; ++b)
+      if (e->slot_group[b] >= 0) hi = b;
+    if (hi < 0) return e->fail(EMU_ERR_STATE, "a decode part of " + std::to_string(B) + " rows with no live slot");
+    if (B <= hi || B > e->n_slots)
+      return e->fail(EMU_ERR_INVALID, "slot mode: B = " + std::to_string(B) + " must cover the highest live slot " +
+                                          std::to_string(hi) + " and stay within " + std::to_string(e->n_slots) + " slots");
+    for (int b = 0; b < B; ++b)
+      if (e->slot_group[b] >= 0 && e->slot_len[b] + 1 > c.llm_max_seq)
+        return e->fail(EMU_ERR_INVALID, "KV cache full at slot " + std::to_string(b));
+  }
+  // the segments: as emu_llm_extend, each ending live (final) or kept
+  SlotList rows, len, fin;
+  EMU_TRY(check_slots(e, host_slots, n, true, &rows));
+  int host_idx[6 * kLlmMaxRows];  // cache rows, prefixes, token counts, first packed rows, then the rows whose logits are read
+  int total = 0, max_new = 0, max_end = 0;
+  for (int i = 0; i < n; ++i) {
+    const int s = rows.r[i], p = host_prefix[i], k = host_new[i], f = host_final[i];
+    if (f != 0 && f != 1) return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + ": final must be 0 or 1, got " + std::to_string(f));
+    if (p < 0 || p > e->slot_kept[s])
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " keeps " + std::to_string(e->slot_kept[s]) +
+                                          " positions, asked to resume at " + std::to_string(p));
+    const int room = f ? c.llm_max_seq : c.llm_max_seq - 1;  // a slot left mid-prefill is kept: at most llm_max_seq - 1
+    if (k < 1 || k > room - p)
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + ": " + std::to_string(k) + " new tokens after " + std::to_string(p) +
+                                          " must be in [1, " + std::to_string(room - p) + "] (" + (f ? "final" : "not final") + ")");
+    host_idx[i] = s;
+    host_idx[kLlmMaxRows + i] = p;
+    host_idx[2 * kLlmMaxRows + i] = k;
+    host_idx[3 * kLlmMaxRows + i] = B + total;
+    len.r[i] = p + k;
+    fin.r[i] = f;
+    total += k;
+    max_new = k > max_new ? k : max_new;
+    max_end = p + k > max_end ? p + k : max_end;
+  }
+  int n_out = 0;  // logits rows: the decode rows, then each segment's last row
+  if (logits)
+    for (int b = 0; b < B; ++b) host_idx[4 * kLlmMaxRows + n_out++] = b;
+  if (logits_last)
+    for (int i = 0; i < n; ++i) host_idx[4 * kLlmMaxRows + n_out++] = host_idx[3 * kLlmMaxRows + i] + host_new[i] - 1;
+  MixedRows mix;
+  mix.B = B; mix.n = n; mix.M = B + total; mix.max_new = max_new; mix.Nk = max_end;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Hd = c.llm_hidden;
+  EMU_TRY(e->ensure(e->step_idx, sizeof(host_idx)));
+  int* d_idx = (int*)e->step_idx.p;
+  mix.seg_row = d_idx;
+  mix.seg_q0 = d_idx + kLlmMaxRows;
+  mix.seg_new = d_idx + 2 * kLlmMaxRows;
+  mix.seg_row0 = d_idx + 3 * kLlmMaxRows;
+  PdlScope pdl_chain(1);
+  if (cudaMemcpyAsync(d_idx, host_idx, sizeof(host_idx), cudaMemcpyHostToDevice, st) != cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "slot list upload failed");
+  EMU_TRY(prefill_stage(e, embeds, mix.M, st, B));
+  if (B > 0) {
+    EMU_TRY(embed_gather(e->embed, token_ids, (bf16*)e->pf_h.p, B, Hd, st));
+    count_launch();
+  }
+  if (beam_src_idx) {
+    EMU_TRY(kv_reparent(e, beam_src_idx, B, st));
+    count_launch();
+  }
+  SlotList prefix;
+  for (int i = 0; i < n; ++i) prefix.r[i] = host_prefix[i];
+  slot_resume_begin_kernel<<<1, 32, 0, st>>>(rows, prefix, e->d_kept_start, e->d_kept_posoff, e->d_join_start, e->d_join_posoff, n);
+  count_launch();
+  EMU_TRY(prefill_layers(e, n, 0, 0, nullptr, nullptr, nullptr, st, nullptr, nullptr, 0, &mix));
+  // live decode slots advance (before the segments' slots may become live), then the segments' slots take their state
+  if (B > 0) advance_pos_kernel<<<1, 32, 0, st>>>(e->d_pos, B, nullptr, e->d_active);
+  slot_step_end_kernel<<<n, 256, 0, st>>>(rows, len, fin, e->d_join_start, e->d_join_posoff, e->d_pos, e->d_start, e->d_posoff,
+                                          e->d_active, e->d_kept_start, e->d_kept_posoff, e->kv_indir, c.llm_max_seq);
+  count_launch(B > 0 ? 2 : 1);
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "mixed step failed");
+  for (int b = 0; b < B; ++b)
+    if (e->slot_group[b] >= 0) {
+      e->slot_len[b] += 1;
+      if (e->slot_grows[b]) e->slot_own[b] += 1;
+    }
+  for (int i = 0; i < n; ++i) {
+    const int s = rows.r[i];
+    e->slot_len[s] = fin.r[i] ? len.r[i] : 0;
+    e->slot_group[s] = fin.r[i] ? s : -1;
+    e->slot_kept[s] = fin.r[i] ? 0 : len.r[i];
+    e->slot_own[s] = fin.r[i] ? len.r[i] : 0;
+    e->slot_grows[s] = fin.r[i] ? 1 : 0;
+  }
+  if (n_out == 0) return EMU_OK;
+  // logits: the rows read, one final norm and one lm_head GEMM over them, then split to the two outputs
+  EMU_TRY(e->ensure(e->pf_last, (size_t)n_out * Hd * 2));
+  EMU_TRY(e->ensure(e->step_logits, (size_t)n_out * c.llm_vocab * sizeof(float)));
+  bf16* last = (bf16*)e->pf_last.p;
+  float* lg = (float*)e->step_logits.p;
+  gather_rows_kernel<<<n_out, 128, 0, st>>>((const bf16*)e->pf_h.p, Hd, d_idx + 4 * kLlmMaxRows, last);
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "logits row gather failed");
+  EMU_TRY(rmsnorm(last, e->final_norm, last, n_out, Hd, c.llm_rms_eps, 0, st));
+  GemmEpilogue el;
+  el.out_fp32 = 1;
+  el.C = lg; el.ldc = c.llm_vocab;
+  EMU_TRY(gemm_bf16(last, Hd, e->lm_head, Hd, n_out, e->Vl, Hd, el, st));
+  count_launch(3);
+  const size_t row_bytes = (size_t)c.llm_vocab * sizeof(float);
+  const int n_dec = logits ? B : 0;
+  if (n_dec > 0 && cudaMemcpyAsync(logits, lg, n_dec * row_bytes, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "decode logits copy failed");
+  if (logits_last && cudaMemcpyAsync(logits_last, lg + (size_t)n_dec * c.llm_vocab, n * row_bytes, cudaMemcpyDeviceToDevice, st) !=
+                         cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "segment logits copy failed");
   return EMU_OK;
 }

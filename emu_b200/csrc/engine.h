@@ -85,6 +85,7 @@ struct EmuEngine {
   float *dec_logits_shard = nullptr, *dec_logits_gather = nullptr;
   // prefill workspaces (grown on demand)
   emu::DevBuf pf_h, pf_xn, pf_qkv, pf_attn, pf_act, pf_tmp, pf_last;
+  emu::DevBuf step_idx, step_logits;  // emu_llm_step: its slot lists and logits rows, and the logits of those rows
   // slot mode (continuous batching, include/emu_b200_slots.h): every cache row is a slot holding its own sequence
   int n_slots = 0;               // > 0: slot mode with this many slots
   std::vector<int> slot_len;     // host mirror of d_pos per slot (0 = free)

@@ -124,6 +124,10 @@ struct AttnArgs {
   // [B] with q_off: batch b's real query rows (right padding beyond them), or null = Nq.  Keys at or past q_off[b] + q_len[b]
   // were not written by the caller: no query reads them and their V rows enter P·V as zeros.
   const int* q_len = nullptr;
+  // [B] with q_off and q_len, packed queries (chunked prefill): batch b's queries are rows q_row0[b] .. q_row0[b] + q_len[b]
+  // - 1 of ONE [q_rows, H, D] view of q and of out (q_bs / o_bs unused); rows outside a batch are never stored.
+  const int* q_row0 = nullptr;
+  int q_rows = 0;
 };
 int attn_prefill(const AttnArgs& a, cudaStream_t st);
 int attn_prefill_tc(const AttnArgs& a, cudaStream_t st);  // attention_tc.cu; EMU_ERR_UNSUPPORTED -> use attn_prefill's own kernel
@@ -168,6 +172,11 @@ int rope_kv_write(bf16* qkv /*[B,N,3*H*D] pair-interleaved q,k*/, int B, int N, 
 int rope_kv_write_rows(bf16* qkv, int B, int N, int H, int D, const bf16* cos, const bf16* sin, const int* pos_off /*[B]*/,
                        const int* q0 /*[B]*/, const int* n_new /*[B]*/, bf16* k_cache, bf16* v_cache, int t_max,
                        const int* kv_row, cudaStream_t st);
+// chunked prefill (emu_llm_step): one launch over the M packed rows of a mixed step (include/emu_b200_chunked.h,
+// emu_op_rope_kv_write_packed); decode rows of slots with active[b] == 0 write no K/V
+int rope_kv_write_packed(bf16* qkv, int M, int B, int n, int H, int D, const bf16* cos, const bf16* sin, const int* pos,
+                         const int* pos_off, const int* active, bf16* q_out, const int* seg_row, const int* seg_q0,
+                         const int* seg_new, const int* seg_posoff, bf16* k_cache, bf16* v_cache, int t_max, cudaStream_t st);
 // positions [0, P) of cache row src -> row dst in every plane of a [outer][rows][H][t_max][D] cache (D % 8 == 0)
 int kv_prefix_copy(bf16* cache, long outer, int rows, int H, int D, int t_max, int src, int dst, int P, cudaStream_t st);
 int embed_gather(const bf16* table, const int* ids, bf16* out, int n, int dim, cudaStream_t st);

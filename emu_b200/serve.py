@@ -167,9 +167,14 @@ class BatchingWorker(threading.Thread):
                 r.done.set()
 
 
-def chat_scheduler(pipeline, n_slots, prefix_cache=False):
+def chat_scheduler(pipeline, n_slots, prefix_cache=False, prefill_chunk=None):
     from .batching import SlotScheduler
-    return SlotScheduler(pipeline.emu_model, n_slots, prefix_cache=prefix_cache)
+    return SlotScheduler(pipeline.emu_model, n_slots, prefix_cache=prefix_cache, prefill_chunk=prefill_chunk)
+
+
+def chunked_chat_scheduler(prefix_cache, prefill_chunk):
+    """a make_scheduler for chat with chunked prefill (and prefix caching if asked)"""
+    return lambda pipeline, n_slots: chat_scheduler(pipeline, n_slots, prefix_cache=prefix_cache, prefill_chunk=prefill_chunk)
 
 
 def chat_prefix_scheduler(pipeline, n_slots):
@@ -344,11 +349,17 @@ class EmuServer:
 
     def __init__(self, chat=None, generate=None, host="0.0.0.0", port=9000, max_wait_ms=0.0, max_images_per_batch=4,
                  cache_dir=None, announce=None, max_body_bytes=256 << 20, chat_scheduler="batching",
-                 generate_scheduler="batching", chat_prefix_cache=False):
+                 generate_scheduler="batching", chat_prefix_cache=False, chat_prefill_chunk=None):
         self.cache_dir = cache_dir
         self.chat_prefix_cache = bool(chat_prefix_cache)
         if self.chat_prefix_cache and chat_scheduler != "continuous":
             raise ValueError("chat_prefix_cache keeps KV-cache slots between requests: it needs chat_scheduler='continuous'")
+        self.chat_prefill_chunk = None if chat_prefill_chunk is None else int(chat_prefill_chunk)
+        if self.chat_prefill_chunk is not None and chat_scheduler != "continuous":
+            raise ValueError("chat_prefill_chunk prefills newcomers inside the live slots' decode steps: it needs "
+                             "chat_scheduler='continuous'")
+        if self.chat_prefill_chunk is not None and self.chat_prefill_chunk < 1:
+            raise ValueError("chat_prefill_chunk must be >= 1, got %d" % self.chat_prefill_chunk)
         self.max_body_bytes = int(max_body_bytes)
         if cache_dir:
             os.makedirs(cache_dir, exist_ok=True)
@@ -362,8 +373,10 @@ class EmuServer:
         if chat_scheduler == "continuous":
             if announce is not None:
                 raise ValueError("continuous batching runs on one GPU: it cannot follow a tensor-parallel instance")
-            self.chat_workers = [ContinuousWorker(p, name="emu-chat-%d" % i,
-                                                  make_scheduler=chat_prefix_scheduler if self.chat_prefix_cache else None,
+            make_scheduler = chat_prefix_scheduler if self.chat_prefix_cache else None
+            if self.chat_prefill_chunk is not None:
+                make_scheduler = chunked_chat_scheduler(self.chat_prefix_cache, self.chat_prefill_chunk)
+            self.chat_workers = [ContinuousWorker(p, name="emu-chat-%d" % i, make_scheduler=make_scheduler,
                                                   make_request=chat_prefix_request if self.chat_prefix_cache else None)
                                  for i, p in enumerate(as_list(chat))]
         elif chat_scheduler == "batching":
@@ -535,6 +548,9 @@ def main(argv=None):
     ap.add_argument("--prefix-cache", action="store_true",
                     help="with --continuous-batching: a finished chat request keeps its KV-cache slot, and a later turn of the "
                          "same conversation resumes from it and prefills only its new tokens")
+    ap.add_argument("--prefill-chunk", type=int, default=None, metavar="C",
+                    help="with --continuous-batching: a newcomer's prompt is prefilled in chunks of at most C tokens, each in "
+                         "the same weight pass as the live requests' next token, so no live request waits for a whole prompt")
     ap.add_argument("--cache-dir", type=str, default="", help="keep request pictures / results here (the reference always does)")
     ap.add_argument("--safety-checker", action="store_true",
                     help="run the built-in NSFW safety checker (the checkpoint's safety_checker.* weights) on every generated "
@@ -542,6 +558,10 @@ def main(argv=None):
     args = ap.parse_args(argv)
     if args.prefix_cache and not args.continuous_batching:
         ap.error("--prefix-cache keeps KV-cache slots between requests: it needs --continuous-batching")
+    if args.prefill_chunk is not None and not args.continuous_batching:
+        ap.error("--prefill-chunk prefills newcomers inside the live requests' decode steps: it needs --continuous-batching")
+    if args.prefill_chunk is not None and args.prefill_chunk < 1:
+        ap.error("--prefill-chunk must be >= 1")
     logging.basicConfig(level=logging.INFO, format="%(asctime)s %(name)s %(levelname)s %(message)s")
     import torch
     import torch.distributed as dist
@@ -596,7 +616,7 @@ def main(argv=None):
                     announce=make_announce() if world > 1 else None,
                     chat_scheduler="continuous" if args.continuous_batching else "batching",
                     generate_scheduler="continuous" if args.continuous_generation else "batching",
-                    chat_prefix_cache=args.prefix_cache)
+                    chat_prefix_cache=args.prefix_cache, chat_prefill_chunk=args.prefill_chunk)
     log.info("serving on %s:%d (chat x%d, generate x%d)", args.host, srv.port, len(chat), len(gen))
     try:
         srv.serve_forever()
