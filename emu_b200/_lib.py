@@ -80,9 +80,9 @@ SLOT_SYMBOLS = ["emu_llm_slots_begin", "emu_llm_join", "emu_llm_fork", "emu_llm_
 # ... and in include/emu_b200_ops.h (the decode-step kernels as stand-alone operators)
 OPS_SYMBOLS = ["emu_op_attn_decode_rows", "emu_op_rope_kv_write", "emu_op_kv_indir_update", "emu_op_kv_reorder",
                "emu_op_argmax_rows", "emu_op_attn_prefill_rows"]
-# ... and in include/emu_b200_prefix.h (prefix caching: kept slots, per-slot continuation and their kernels)
+# ... and in include/emu_b200_prefix.h (prefix caching: kept slots, per-slot continuation and the prefix copy kernel)
 PREFIX_SYMBOLS = ["emu_llm_leave_keep", "emu_llm_slot_kept", "emu_llm_copy_prefix", "emu_llm_extend", "emu_llm_kv_cache",
-                  "emu_op_rope_kv_write_rows", "emu_op_attn_prefill_offset", "emu_op_kv_prefix_copy"]
+                  "emu_op_kv_prefix_copy"]
 # ... and in include/emu_b200_chunked.h (chunked prefill: the mixed decode + prefill step and its kernels)
 CHUNKED_SYMBOLS = ["emu_llm_step", "emu_op_rope_kv_write_packed", "emu_op_attn_prefill_packed"]
 # ... and in include/emu_b200_gen_slots.h (latent slots: continuous batching for image generation)
@@ -788,37 +788,6 @@ def op_attn_prefill_rows(q, k, v, scale, causal=False, kv_start=None, kv_row=Non
     check(load().emu_op_attn_prefill_rows(_ptr(q), _ptr(k), _ptr(v), _ptr(out), B, H, Nq, Nk, D, st12, C.c_float(scale),
                                           1 if causal else 0, _i32(kv_start, "kv_start"), _i32(kv_row, "kv_row"),
                                           k.shape[0] if kv_row is not None else 0, _stream()))
-    return out
-
-
-# ---- prefix caching kernels (include/emu_b200_prefix.h) ----
-def op_rope_kv_write_rows(qkv, H, D, rope_cos, rope_sin, k_cache, v_cache, pos_off, q0, n_new, kv_row=None):
-    """qkv [B, N, 3*H*D] right-padded: batch b's first n_new[b] tokens rotated in place and their k / v written at cache slots
-    q0[b] + n of row kv_row[b]; caches [rows, H, T, D] written in place"""
-    require_cuda()
-    B, N, _ = qkv.shape
-    assert qkv.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
-    check(load().emu_op_rope_kv_write_rows(_ptr(qkv), B, N, H, D, _ptr(rope_cos), _ptr(rope_sin), _i32(pos_off, "pos_off"),
-                                           _i32(q0, "q0"), _i32(n_new, "n_new"), _i32(kv_row, "kv_row"), _ptr(k_cache),
-                                           _ptr(v_cache), k_cache.shape[2], _stream()))
-
-
-def op_attn_prefill_offset(q, k, v, scale, q_off, kv_start=None, kv_row=None, q_len=None):
-    """causal attention with a per-batch query offset: q [B,Nq,H,D], query i of batch b at key position q_off[b] + i; k/v
-    [rows,Nk,H,D] views read at batch kv_row[b] (None: b) -> [B,Nq,H,D]"""
-    require_cuda()
-    B, Nq, H, D = q.shape
-    Nk = k.shape[1]
-    out = torch.empty(B, Nq, H, D, dtype=torch.bfloat16, device=q.device)
-    st = []
-    for t in (q, k, v, out):
-        assert t.stride(3) == 1
-        st += [t.stride(0), t.stride(1), t.stride(2)]
-    st12 = (C.c_int64 * 12)(*st)
-    check(load().emu_op_attn_prefill_offset(_ptr(q), _ptr(k), _ptr(v), _ptr(out), B, H, Nq, Nk, D, st12, C.c_float(scale),
-                                            _i32(q_off, "q_off"), _i32(q_len, "q_len"), _i32(kv_start, "kv_start"),
-                                            _i32(kv_row, "kv_row"),
-                                            k.shape[0] if kv_row is not None else 0, _stream()))
     return out
 
 

@@ -269,9 +269,9 @@ __device__ __forceinline__ void fa_load_tile(bf16* dst, const bf16* src, long ts
   }
 }
 
-// kRowOff: the causal offset is per batch, a.q_off[b] (prefix caching).  kPacked (with kRowOff): batch b's queries are the
-// rows a.q_row0[b] .. + a.q_len[b] of one packed view (chunked prefill); rows past its q_len are neither loaded nor stored.
-template <int DP, bool kRowOff, bool kPacked = false>
+// kPacked (slot mode): batch b's queries are the rows a.q_row0[b] .. + a.q_len[b] of one packed view, at key positions
+// a.q_off[b] + i; rows past its q_len are neither loaded nor stored, and keys at or past a.q_off[b] + a.q_len[b] load as zeros.
+template <int DP, bool kPacked>
 __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs a) {
   constexpr int LD = FaSmem<DP>::LD;
   constexpr int KS = DP / 16;  // k-steps over the head dim
@@ -293,9 +293,9 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
   const bf16* kp = a.k + (long)kvb * a.k_bs + (long)h * a.k_hs;
   const bf16* vp = a.v + (long)kvb * a.v_bs + (long)h * a.v_hs;
   const int kv_lo = a.kv_start ? a.kv_start[b] : 0;
-  const int shift = kRowOff ? a.q_off[b] : a.Nk - a.Nq;  // causal: key j visible to query i iff j <= i + shift
-  // keys of this batch: all Nk, or (kRowOff) up to the end of its real rows; past it the tiles load as zeros
-  const int kv_n = kRowOff ? min(a.Nk, shift + (a.q_len ? a.q_len[b] : a.Nq)) : a.Nk;
+  const int shift = kPacked ? a.q_off[b] : a.Nk - a.Nq;  // causal: key j visible to query i iff j <= i + shift
+  // keys of this batch: all Nk, or (kPacked) up to the end of its rows; past it the tiles load as zeros
+  const int kv_n = kPacked ? min(a.Nk, shift + (a.q_len ? a.q_len[b] : a.Nq)) : a.Nk;
   int kv_hi = kv_n;
   if (a.causal) kv_hi = min(kv_n, q0 + kFaBM + shift);
   const int nb0 = kv_lo / kFaBN;
@@ -447,17 +447,17 @@ __global__ void __launch_bounds__(kFaThreads) attn_prefill_kernel(const AttnArgs
   }
 }
 
-template <int DP, bool kRowOff = false, bool kPacked = false>
+template <int DP, bool kPacked = false>
 static int launch_fa(const AttnArgs& a, cudaStream_t st) {
   static bool set = false;
   if (!set) {
-    if (cudaFuncSetAttribute(attn_prefill_kernel<DP, kRowOff, kPacked>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    if (cudaFuncSetAttribute(attn_prefill_kernel<DP, kPacked>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              FaSmem<DP>::kBytes) != cudaSuccess)
       return EMU_ERR_CUDA;
     set = true;
   }
   dim3 grid((a.Nq + kFaBM - 1) / kFaBM, a.H, a.B);
-  attn_prefill_kernel<DP, kRowOff, kPacked><<<grid, kFaThreads, FaSmem<DP>::kBytes, st>>>(a);
+  attn_prefill_kernel<DP, kPacked><<<grid, kFaThreads, FaSmem<DP>::kBytes, st>>>(a);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
@@ -477,14 +477,8 @@ int attn_prefill(const AttnArgs& a, cudaStream_t st) {
     const int rc = attn_prefill_tc(a, st);
     if (rc != EMU_ERR_UNSUPPORTED) return rc;
   }
-  if (a.q_off) {  // prefix caching: causal, the LLaMA head dims only
-    if (!a.causal || a.bias) return EMU_ERR_INVALID;
-    if (a.q_row0) {  // chunked prefill: packed queries
-      if (!a.q_len) return EMU_ERR_INVALID;
-      if (a.D == 64) return launch_fa<64, true, true>(a, st);
-      if (a.D == 128) return launch_fa<128, true, true>(a, st);
-      return EMU_ERR_INVALID;
-    }
+  if (a.q_off || a.q_len || a.q_row0) {  // packed queries (slot mode): causal, the LLaMA head dims only
+    if (!a.q_off || !a.q_len || !a.q_row0 || !a.causal || a.bias) return EMU_ERR_INVALID;
     if (a.D == 64) return launch_fa<64, true>(a, st);
     if (a.D == 128) return launch_fa<128, true>(a, st);
     return EMU_ERR_INVALID;

@@ -47,8 +47,8 @@ struct AtParams {
   long o_bs, o_ts, o_hs;
   const int* kv_start;
   const int* kv_row;  // [B] K/V batch coordinate of query batch b, or null = b
-  const int* q_off;   // [B] kRowOff: key position of query 0 of batch b (AttnArgs::q_off)
-  const int* q_len;   // [B] kRowOff: real query rows of batch b, or null = Nq (AttnArgs::q_len)
+  const int* q_off;   // [B] kPacked: key position of query 0 of batch b (AttnArgs::q_off)
+  const int* q_len;   // [B] kPacked: query rows of batch b (AttnArgs::q_len)
   int Nq, Nk, D;  // D = real head dim (<= DT)
   int causal;
   float scale_log2;  // scale * log2(e)
@@ -63,10 +63,10 @@ __device__ __forceinline__ void load_rows(void* dst, const CUtensorMap* m, uint6
   else tma_load_4d(dst, m, bar, d0, tok, head, batch);
 }
 
-// kRowOff: the causal offset is per batch (prefix caching), so each CTA bounds its key loop by its own batch's offset.
-// kPacked (with kRowOff, chunked prefill): batch b's queries are rows q_row0[b] .. + q_len[b] of ONE packed q / out view; a
-// CTA past its batch's rows does nothing, and rows past them (the next batch's, or zeros past the view) are never stored.
-template <int DT, int BN, bool kRowOff, bool kPacked = false>
+// kPacked (slot mode): batch b's queries are rows q_row0[b] .. + q_len[b] of ONE packed q / out view at key positions
+// q_off[b] + i, so each CTA bounds its key loop by its own batch's offset; a CTA past its batch's rows does nothing, and rows
+// past them (the next batch's, or zeros past the view) are never stored.
+template <int DT, int BN, bool kPacked>
 __global__ void __launch_bounds__(AtCfg<DT, BN>::kThreads, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AtParams p) {
@@ -82,9 +82,9 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128, head = blockIdx.y, batch = blockIdx.z;
-  const int off = kRowOff ? p.q_off[batch] : p.Nk - p.Nq;
-  // keys of this batch: all Nk, or (kRowOff) up to the end of its real rows, which is all the caller wrote
-  const int kv_n = kRowOff ? min(p.Nk, off + (p.q_len ? p.q_len[batch] : p.Nq)) : p.Nk;
+  const int off = kPacked ? p.q_off[batch] : p.Nk - p.Nq;
+  // keys of this batch: all Nk, or (kPacked) up to the end of its rows, which is all the caller wrote
+  const int kv_n = kPacked ? min(p.Nk, off + (p.q_len ? p.q_len[batch] : p.Nq)) : p.Nk;
   const int q_n = kPacked ? p.q_len[batch] : p.Nq;  // this batch's query rows
   int kmax = kv_n - 1;  // last key any query row of this CTA may see
   if (p.causal) kmax = min(kmax, min(q0 + 127, q_n - 1) + off);
@@ -206,7 +206,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
       for (int i = 0; i < DT / 2; ++i) o[i] *= corr[(i >> 1) & 1];
       // ---- O += P V_j : V is used in place as an MN-major B operand (64-wide d chunks BN*128 B apart, 8-key groups 1 KB) ----
       mbar_wait(&v_full[s], ph);
-      if (kRowOff && k0 + BN > kv_n) {
+      if (kPacked && k0 + BN > kv_n) {
         // the tile runs past this batch's last written key: zero those V rows (128 B each in every 64-wide chunk, whatever
         // the swizzle) so a stale non-finite value cannot reach O through a zero probability.  Both consumer warpgroups
         // write the same zeros; each makes its own writes visible to its wgmma before issuing it.
@@ -248,12 +248,12 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   }
 }
 
-template <int DT, int BN, bool kRowOff = false, bool kPacked = false>
+template <int DT, int BN, bool kPacked = false>
 int launch_attn_tc(const AttnArgs& a, cudaStream_t st) {
   using C = AtCfg<DT, BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(attn_tc_kernel<DT, BN, kRowOff, kPacked>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem) !=
+    if (cudaFuncSetAttribute(attn_tc_kernel<DT, BN, kPacked>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem) !=
         cudaSuccess)
       return EMU_ERR_CUDA;
     attr_set = true;
@@ -274,7 +274,7 @@ int launch_attn_tc(const AttnArgs& a, cudaStream_t st) {
   p.pdl = g_pdl_chain;
   p.q_row0 = a.q_row0;
   dim3 grid((a.Nq + 127) / 128, a.H, a.B);
-  return launch_kernel(attn_tc_kernel<DT, BN, kRowOff, kPacked>, grid, dim3(C::kThreads), C::kSmem, st, p.pdl, tq, tk, tv, p);
+  return launch_kernel(attn_tc_kernel<DT, BN, kPacked>, grid, dim3(C::kThreads), C::kSmem, st, p.pdl, tq, tk, tv, p);
 }
 
 }  // namespace
@@ -288,14 +288,9 @@ int attn_prefill_tc(const AttnArgs& a, cudaStream_t st) {
   if ((reinterpret_cast<uintptr_t>(a.q) & 15) || (reinterpret_cast<uintptr_t>(a.k) & 15) || (reinterpret_cast<uintptr_t>(a.v) & 15))
     return EMU_ERR_UNSUPPORTED;
   if (a.H > 65535 || a.B > 65535) return EMU_ERR_UNSUPPORTED;
-  if (a.q_off) {  // prefix caching: the LLaMA head dims only
+  if (a.q_off || a.q_len || a.q_row0) {  // packed queries (slot mode): the LLaMA head dims only
+    if (!a.q_off || !a.q_len || !a.q_row0 || a.q_rows < 1) return EMU_ERR_INVALID;
     if (!a.causal) return EMU_ERR_UNSUPPORTED;
-    if (a.q_row0) {  // chunked prefill: packed queries
-      if (!a.q_len || a.q_rows < 1) return EMU_ERR_INVALID;
-      if (a.D == 64) return launch_attn_tc<64, 128, true, true>(a, st);
-      if (a.D == 128) return launch_attn_tc<128, 64, true, true>(a, st);
-      return EMU_ERR_UNSUPPORTED;
-    }
     if (a.D == 64) return launch_attn_tc<64, 128, true>(a, st);
     if (a.D == 128) return launch_attn_tc<128, 64, true>(a, st);
     return EMU_ERR_UNSUPPORTED;

@@ -223,34 +223,6 @@ extern "C" int emu_op_attn_prefill_rows(const void* q, const void* k, const void
   return attn_prefill(a, (cudaStream_t)s);
 }
 
-extern "C" int emu_op_rope_kv_write_rows(void* qkv, int B, int N, int H, int D, const void* rope_cos, const void* rope_sin,
-                                         const int32_t* pos_off, const int32_t* q0, const int32_t* n_new, const int32_t* kv_row,
-                                         void* k_cache, void* v_cache, int t_max, emu_stream_t s) {
-  if (!qkv || !rope_cos || !rope_sin || !pos_off || !q0 || !n_new || !k_cache || !v_cache) return EMU_ERR_INVALID;
-  if (B < 1 || B > kLlmMaxRows || N < 1 || H < 1 || !llm_head_dim_ok(D) || t_max < 1) return EMU_ERR_INVALID;
-  count_launch();
-  return rope_kv_write_rows((bf16*)qkv, B, N, H, D, (const bf16*)rope_cos, (const bf16*)rope_sin, pos_off, q0, n_new,
-                            (bf16*)k_cache, (bf16*)v_cache, t_max, kv_row, (cudaStream_t)s);
-}
-
-extern "C" int emu_op_attn_prefill_offset(const void* q, const void* k, const void* v, void* out, int B, int H, int Nq, int Nk,
-                                          int D, const int64_t* st12, float scale, const int32_t* q_off, const int32_t* q_len,
-                                          const int32_t* kv_start, const int32_t* kv_row, int kv_rows, emu_stream_t s) {
-  if (!q || !k || !v || !out || !st12 || !q_off) return EMU_ERR_INVALID;
-  if (B < 1 || B > kLlmMaxRows || H < 1 || Nq < 1 || Nk < 1 || !llm_head_dim_ok(D)) return EMU_ERR_INVALID;
-  if (kv_row && (kv_rows < 1 || kv_rows > kLlmMaxRows)) return EMU_ERR_INVALID;
-  AttnArgs a;
-  a.q = (const bf16*)q; a.k = (const bf16*)k; a.v = (const bf16*)v; a.out = (bf16*)out;
-  a.q_bs = st12[0]; a.q_ts = st12[1]; a.q_hs = st12[2];
-  a.k_bs = st12[3]; a.k_ts = st12[4]; a.k_hs = st12[5];
-  a.v_bs = st12[6]; a.v_ts = st12[7]; a.v_hs = st12[8];
-  a.o_bs = st12[9]; a.o_ts = st12[10]; a.o_hs = st12[11];
-  a.B = B; a.H = H; a.Nq = Nq; a.Nk = Nk; a.D = D; a.scale = scale; a.causal = 1; a.kv_start = kv_start;
-  a.kv_row = kv_row; a.kv_rows = kv_row ? kv_rows : 0; a.q_off = q_off; a.q_len = q_len;
-  count_launch();
-  return attn_prefill(a, (cudaStream_t)s);
-}
-
 extern "C" int emu_op_kv_prefix_copy(void* cache, int outer, int rows, int H, int D, int t_max, int src, int dst, int P,
                                      emu_stream_t s) {
   if (!cache || (reinterpret_cast<uintptr_t>(cache) & 15)) return EMU_ERR_INVALID;  // moved as 16-byte words

@@ -195,13 +195,10 @@ int layernorm(const bf16* x, const bf16* w, const bf16* b, const bf16* residual,
 // prefill: RoPE on q (in place) and k, append k/v to the cache.  q/k head dims are pair-interleaved
 // (element 2j = original j, 2j+1 = original j + D/2) by the weight packer, so a rotation pair is one 4-byte word.
 // ----------------------------------------------------------------------------------------------
-// kRows (prefix caching, emu_llm_extend): batch b's tokens sit at cache slots pos_dev[b] + n and only the first n_dev[b] of
-// its N tokens are real (right padding); the padding is neither rotated nor written
-template <bool kRows>
 __global__ void rope_kv_write_kernel(bf16* qkv, int B, int N, int H, int D, const bf16* __restrict__ cos_t,
                                      const bf16* __restrict__ sin_t, const int* pos_off, int pos0, bf16* k_cache,
                                      bf16* v_cache, int t_max, const int* __restrict__ pos_dev, bf16* q_out,
-                                     const int* __restrict__ kv_row, const int* __restrict__ n_dev) {
+                                     const int* __restrict__ kv_row) {
   const int half = D >> 1;
   const long total = (long)B * N * H * half;
   for (long idx = blockIdx.x * (long)blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
@@ -209,7 +206,6 @@ __global__ void rope_kv_write_kernel(bf16* qkv, int B, int N, int H, int D, cons
     const int h = (idx / half) % H;
     const int n = (idx / ((long)half * H)) % N;
     const int b = idx / ((long)half * H * N);
-    if (kRows && n >= n_dev[b]) continue;
     bf16* base = qkv + ((long)b * N + n) * 3 * H * D;
     // CUDA-graphed decode: the cache slot of every row's new token lives on the device (rows differ in slot mode)
     const int p0 = pos_dev ? pos_dev[b] : pos0;
@@ -238,22 +234,12 @@ int rope_kv_write(bf16* qkv, int B, int N, int H, int D, const bf16* cos_t, cons
                   const int* kv_row) {
   const long total = (long)B * N * H * (D / 2);
   const int grid = (int)((total + 255) / 256 < 4 * kNumSMs ? (total + 255) / 256 : 4 * kNumSMs);
-  rope_kv_write_kernel<false><<<grid, 256, 0, st>>>(qkv, B, N, H, D, cos_t, sin_t, pos_off, pos0, k_cache, v_cache, t_max, pos_dev,
-                                                    q_out, kv_row, nullptr);
+  rope_kv_write_kernel<<<grid, 256, 0, st>>>(qkv, B, N, H, D, cos_t, sin_t, pos_off, pos0, k_cache, v_cache, t_max, pos_dev, q_out,
+                                             kv_row);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 
-int rope_kv_write_rows(bf16* qkv, int B, int N, int H, int D, const bf16* cos_t, const bf16* sin_t, const int* pos_off,
-                       const int* q0, const int* n_new, bf16* k_cache, bf16* v_cache, int t_max, const int* kv_row,
-                       cudaStream_t st) {
-  const long total = (long)B * N * H * (D / 2);
-  const int grid = (int)((total + 255) / 256 < 4 * kNumSMs ? (total + 255) / 256 : 4 * kNumSMs);
-  rope_kv_write_kernel<true><<<grid, 256, 0, st>>>(qkv, B, N, H, D, cos_t, sin_t, pos_off, 0, k_cache, v_cache, t_max, q0, nullptr,
-                                                   kv_row, n_new);
-  return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
-}
-
-// chunked prefill (emu_llm_step): the M packed rows of a mixed step, one CTA per row.  Row m < B is the decode token of slot m
+// slot mode (emu_llm_join, emu_llm_extend, emu_llm_step): the M packed rows of a mixed step, one CTA per row.  Row m < B is the decode token of slot m
 // (cache slot pos[m], q compact to q_out, k / v only if the slot is live); the rows after it are the segments back to back,
 // row j of segment i at cache slot seg_q0[i] + j of row seg_row[i] (q in place).  Same rotation and rounding as above.
 __global__ void rope_kv_write_packed_kernel(bf16* qkv, int B, int n, int H, int D, const bf16* __restrict__ cos_t,
@@ -303,8 +289,11 @@ __global__ void rope_kv_write_packed_kernel(bf16* qkv, int B, int n, int H, int 
 int rope_kv_write_packed(bf16* qkv, int M, int B, int n, int H, int D, const bf16* cos_t, const bf16* sin_t, const int* pos,
                          const int* pos_off, const int* active, bf16* q_out, const int* seg_row, const int* seg_q0,
                          const int* seg_new, const int* seg_posoff, bf16* k_cache, bf16* v_cache, int t_max, cudaStream_t st) {
-  rope_kv_write_packed_kernel<<<M, 256, 0, st>>>(qkv, B, n, H, D, cos_t, sin_t, pos, pos_off, active, q_out, seg_row, seg_q0,
-                                                 seg_new, seg_posoff, k_cache, v_cache, t_max);
+  // one CTA per row with a thread for each of its H * D / 2 rotation pairs (up to 1024): a short prefill has few rows, and a
+  // CTA that loops over its row would leave most of the GPU idle
+  const int pairs = H * (D / 2), threads = pairs < 1024 ? (pairs + 31) / 32 * 32 : 1024;
+  rope_kv_write_packed_kernel<<<M, threads, 0, st>>>(qkv, B, n, H, D, cos_t, sin_t, pos, pos_off, active, q_out, seg_row, seg_q0,
+                                                     seg_new, seg_posoff, k_cache, v_cache, t_max);
   return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
 }
 

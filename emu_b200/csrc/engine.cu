@@ -98,23 +98,11 @@ __global__ void mask_start_kernel(const int* __restrict__ mask, int N, int* star
     posoff[b] = hf ? base + s : 0;
   }
 }
-// slot mode: the per-row state of a set of slots.  A join sets length `len`, the left-pad start / position offset from the
-// join-local arrays and marks the slot live; a leave (len 0, no arrays) zeroes and frees it.  Either way the slot's row of
-// the re-parenting table becomes identity (it may have belonged to a beam group).  One CTA per slot.
+// slot mode: a host list of slots (or of per-slot values) passed to a kernel by value.  A kernel that frees a slot or makes
+// it live resets the slot's row of the re-parenting table to identity (it may have belonged to a beam group).
 struct SlotList {
   int r[kLlmMaxRows];
 };
-__global__ void slot_set_kernel(SlotList rows, const int* __restrict__ src_start, const int* __restrict__ src_posoff, int len,
-                                int* pos, int* start, int* posoff, int* active, int* indir, int t_max) {
-  const int b = blockIdx.x, row = rows.r[b];
-  if (threadIdx.x == 0) {
-    pos[row] = len;
-    start[row] = src_start ? src_start[b] : 0;
-    posoff[row] = src_posoff ? src_posoff[b] : 0;
-    active[row] = len > 0 ? 1 : 0;
-  }
-  for (int t = threadIdx.x; t < t_max; t += blockDim.x) indir[(long)row * t_max + t] = row;
-}
 // slot mode: the slots dst continue slot src's sequence — its table row up to its length (identity beyond: a slot's own
 // new tokens are in its own row), its length, start and position offset.  One CTA per destination.
 __global__ void slot_fork_kernel(int src, SlotList dst, int* pos, int* start, int* posoff, int* active, int* indir, int t_max) {
@@ -129,7 +117,7 @@ __global__ void slot_fork_kernel(int src, SlotList dst, int* pos, int* start, in
     active[row] = 1;
   }
 }
-// prefix caching: slots leave keeping their first keep.r[b] cache positions (0 = a plain leave, as slot_set_kernel).  The real
+// slots leave keeping their first keep.r[b] cache positions (0 = a plain leave, prefix caching otherwise).  The real
 // left-pad start / position offset move to the kept arrays, and the slot is parked at pos = start = keep: the decode step
 // computes every free slot below B and appends its junk token at pos, which then lands at position keep, past the kept
 // prefix (a resume overwrites it before anything reads it), and its attention reads that one key.
@@ -160,8 +148,8 @@ __global__ void slot_copy_state_kernel(int src, int src_kept, int dst, int P, in
   }
   for (int t = threadIdx.x; t < t_max; t += blockDim.x) indir[(long)dst * t_max + t] = dst;
 }
-// emu_llm_extend, before the layers: the join-local start / position offset of every resuming slot (its kept ones; zero for
-// a slot that starts from nothing).  One thread per slot.
+// slot-mode prefill, before the layers: the join-local start / position offset of every segment's slot (its kept ones; zero
+// for a slot that starts from nothing).  One thread per slot.
 __global__ void slot_resume_begin_kernel(SlotList rows, SlotList prefix, const int* __restrict__ kept_start,
                                          const int* __restrict__ kept_posoff, int* join_start, int* join_posoff, int n) {
   const int b = threadIdx.x;
@@ -170,21 +158,8 @@ __global__ void slot_resume_begin_kernel(SlotList rows, SlotList prefix, const i
   join_start[b] = p > 0 ? kept_start[row] : 0;
   join_posoff[b] = p > 0 ? kept_posoff[row] : 0;
 }
-// ... after the layers: the slots are live at length len.r[b].  One CTA per slot.
-__global__ void slot_resume_end_kernel(SlotList rows, SlotList len, const int* __restrict__ join_start,
-                                       const int* __restrict__ join_posoff, int* pos, int* start, int* posoff, int* active,
-                                       int* indir, int t_max) {
-  const int b = blockIdx.x, row = rows.r[b];
-  if (threadIdx.x == 0) {
-    pos[row] = len.r[b];
-    start[row] = join_start[b];
-    posoff[row] = join_posoff[b];
-    active[row] = 1;
-  }
-  for (int t = threadIdx.x; t < t_max; t += blockDim.x) indir[(long)row * t_max + t] = row;
-}
-// emu_llm_step, after the layers: segment b's slot becomes live at len.r[b] (final.r[b]) or is kept there, as
-// slot_keep_kernel leaves a slot (its start / position offset saved, parked at pos = start = len).  One CTA per slot.
+// ... after the layers: segment b's slot becomes live at len.r[b] (final.r[b]) or is kept there, as slot_keep_kernel
+// leaves a slot (its start / position offset saved, parked at pos = start = len).  One CTA per slot.
 __global__ void slot_step_end_kernel(SlotList rows, SlotList len, SlotList final_, const int* __restrict__ join_start,
                                      const int* __restrict__ join_posoff, int* pos, int* start, int* posoff, int* active,
                                      int* kept_start, int* kept_posoff, int* indir, int t_max) {
@@ -208,13 +183,6 @@ __global__ void slot_step_end_kernel(SlotList rows, SlotList len, SlotList final
 __global__ void gather_rows_kernel(const bf16* __restrict__ h, int Hd, const int* __restrict__ idx, bf16* out) {
   const int b = blockIdx.x;
   const uint4* src = reinterpret_cast<const uint4*>(h + (long)idx[b] * Hd);
-  uint4* dst = reinterpret_cast<uint4*>(out + (long)b * Hd);
-  for (int i = threadIdx.x; i < Hd / 8; i += blockDim.x) dst[i] = src[i];
-}
-// the hidden row of every sequence's last real token: row b * N + n_new[b] - 1 -> out row b (16-byte words)
-__global__ void gather_last_rows_kernel(const bf16* __restrict__ h, int N, int Hd, const int* __restrict__ n_new, bf16* out) {
-  const int b = blockIdx.x;
-  const uint4* src = reinterpret_cast<const uint4*>(h + ((long)b * N + n_new[b] - 1) * Hd);
   uint4* dst = reinterpret_cast<uint4*>(out + (long)b * Hd);
   for (int i = threadIdx.x; i < Hd / 8; i += blockDim.x) dst[i] = src[i];
 }
@@ -420,13 +388,11 @@ extern "C" int emu_engine_create(const EmuConfig* cfg, int tp_rank, int tp_size,
     e->d_pos = (int*)e->dmalloc(3 * kLlmMaxRows * sizeof(int));
     e->d_start = e->d_pos + kLlmMaxRows;
     e->d_posoff = e->d_pos + 2 * kLlmMaxRows;
-    e->d_active = (int*)e->dmalloc(4 * kLlmMaxRows * sizeof(int));
-    e->d_join_rows = e->d_active + kLlmMaxRows;
-    e->d_join_start = e->d_active + 2 * kLlmMaxRows;
-    e->d_join_posoff = e->d_active + 3 * kLlmMaxRows;
-    e->d_kept_start = (int*)e->dmalloc(5 * kLlmMaxRows * sizeof(int));
+    e->d_active = (int*)e->dmalloc(3 * kLlmMaxRows * sizeof(int));
+    e->d_join_start = e->d_active + kLlmMaxRows;
+    e->d_join_posoff = e->d_active + 2 * kLlmMaxRows;
+    e->d_kept_start = (int*)e->dmalloc(2 * kLlmMaxRows * sizeof(int));
     e->d_kept_posoff = e->d_kept_start + kLlmMaxRows;
-    e->d_ext = e->d_kept_start + 2 * kLlmMaxRows;
     if (c.llm_max_batch > 8) {  // wide decode (more than 8 cache rows: the C4 workload, 4 prompts x 5 beams) runs on the GEMM path
       e->dec_xn = (bf16*)e->dmalloc((size_t)c.llm_max_batch * c.llm_hidden * 2);
       e->dec_qkv = (bf16*)e->dmalloc((size_t)c.llm_max_batch * 3 * e->Hl * c.llm_head_dim * 2);
@@ -465,8 +431,8 @@ extern "C" int emu_engine_create(const EmuConfig* cfg, int tp_rank, int tp_size,
     rope_table_kernel<<<2 * kNumSMs, 256>>>(e->rope_cos, e->rope_sin, max_pos, half, c.llm_rope_theta);
     cudaMemset(e->dec_counters, 0, (size_t)Bm * e->Hl * sizeof(int));
     cudaMemset(e->d_pos, 0, 3 * kLlmMaxRows * sizeof(int));
-    cudaMemset(e->d_active, 0, 4 * kLlmMaxRows * sizeof(int));
-    cudaMemset(e->d_kept_start, 0, 5 * kLlmMaxRows * sizeof(int));
+    cudaMemset(e->d_active, 0, 3 * kLlmMaxRows * sizeof(int));
+    cudaMemset(e->d_kept_start, 0, 2 * kLlmMaxRows * sizeof(int));
     kv_indir_identity(e->kv_indir, Bm, c.llm_max_seq, 0);
   }
   if (c.vit_layers > 0) {
@@ -856,11 +822,7 @@ extern "C" int emu_llm_reset(EmuEngine* e, emu_stream_t s) {
   e->cur_len = 0;
   e->cache_B = 0;
   e->n_slots = 0;
-  e->slot_len.clear();
-  e->slot_group.clear();
-  e->slot_kept.clear();
-  e->slot_own.clear();
-  e->slot_grows.clear();
+  e->slots.clear();
   if (e->d_pos && cudaMemsetAsync(e->d_pos, 0, 3 * kLlmMaxRows * sizeof(int), (cudaStream_t)s) != cudaSuccess) return EMU_ERR_CUDA;
   if (e->kv_indir && e->kv_indir_dirty) {
     EMU_TRY(kv_indir_identity(e->kv_indir, e->cfg.llm_max_batch, e->cfg.llm_max_seq, (cudaStream_t)s));
@@ -893,7 +855,7 @@ static int kv_reparent(EmuEngine* e, const int32_t* src_idx, int B, cudaStream_t
   e->kv_indir_dirty = true;
   if (e->n_slots > 0) {  // slots differ in length: every row copies its own, read from the device positions
     int n_tok = 0;
-    for (int b = 0; b < B; ++b) n_tok = e->slot_len[b] > n_tok ? e->slot_len[b] : n_tok;
+    for (int b = 0; b < B; ++b) n_tok = e->slots[b].len > n_tok ? e->slots[b].len : n_tok;
     return kv_indir_update(e->kv_indir, src_idx, B, c.llm_max_seq, n_tok, st, e->d_pos);
   }
   return kv_indir_update(e->kv_indir, src_idx, B, c.llm_max_seq, e->cur_len, st);
@@ -938,9 +900,8 @@ extern "C" int emu_project(EmuEngine* e, int which, const void* x, int M, void* 
   return gemm_bf16((const bf16*)x, in, W, in, M, out, in, ep, st);
 }
 
-// prefill workspaces for M = B x N prompt tokens; the embeddings go to pf_h (from row `skip` on: emu_llm_step's decode rows
-// come first)
-static int prefill_stage(EmuEngine* e, const void* inputs_embeds, long M, cudaStream_t st, long skip = 0) {
+// prefill workspaces for M prompt tokens; the embeddings go to pf_h (null: the caller stages them)
+static int prefill_stage(EmuEngine* e, const void* inputs_embeds, long M, cudaStream_t st) {
   const EmuConfig& c = e->cfg;
   const int Hd = c.llm_hidden, D = c.llm_head_dim, Hl = e->Hl, Fl = e->Fl;
   EMU_TRY(e->ensure(e->pf_h, (size_t)M * Hd * 2));
@@ -949,20 +910,19 @@ static int prefill_stage(EmuEngine* e, const void* inputs_embeds, long M, cudaSt
   EMU_TRY(e->ensure(e->pf_attn, (size_t)M * Hl * D * 2));
   EMU_TRY(e->ensure(e->pf_act, (size_t)M * Fl * 2));
   if (e->tp_size > 1) EMU_TRY(e->ensure(e->pf_tmp, (size_t)M * Hd * 2));
-  if (cudaMemcpyAsync((bf16*)e->pf_h.p + skip * Hd, inputs_embeds, (size_t)(M - skip) * Hd * 2, cudaMemcpyDeviceToDevice, st) !=
-      cudaSuccess)
+  if (inputs_embeds && cudaMemcpyAsync(e->pf_h.p, inputs_embeds, (size_t)M * Hd * 2, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
     return e->fail(EMU_ERR_CUDA, "embeds copy failed");
   return EMU_OK;
 }
 
-// emu_llm_step: B decode rows, then n segments packed back to back; M rows in all.  Device [n]: the segments' cache rows,
-// prefix lengths, token counts and first packed rows.
+// slot-mode prefill: B decode rows, then n segments packed back to back; M rows in all.  Device [n]: the segments' cache
+// rows, prefix lengths, token counts and first packed rows.
 struct MixedRows {
   int B, n, M, max_new, Nk;
   const int *seg_row, *seg_q0, *seg_new, *seg_row0;
 };
 
-// one layer's RoPE / KV append and attention of a mixed step: the decode rows through the row-table decode attention, written
+// one layer's RoPE / KV append and attention of slot-mode rows: the decode rows through the row-table decode attention, written
 // straight into the first B rows of att; the segments through the packed-query prefill attention
 static int mixed_attention(EmuEngine* e, const MixedRows& m, bf16* qkv, bf16* att, bf16* kc, bf16* vc, float scale,
                            cudaStream_t st) {
@@ -985,13 +945,10 @@ static int mixed_attention(EmuEngine* e, const MixedRows& m, bf16* qkv, bf16* at
   return attn_prefill(a, st);
 }
 
-// the decoder layers over the B x N prompt tokens in pf_h: k / v of batch b go to cache row kv_row[b] (null: row b) at
-// slots [pos0, pos0 + N), rotated at position slot - posoff[b]; the attention reads keys [start[b], pos0 + N) of that row.
-// With q0 (prefix caching, device [B]): batch b's tokens go to slots [q0[b], q0[b] + n_new[b]) instead (the rest of its N
-// rows are right padding) and read keys [start[b], q0[b] + i]; Nk = the key extent of the longest row.
-// With mix (emu_llm_step): the M = mix->M packed rows of a mixed step instead, attention by mixed_attention.
-static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start, const int* posoff, const int* kv_row,
-                          cudaStream_t st, const int* q0 = nullptr, const int* n_new = nullptr, int Nk = 0,
+// the decoder layers over the B x N prompt tokens in pf_h: k / v of batch b go to cache row b at slots [pos0, pos0 + N),
+// rotated at position slot - posoff[b]; the attention reads keys [start[b], pos0 + N) of that row.
+// With mix (slot mode): the M = mix->M packed rows of mix instead, attention by mixed_attention.
+static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start, const int* posoff, cudaStream_t st,
                           const MixedRows* mix = nullptr) {
   const EmuConfig& c = e->cfg;
   const int Hd = c.llm_hidden, D = c.llm_head_dim, Hl = e->Hl, Fl = e->Fl;
@@ -1014,21 +971,13 @@ static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start
     if (mix) {
       EMU_TRY(mixed_attention(e, *mix, qkv, att, kc, vc, scale, st));
     } else {
-      if (q0) EMU_TRY(rope_kv_write_rows(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, q0, n_new, kc, vc, c.llm_max_seq, kv_row, st));
-      else EMU_TRY(rope_kv_write(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, pos0, kc, vc, c.llm_max_seq, st, nullptr, nullptr,
-                                 kv_row));
+      EMU_TRY(rope_kv_write(qkv, B, N, Hl, D, e->rope_cos, e->rope_sin, posoff, pos0, kc, vc, c.llm_max_seq, st));
       AttnArgs a;
       a.q = qkv; a.q_bs = (long)N * 3 * Hl * D; a.q_ts = 3 * Hl * D; a.q_hs = D;
       a.k = kc; a.k_bs = (long)Hl * c.llm_max_seq * D; a.k_hs = (long)c.llm_max_seq * D; a.k_ts = D;
       a.v = vc; a.v_bs = a.k_bs; a.v_hs = a.k_hs; a.v_ts = D;
       a.out = att; a.o_bs = (long)N * Hl * D; a.o_ts = Hl * D; a.o_hs = D;
       a.B = B; a.H = Hl; a.Nq = N; a.Nk = pos0 + N; a.D = D; a.scale = scale; a.causal = 1; a.kv_start = start;
-      a.kv_row = kv_row; a.kv_rows = kv_row ? c.llm_max_batch : 0;
-      if (q0) {
-        a.q_off = q0;
-        a.q_len = n_new;
-        a.Nk = Nk;
-      }
       EMU_TRY(attn_prefill(a, st));
     }
     if (e->tp_size == 1) {
@@ -1064,19 +1013,19 @@ static int prefill_layers(EmuEngine* e, int B, int N, int pos0, const int* start
   return EMU_OK;
 }
 
-// final norm of every prompt token (last_hidden) and the logits of every sequence's last position (logits_last).  With n_new
-// (device [B], right-padded rows): the logits of row b's token n_new[b] - 1, gathered to pf_last first.
+// final norm of every prompt token (last_hidden) and the logits of every sequence's last position (logits_last).  With rows
+// (device [B], slot mode): the logits of hidden rows rows[0 .. B) of pf_h instead, gathered to pf_last first (N = 1).
 static int prefill_outputs(EmuEngine* e, int B, int N, void* last_hidden, float* logits_last, cudaStream_t st,
-                           const int* n_new = nullptr) {
+                           const int* rows = nullptr) {
   const EmuConfig& c = e->cfg;
   const int Hd = c.llm_hidden;
   const long M = (long)B * N;
   bf16* h = (bf16*)e->pf_h.p;
-  if (n_new && logits_last) {
+  if (rows && logits_last) {
     EMU_TRY(e->ensure(e->pf_last, (size_t)B * Hd * 2));
-    gather_last_rows_kernel<<<B, 128, 0, st>>>(h, N, Hd, n_new, (bf16*)e->pf_last.p);
+    gather_rows_kernel<<<B, 128, 0, st>>>(h, Hd, rows, (bf16*)e->pf_last.p);
     count_launch();
-    if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "last-token gather failed");
+    if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "logits row gather failed");
     h = (bf16*)e->pf_last.p;
     N = 1;
   }
@@ -1088,7 +1037,7 @@ static int prefill_outputs(EmuEngine* e, int B, int N, void* last_hidden, float*
     // more rows than the skinny GEMV takes: final norm of the last position of every sequence, then the wgmma GEMM
     EMU_TRY(e->ensure(e->pf_last, (size_t)B * Hd * 2));
     bf16* last = (bf16*)e->pf_last.p;
-    if (!n_new && cudaMemcpy2DAsync(last, (size_t)Hd * 2, h + (size_t)(N - 1) * Hd, (size_t)N * Hd * 2, (size_t)Hd * 2, B,
+    if (!rows && cudaMemcpy2DAsync(last, (size_t)Hd * 2, h + (size_t)(N - 1) * Hd, (size_t)N * Hd * 2, (size_t)Hd * 2, B,
                                     cudaMemcpyDeviceToDevice, st) != cudaSuccess)
       return e->fail(EMU_ERR_CUDA, "last-position gather failed");
     EMU_TRY(rmsnorm(last, e->final_norm, last, B, Hd, c.llm_rms_eps, 0, st));
@@ -1145,7 +1094,7 @@ extern "C" int emu_llm_prefill(EmuEngine* e, const void* inputs_embeds, const in
     count_launch();
     e->cache_B = B;
   }
-  EMU_TRY(prefill_layers(e, B, N, pos0, e->d_start, e->d_posoff, nullptr, st));
+  EMU_TRY(prefill_layers(e, B, N, pos0, e->d_start, e->d_posoff, st));
   e->cur_len = pos0 + N;
   set_int_kernel<<<1, 32, 0, st>>>(e->d_pos, kLlmMaxRows, e->cur_len);  // slot of the next token
   count_launch();
@@ -1403,6 +1352,22 @@ static int decode_step_body(EmuEngine* e, const int32_t* token_ids, const void* 
   return EMU_OK;
 }
 
+// slot mode's decode rows 0 .. B - 1: B covers the highest live slot and stays within the slots, and every live slot among
+// them has room for one more token
+static int check_decode_rows(EmuEngine* e, int B, const std::string& none_live) {
+  int hi = -1;
+  for (int b = 0; b < e->n_slots; ++b)
+    if (e->slots[b].live()) hi = b;
+  if (hi < 0) return e->fail(EMU_ERR_STATE, none_live);
+  if (B <= hi || B > e->n_slots)
+    return e->fail(EMU_ERR_INVALID, "slot mode: B = " + std::to_string(B) + " must cover the highest live slot " +
+                                        std::to_string(hi) + " and stay within " + std::to_string(e->n_slots) + " slots");
+  for (int b = 0; b < B; ++b)
+    if (e->slots[b].live() && e->slots[b].len + 1 > e->cfg.llm_max_seq)
+      return e->fail(EMU_ERR_INVALID, "KV cache full at slot " + std::to_string(b));
+  return EMU_OK;
+}
+
 extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void* embeds, const int32_t* beam_src_idx,
                               int B, float* logits, void* hidden, int32_t* next_ids, int ban_id, emu_stream_t stream) {
   if (!e || B < 1 || ((token_ids == nullptr) == (embeds == nullptr))) return EMU_ERR_INVALID;
@@ -1410,16 +1375,7 @@ extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void
   const EmuConfig& c = e->cfg;
   cudaStream_t st = (cudaStream_t)stream;
   if (e->n_slots > 0) {
-    int hi = -1;
-    for (int b = 0; b < e->n_slots; ++b)
-      if (e->slot_group[b] >= 0) hi = b;
-    if (hi < 0) return e->fail(EMU_ERR_STATE, "decode with no live slot");
-    if (B <= hi || B > e->n_slots)
-      return e->fail(EMU_ERR_INVALID, "slot mode: B = " + std::to_string(B) + " must cover the highest live slot " +
-                                          std::to_string(hi) + " and stay within " + std::to_string(e->n_slots) + " slots");
-    for (int b = 0; b < B; ++b)
-      if (e->slot_group[b] >= 0 && e->slot_len[b] + 1 > c.llm_max_seq)
-        return e->fail(EMU_ERR_INVALID, "KV cache full at slot " + std::to_string(b));
+    EMU_TRY(check_decode_rows(e, B, "decode with no live slot"));
   } else {
     if (e->cur_len < 1) return e->fail(EMU_ERR_STATE, "decode before prefill");
     if (B != e->cache_B) return e->fail(EMU_ERR_STATE, "batch differs from cached batch");
@@ -1470,11 +1426,7 @@ extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void
     count_launch(e->graph_nodes[key]);
   }
   if (e->n_slots > 0) {
-    for (int b = 0; b < B; ++b)
-      if (e->slot_group[b] >= 0) {
-        e->slot_len[b] += 1;
-        if (e->slot_grows[b]) e->slot_own[b] += 1;
-      }
+    for (int b = 0; b < B; ++b) e->slots[b].advance();
   } else {
     e->cur_len += 1;
   }
@@ -1486,6 +1438,7 @@ extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void
 // ================================================================================================
 static int slot_mode_ok(EmuEngine* e) {
   if (e->cfg.llm_layers < 1) return e->fail(EMU_ERR_STATE, "engine has no LLM");
+  if (e->tp_size > 1) return e->fail(EMU_ERR_UNSUPPORTED, "slot mode under tensor parallelism");
   if (e->n_slots < 1) return e->fail(EMU_ERR_STATE, "not in slot mode (emu_llm_slots_begin)");
   return EMU_OK;
 }
@@ -1499,8 +1452,8 @@ static int check_slots(EmuEngine* e, const int32_t* slots, int n, bool want_free
       return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " out of range [0, " + std::to_string(e->n_slots) + ")");
     for (int j = 0; j < i; ++j)
       if (slots[j] == s) return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " named twice");
-    if (want_free && e->slot_group[s] >= 0) return e->fail(EMU_ERR_STATE, "slot " + std::to_string(s) + " is occupied");
-    if (!want_free && e->slot_group[s] < 0) return e->fail(EMU_ERR_STATE, "slot " + std::to_string(s) + " is free");
+    if (want_free && e->slots[s].live()) return e->fail(EMU_ERR_STATE, "slot " + std::to_string(s) + " is occupied");
+    if (!want_free && !e->slots[s].live()) return e->fail(EMU_ERR_STATE, "slot " + std::to_string(s) + " is free");
     out->r[i] = s;
   }
   return EMU_OK;
@@ -1509,14 +1462,111 @@ static int check_slots(EmuEngine* e, const int32_t* slots, int n, bool want_free
 // a beam group leaves together: its slots' table rows point into each other
 static int check_groups_leave(EmuEngine* e, const SlotList& rows, int n) {
   for (int b = 0; b < e->n_slots; ++b) {
-    if (e->slot_group[b] < 0) continue;
+    if (!e->slots[b].live()) continue;
     bool named = false, group_named = false;
     for (int i = 0; i < n; ++i) {
       named |= rows.r[i] == b;
-      group_named |= e->slot_group[rows.r[i]] == e->slot_group[b];
+      group_named |= e->slots[rows.r[i]].group == e->slots[b].group;
     }
     if (group_named && !named)
       return e->fail(EMU_ERR_STATE, "slot " + std::to_string(b) + " belongs to a leaving beam group and must leave with it");
+  }
+  return EMU_OK;
+}
+
+// the segments of a slot-mode prefill: free slot slot.r[i] continues after its first prefix.r[i] kept positions with
+// n_new.r[i] tokens and ends live (final_.r[i]) or kept at prefix + n_new
+struct Segments {
+  int n = 0;
+  SlotList slot, prefix, n_new, final_;
+};
+
+// slot mode's one prefill path, behind emu_llm_join, emu_llm_extend and emu_llm_step, in one pass over the weights: B decode
+// rows (token_ids, beams re-parented by beam_src_idx first; B may be 0), then the segments' tokens packed back to back.
+// Segment i's embeddings are rows [i * ld, i * ld + n_new[i]) of embeds (ld = 0: already packed).  mask [n, N], every segment
+// starting from nothing with N tokens: the left-pad starts and HF position offsets.  logits [B, vocab] of the decode rows
+// and logits_last [n, vocab] of each segment's last token, either may be null.  `what` names the call in a CUDA failure.
+static int slot_prefill(EmuEngine* e, const int32_t* token_ids, const int32_t* beam_src_idx, int B, float* logits,
+                        const Segments& sg, const void* embeds, int ld, const int32_t* mask, float* logits_last,
+                        const char* what, cudaStream_t st) {
+  const EmuConfig& c = e->cfg;
+  const int Hd = c.llm_hidden, n = sg.n, K = kLlmMaxRows;
+  int host_idx[6 * K];  // cache rows, prefixes, token counts, first packed rows, then the rows whose logits are read
+  SlotList len;
+  MixedRows m;
+  m.B = B; m.n = n; m.M = B; m.max_new = 0; m.Nk = 0;
+  for (int i = 0; i < n; ++i) {
+    const int k = sg.n_new.r[i];
+    host_idx[i] = sg.slot.r[i];
+    host_idx[K + i] = sg.prefix.r[i];
+    host_idx[2 * K + i] = k;
+    host_idx[3 * K + i] = m.M;
+    len.r[i] = sg.prefix.r[i] + k;
+    m.M += k;
+    m.max_new = k > m.max_new ? k : m.max_new;
+    m.Nk = len.r[i] > m.Nk ? len.r[i] : m.Nk;
+  }
+  int n_out = 0;  // logits rows: the decode rows, then each segment's last row
+  if (logits)
+    for (int b = 0; b < B; ++b) host_idx[4 * K + n_out++] = b;
+  if (logits_last)
+    for (int i = 0; i < n; ++i) host_idx[4 * K + n_out++] = host_idx[3 * K + i] + sg.n_new.r[i] - 1;
+  EMU_TRY(e->ensure(e->step_idx, sizeof(host_idx)));
+  int* d_idx = (int*)e->step_idx.p;
+  m.seg_row = d_idx;
+  m.seg_q0 = d_idx + K;
+  m.seg_new = d_idx + 2 * K;
+  m.seg_row0 = d_idx + 3 * K;
+  PdlScope pdl_chain(1);
+  if (cudaMemcpyAsync(d_idx, host_idx, sizeof(host_idx), cudaMemcpyHostToDevice, st) != cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "slot list upload failed");
+  EMU_TRY(prefill_stage(e, nullptr, m.M, st));
+  bf16* h = (bf16*)e->pf_h.p;
+  for (int i = 0; i < (ld > 0 ? n : 1); ++i) {  // one copy per segment; packed embeddings in one
+    const long dst = ld > 0 ? host_idx[3 * K + i] : B, rows = ld > 0 ? sg.n_new.r[i] : m.M - B;
+    if (cudaMemcpyAsync(h + dst * Hd, (const bf16*)embeds + (long)i * ld * Hd, (size_t)rows * Hd * 2, cudaMemcpyDeviceToDevice,
+                        st) != cudaSuccess)
+      return e->fail(EMU_ERR_CUDA, "embeds copy failed");
+  }
+  if (B > 0) {
+    EMU_TRY(embed_gather(e->embed, token_ids, h, B, Hd, st));
+    count_launch();
+  }
+  if (beam_src_idx) {
+    EMU_TRY(kv_reparent(e, beam_src_idx, B, st));
+    count_launch();
+  }
+  slot_resume_begin_kernel<<<1, 32, 0, st>>>(sg.slot, sg.prefix, e->d_kept_start, e->d_kept_posoff, e->d_join_start,
+                                             e->d_join_posoff, n);
+  if (mask) mask_start_kernel<<<n, 32, 0, st>>>(mask, sg.n_new.r[0], e->d_join_start, e->d_join_posoff, 1, 0);
+  count_launch(mask ? 2 : 1);
+  EMU_TRY(prefill_layers(e, 0, 0, 0, nullptr, nullptr, st, &m));
+  // live decode slots advance (before the segments' slots may become live), then the segments' slots take their state
+  if (B > 0) advance_pos_kernel<<<1, 32, 0, st>>>(e->d_pos, B, nullptr, e->d_active);
+  slot_step_end_kernel<<<n, 256, 0, st>>>(sg.slot, len, sg.final_, e->d_join_start, e->d_join_posoff, e->d_pos, e->d_start,
+                                          e->d_posoff, e->d_active, e->d_kept_start, e->d_kept_posoff, e->kv_indir, c.llm_max_seq);
+  count_launch(B > 0 ? 2 : 1);
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, std::string(what) + " failed");
+  for (int b = 0; b < B; ++b) e->slots[b].advance();
+  for (int i = 0; i < n; ++i) {
+    Slot& s = e->slots[sg.slot.r[i]];
+    if (sg.final_.r[i]) s.set_live(sg.slot.r[i], len.r[i]);
+    else s.set_kept(len.r[i]);
+  }
+  if (n_out == 0) return EMU_OK;
+  // the rows' logits in one pass over lm_head, written straight to the one output asked for, or split to both
+  float* out = logits ? logits : logits_last;
+  if (logits && logits_last) {
+    EMU_TRY(e->ensure(e->step_logits, (size_t)n_out * c.llm_vocab * sizeof(float)));
+    out = (float*)e->step_logits.p;
+  }
+  EMU_TRY(prefill_outputs(e, n_out, 1, nullptr, out, st, d_idx + 4 * K));
+  if (logits && logits_last) {
+    const size_t row_bytes = (size_t)c.llm_vocab * sizeof(float);
+    if (cudaMemcpyAsync(logits, out, B * row_bytes, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+      return e->fail(EMU_ERR_CUDA, "decode logits copy failed");
+    if (cudaMemcpyAsync(logits_last, out + (size_t)B * c.llm_vocab, n * row_bytes, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+      return e->fail(EMU_ERR_CUDA, "segment logits copy failed");
   }
   return EMU_OK;
 }
@@ -1534,11 +1584,7 @@ extern "C" int emu_llm_slots_begin(EmuEngine* e, int n_slots, emu_stream_t s) {
   if (cudaMemsetAsync(e->d_active, 0, kLlmMaxRows * sizeof(int), (cudaStream_t)s) != cudaSuccess)
     return e->fail(EMU_ERR_CUDA, "slot state reset failed");
   e->n_slots = n_slots;
-  e->slot_len.assign(n_slots, 0);
-  e->slot_group.assign(n_slots, -1);
-  e->slot_kept.assign(n_slots, 0);
-  e->slot_own.assign(n_slots, 0);
-  e->slot_grows.assign(n_slots, 0);
+  e->slots.assign(n_slots, Slot());
   e->kv_indir_dirty = true;  // joins, forks and leaves rewrite table rows: emu_llm_reset restores the identity
   return EMU_OK;
 }
@@ -1550,37 +1596,23 @@ extern "C" int emu_llm_join(EmuEngine* e, const int32_t* host_slots, int n, cons
   EMU_TRY(llm_ready(e));
   const EmuConfig& c = e->cfg;
   if (N > c.llm_max_seq) return e->fail(EMU_ERR_INVALID, "prompt of " + std::to_string(N) + " tokens exceeds llm_max_seq");
-  SlotList rows;
-  EMU_TRY(check_slots(e, host_slots, n, true, &rows));
-  cudaStream_t st = (cudaStream_t)stream;
-  PdlScope pdl_chain(1);
-  if (cudaMemcpyAsync(e->d_join_rows, rows.r, n * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess)
-    return e->fail(EMU_ERR_CUDA, "slot list upload failed");
-  EMU_TRY(prefill_stage(e, inputs_embeds, (long)n * N, st));
-  // left-pad starts and HF position offsets of the joining sequences, join-local; scattered to their slots below
-  if (attention_mask) mask_start_kernel<<<n, 32, 0, st>>>(attention_mask, N, e->d_join_start, e->d_join_posoff, 1, 0);
-  else cudaMemsetAsync(e->d_join_start, 0, 2 * kLlmMaxRows * sizeof(int), st);
-  count_launch();
-  EMU_TRY(prefill_layers(e, n, N, 0, e->d_join_start, e->d_join_posoff, e->d_join_rows, st));
-  slot_set_kernel<<<n, 256, 0, st>>>(rows, e->d_join_start, e->d_join_posoff, N, e->d_pos, e->d_start, e->d_posoff, e->d_active,
-                                     e->kv_indir, c.llm_max_seq);
-  count_launch();
-  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot join failed");
+  Segments sg;
+  sg.n = n;
+  EMU_TRY(check_slots(e, host_slots, n, true, &sg.slot));
   for (int i = 0; i < n; ++i) {
-    e->slot_len[rows.r[i]] = N;
-    e->slot_group[rows.r[i]] = rows.r[i];
-    e->slot_kept[rows.r[i]] = 0;
-    e->slot_own[rows.r[i]] = N;
-    e->slot_grows[rows.r[i]] = 1;
+    sg.prefix.r[i] = 0;
+    sg.n_new.r[i] = N;
+    sg.final_.r[i] = 1;
   }
-  return prefill_outputs(e, n, N, nullptr, logits_last, st);
+  return slot_prefill(e, nullptr, nullptr, 0, nullptr, sg, inputs_embeds, 0, attention_mask, logits_last, "slot join",
+                      (cudaStream_t)stream);
 }
 
 extern "C" int emu_llm_fork(EmuEngine* e, int src_slot, const int32_t* host_dst_slots, int n, emu_stream_t stream) {
   if (!e || !host_dst_slots || n < 1) return EMU_ERR_INVALID;
   EMU_TRY(slot_mode_ok(e));
   if (src_slot < 0 || src_slot >= e->n_slots) return e->fail(EMU_ERR_INVALID, "source slot " + std::to_string(src_slot) + " out of range");
-  if (e->slot_group[src_slot] < 0) return e->fail(EMU_ERR_STATE, "source slot " + std::to_string(src_slot) + " is free");
+  if (!e->slots[src_slot].live()) return e->fail(EMU_ERR_STATE, "source slot " + std::to_string(src_slot) + " is free");
   SlotList dst;
   EMU_TRY(check_slots(e, host_dst_slots, n, true, &dst));
   const EmuConfig& c = e->cfg;
@@ -1588,61 +1620,34 @@ extern "C" int emu_llm_fork(EmuEngine* e, int src_slot, const int32_t* host_dst_
                                                         c.llm_max_seq);
   count_launch();
   if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot fork failed");
-  for (int i = 0; i < n; ++i) {
-    e->slot_len[dst.r[i]] = e->slot_len[src_slot];
-    e->slot_group[dst.r[i]] = e->slot_group[src_slot];
-    e->slot_kept[dst.r[i]] = 0;
-    e->slot_own[dst.r[i]] = 0;  // its table row points into the source's row
-    e->slot_grows[dst.r[i]] = 0;
-  }
-  e->slot_grows[src_slot] = 0;  // beam re-parenting scatters the group's new positions over its rows
+  for (int i = 0; i < n; ++i) e->slots[dst.r[i]].set_fork(e->slots[src_slot]);
+  e->slots[src_slot].grows = false;  // beam re-parenting scatters the group's new positions over its rows
   return EMU_OK;
 }
 
 extern "C" int emu_llm_leave(EmuEngine* e, const int32_t* host_slots, int n, emu_stream_t stream) {
-  if (!e || !host_slots || n < 1) return EMU_ERR_INVALID;
-  EMU_TRY(slot_mode_ok(e));
-  SlotList rows;
-  EMU_TRY(check_slots(e, host_slots, n, false, &rows));
-  EMU_TRY(check_groups_leave(e, rows, n));
-  const EmuConfig& c = e->cfg;
-  slot_set_kernel<<<n, 256, 0, (cudaStream_t)stream>>>(rows, nullptr, nullptr, 0, e->d_pos, e->d_start, e->d_posoff, e->d_active,
-                                                       e->kv_indir, c.llm_max_seq);
-  count_launch();
-  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot leave failed");
-  for (int i = 0; i < n; ++i) {
-    e->slot_len[rows.r[i]] = 0;
-    e->slot_group[rows.r[i]] = -1;
-    e->slot_kept[rows.r[i]] = 0;
-    e->slot_own[rows.r[i]] = 0;
-    e->slot_grows[rows.r[i]] = 0;
-  }
-  return EMU_OK;
+  static const int32_t keep_none[kLlmMaxRows] = {};  // n is checked against n_slots <= kLlmMaxRows before it is read
+  return emu_llm_leave_keep(e, host_slots, keep_none, n, stream);
 }
 
 extern "C" int emu_llm_slot_len(EmuEngine* e, int slot) {
   if (!e || e->n_slots < 1 || slot < 0 || slot >= e->n_slots) return -1;
-  return e->slot_len[slot];
+  return e->slots[slot].len;
 }
 
 // ================================================================================================
 // prefix caching: kept slots and per-slot continuation (include/emu_b200_prefix.h)
 // ================================================================================================
-static int prefix_mode_ok(EmuEngine* e) {
-  if (e->tp_size > 1) return e->fail(EMU_ERR_UNSUPPORTED, "prefix caching under tensor parallelism");
-  return slot_mode_ok(e);
-}
-
 extern "C" int emu_llm_leave_keep(EmuEngine* e, const int32_t* host_slots, const int32_t* host_keep, int n, emu_stream_t stream) {
   if (!e || !host_slots || !host_keep || n < 1) return EMU_ERR_INVALID;
-  EMU_TRY(prefix_mode_ok(e));
+  EMU_TRY(slot_mode_ok(e));
   SlotList rows, keep;
   EMU_TRY(check_slots(e, host_slots, n, false, &rows));
   EMU_TRY(check_groups_leave(e, rows, n));
   const EmuConfig& c = e->cfg;
   for (int i = 0; i < n; ++i) {
     const int s = rows.r[i], k = host_keep[i];
-    const int own = e->slot_own[s];
+    const int own = e->slots[s].own;
     if (k < 0 || k > own || k > c.llm_max_seq - 1)
       return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " may keep 0 .. " +
                                           std::to_string(own < c.llm_max_seq - 1 ? own : c.llm_max_seq - 1) +
@@ -1654,33 +1659,26 @@ extern "C" int emu_llm_leave_keep(EmuEngine* e, const int32_t* host_slots, const
                                                         e->d_kept_posoff, e->kv_indir, c.llm_max_seq);
   count_launch();
   if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot leave failed");
-  for (int i = 0; i < n; ++i) {
-    const int s = rows.r[i];
-    e->slot_len[s] = 0;
-    e->slot_group[s] = -1;
-    e->slot_kept[s] = keep.r[i];
-    e->slot_own[s] = 0;
-    e->slot_grows[s] = 0;
-  }
+  for (int i = 0; i < n; ++i) e->slots[rows.r[i]].set_kept(keep.r[i]);
   return EMU_OK;
 }
 
 extern "C" int emu_llm_slot_kept(EmuEngine* e, int slot) {
   if (!e || e->n_slots < 1 || slot < 0 || slot >= e->n_slots) return -1;
-  return e->slot_kept[slot];
+  return e->slots[slot].kept;
 }
 
 extern "C" int emu_llm_copy_prefix(EmuEngine* e, int src_slot, int dst_slot, int P, emu_stream_t stream) {
   if (!e) return EMU_ERR_INVALID;
-  EMU_TRY(prefix_mode_ok(e));
+  EMU_TRY(slot_mode_ok(e));
   const EmuConfig& c = e->cfg;
   if (src_slot < 0 || src_slot >= e->n_slots) return e->fail(EMU_ERR_INVALID, "source slot " + std::to_string(src_slot) + " out of range");
   if (dst_slot < 0 || dst_slot >= e->n_slots)
     return e->fail(EMU_ERR_INVALID, "destination slot " + std::to_string(dst_slot) + " out of range");
   if (dst_slot == src_slot) return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(src_slot) + " copied onto itself");
-  if (e->slot_group[dst_slot] >= 0) return e->fail(EMU_ERR_STATE, "destination slot " + std::to_string(dst_slot) + " is occupied");
-  const bool live = e->slot_group[src_slot] >= 0;
-  const int avail = live ? e->slot_own[src_slot] : e->slot_kept[src_slot];
+  if (e->slots[dst_slot].live()) return e->fail(EMU_ERR_STATE, "destination slot " + std::to_string(dst_slot) + " is occupied");
+  const bool live = e->slots[src_slot].live();
+  const int avail = live ? e->slots[src_slot].own : e->slots[src_slot].kept;
   if (!live && avail == 0) return e->fail(EMU_ERR_STATE, "source slot " + std::to_string(src_slot) + " is free and keeps nothing");
   if (P < 1 || P > avail || P > c.llm_max_seq - 1)
     return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(src_slot) + " holds " + std::to_string(avail) +
@@ -1692,63 +1690,37 @@ extern "C" int emu_llm_copy_prefix(EmuEngine* e, int src_slot, int dst_slot, int
                                             e->d_kept_start, e->d_kept_posoff, e->kv_indir, c.llm_max_seq);
   count_launch(2);
   if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "prefix copy failed");
-  e->slot_kept[dst_slot] = P;
+  e->slots[dst_slot].set_kept(P);
   return EMU_OK;
 }
 
 extern "C" int emu_llm_extend(EmuEngine* e, const int32_t* host_slots, const int32_t* host_prefix, const int32_t* host_new, int n,
                               const void* inputs_embeds, int N, float* logits_last, emu_stream_t stream) {
   if (!e || !host_slots || !host_prefix || !host_new || !inputs_embeds || n < 1 || N < 1) return EMU_ERR_INVALID;
-  EMU_TRY(prefix_mode_ok(e));
+  EMU_TRY(slot_mode_ok(e));
   EMU_TRY(llm_ready(e));
   const EmuConfig& c = e->cfg;
   if (N > c.llm_max_seq) return e->fail(EMU_ERR_INVALID, "suffix of " + std::to_string(N) + " tokens exceeds llm_max_seq");
-  SlotList rows, prefix, len;
-  EMU_TRY(check_slots(e, host_slots, n, true, &rows));
-  int host_ext[3 * kLlmMaxRows];
-  int max_prefix = 0;
+  Segments sg;
+  sg.n = n;
+  EMU_TRY(check_slots(e, host_slots, n, true, &sg.slot));
   for (int i = 0; i < n; ++i) {
-    const int s = rows.r[i], p = host_prefix[i], k = host_new[i];
-    if (p < 0 || p > e->slot_kept[s])
-      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " keeps " + std::to_string(e->slot_kept[s]) +
+    const int s = sg.slot.r[i], p = host_prefix[i], k = host_new[i];
+    if (p < 0 || p > e->slots[s].kept)
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " keeps " + std::to_string(e->slots[s].kept) +
                                           " positions, asked to resume at " + std::to_string(p));
     if (k < 1 || k > N)
       return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + ": " + std::to_string(k) + " new tokens, N = " + std::to_string(N));
     if (p + k > c.llm_max_seq)
       return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + ": " + std::to_string(p) + " + " + std::to_string(k) +
                                           " positions exceed llm_max_seq");
-    prefix.r[i] = p;
-    len.r[i] = p + k;
-    host_ext[i] = s;
-    host_ext[kLlmMaxRows + i] = p;
-    host_ext[2 * kLlmMaxRows + i] = k;
-    max_prefix = p > max_prefix ? p : max_prefix;
+    sg.prefix.r[i] = p;
+    sg.n_new.r[i] = k;
+    sg.final_.r[i] = 1;
   }
-  const int Nk = max_prefix + N < c.llm_max_seq ? max_prefix + N : c.llm_max_seq;
-  cudaStream_t st = (cudaStream_t)stream;
-  PdlScope pdl_chain(1);
-  if (cudaMemcpyAsync(e->d_ext, host_ext, sizeof(host_ext), cudaMemcpyHostToDevice, st) != cudaSuccess)
-    return e->fail(EMU_ERR_CUDA, "slot list upload failed");
-  const int* d_rows = e->d_ext;
-  const int* d_q0 = e->d_ext + kLlmMaxRows;
-  const int* d_new = e->d_ext + 2 * kLlmMaxRows;
-  EMU_TRY(prefill_stage(e, inputs_embeds, (long)n * N, st));
-  slot_resume_begin_kernel<<<1, 32, 0, st>>>(rows, prefix, e->d_kept_start, e->d_kept_posoff, e->d_join_start, e->d_join_posoff, n);
-  count_launch();
-  EMU_TRY(prefill_layers(e, n, N, 0, e->d_join_start, e->d_join_posoff, d_rows, st, d_q0, d_new, Nk));
-  slot_resume_end_kernel<<<n, 256, 0, st>>>(rows, len, e->d_join_start, e->d_join_posoff, e->d_pos, e->d_start, e->d_posoff,
-                                            e->d_active, e->kv_indir, c.llm_max_seq);
-  count_launch();
-  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "slot extend failed");
-  for (int i = 0; i < n; ++i) {
-    const int s = rows.r[i];
-    e->slot_len[s] = len.r[i];
-    e->slot_group[s] = s;
-    e->slot_kept[s] = 0;
-    e->slot_own[s] = len.r[i];
-    e->slot_grows[s] = 1;
-  }
-  return prefill_outputs(e, n, N, nullptr, logits_last, st, d_new);
+  // the right-padded [n, N] rows are compacted as they are staged: no kernel sees a padding row
+  return slot_prefill(e, nullptr, nullptr, 0, nullptr, sg, inputs_embeds, N, nullptr, logits_last, "slot extend",
+                      (cudaStream_t)stream);
 }
 
 extern "C" int emu_llm_kv_cache(EmuEngine* e, void** kv, int64_t* dims5) {
@@ -1773,119 +1745,27 @@ extern "C" int emu_llm_step(EmuEngine* e, const int32_t* token_ids, const int32_
   if (!e || !host_slots || !host_prefix || !host_new || !host_final || !embeds || n < 1 || B < 0) return EMU_ERR_INVALID;
   if (B > 0 && !token_ids) return EMU_ERR_INVALID;
   if (B == 0 && (beam_src_idx || logits)) return EMU_ERR_INVALID;
-  EMU_TRY(prefix_mode_ok(e));
-  if (e->kv_copy) return e->fail(EMU_ERR_UNSUPPORTED, "chunked prefill with EMU_KV_COPY=1");
+  EMU_TRY(slot_mode_ok(e));
   EMU_TRY(llm_ready(e));
   const EmuConfig& c = e->cfg;
-  // the decode part: as emu_llm_decode in slot mode
-  if (B > 0) {
-    int hi = -1;
-    for (int b = 0; b < e->n_slots; ++b)
-      if (e->slot_group[b] >= 0) hi = b;
-    if (hi < 0) return e->fail(EMU_ERR_STATE, "a decode part of " + std::to_string(B) + " rows with no live slot");
-    if (B <= hi || B > e->n_slots)
-      return e->fail(EMU_ERR_INVALID, "slot mode: B = " + std::to_string(B) + " must cover the highest live slot " +
-                                          std::to_string(hi) + " and stay within " + std::to_string(e->n_slots) + " slots");
-    for (int b = 0; b < B; ++b)
-      if (e->slot_group[b] >= 0 && e->slot_len[b] + 1 > c.llm_max_seq)
-        return e->fail(EMU_ERR_INVALID, "KV cache full at slot " + std::to_string(b));
-  }
+  if (B > 0) EMU_TRY(check_decode_rows(e, B, "a decode part of " + std::to_string(B) + " rows with no live slot"));
   // the segments: as emu_llm_extend, each ending live (final) or kept
-  SlotList rows, len, fin;
-  EMU_TRY(check_slots(e, host_slots, n, true, &rows));
-  int host_idx[6 * kLlmMaxRows];  // cache rows, prefixes, token counts, first packed rows, then the rows whose logits are read
-  int total = 0, max_new = 0, max_end = 0;
+  Segments sg;
+  sg.n = n;
+  EMU_TRY(check_slots(e, host_slots, n, true, &sg.slot));
   for (int i = 0; i < n; ++i) {
-    const int s = rows.r[i], p = host_prefix[i], k = host_new[i], f = host_final[i];
+    const int s = sg.slot.r[i], p = host_prefix[i], k = host_new[i], f = host_final[i];
     if (f != 0 && f != 1) return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + ": final must be 0 or 1, got " + std::to_string(f));
-    if (p < 0 || p > e->slot_kept[s])
-      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " keeps " + std::to_string(e->slot_kept[s]) +
+    if (p < 0 || p > e->slots[s].kept)
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + " keeps " + std::to_string(e->slots[s].kept) +
                                           " positions, asked to resume at " + std::to_string(p));
     const int room = f ? c.llm_max_seq : c.llm_max_seq - 1;  // a slot left mid-prefill is kept: at most llm_max_seq - 1
     if (k < 1 || k > room - p)
       return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(s) + ": " + std::to_string(k) + " new tokens after " + std::to_string(p) +
                                           " must be in [1, " + std::to_string(room - p) + "] (" + (f ? "final" : "not final") + ")");
-    host_idx[i] = s;
-    host_idx[kLlmMaxRows + i] = p;
-    host_idx[2 * kLlmMaxRows + i] = k;
-    host_idx[3 * kLlmMaxRows + i] = B + total;
-    len.r[i] = p + k;
-    fin.r[i] = f;
-    total += k;
-    max_new = k > max_new ? k : max_new;
-    max_end = p + k > max_end ? p + k : max_end;
+    sg.prefix.r[i] = p;
+    sg.n_new.r[i] = k;
+    sg.final_.r[i] = f;
   }
-  int n_out = 0;  // logits rows: the decode rows, then each segment's last row
-  if (logits)
-    for (int b = 0; b < B; ++b) host_idx[4 * kLlmMaxRows + n_out++] = b;
-  if (logits_last)
-    for (int i = 0; i < n; ++i) host_idx[4 * kLlmMaxRows + n_out++] = host_idx[3 * kLlmMaxRows + i] + host_new[i] - 1;
-  MixedRows mix;
-  mix.B = B; mix.n = n; mix.M = B + total; mix.max_new = max_new; mix.Nk = max_end;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int Hd = c.llm_hidden;
-  EMU_TRY(e->ensure(e->step_idx, sizeof(host_idx)));
-  int* d_idx = (int*)e->step_idx.p;
-  mix.seg_row = d_idx;
-  mix.seg_q0 = d_idx + kLlmMaxRows;
-  mix.seg_new = d_idx + 2 * kLlmMaxRows;
-  mix.seg_row0 = d_idx + 3 * kLlmMaxRows;
-  PdlScope pdl_chain(1);
-  if (cudaMemcpyAsync(d_idx, host_idx, sizeof(host_idx), cudaMemcpyHostToDevice, st) != cudaSuccess)
-    return e->fail(EMU_ERR_CUDA, "slot list upload failed");
-  EMU_TRY(prefill_stage(e, embeds, mix.M, st, B));
-  if (B > 0) {
-    EMU_TRY(embed_gather(e->embed, token_ids, (bf16*)e->pf_h.p, B, Hd, st));
-    count_launch();
-  }
-  if (beam_src_idx) {
-    EMU_TRY(kv_reparent(e, beam_src_idx, B, st));
-    count_launch();
-  }
-  SlotList prefix;
-  for (int i = 0; i < n; ++i) prefix.r[i] = host_prefix[i];
-  slot_resume_begin_kernel<<<1, 32, 0, st>>>(rows, prefix, e->d_kept_start, e->d_kept_posoff, e->d_join_start, e->d_join_posoff, n);
-  count_launch();
-  EMU_TRY(prefill_layers(e, n, 0, 0, nullptr, nullptr, nullptr, st, nullptr, nullptr, 0, &mix));
-  // live decode slots advance (before the segments' slots may become live), then the segments' slots take their state
-  if (B > 0) advance_pos_kernel<<<1, 32, 0, st>>>(e->d_pos, B, nullptr, e->d_active);
-  slot_step_end_kernel<<<n, 256, 0, st>>>(rows, len, fin, e->d_join_start, e->d_join_posoff, e->d_pos, e->d_start, e->d_posoff,
-                                          e->d_active, e->d_kept_start, e->d_kept_posoff, e->kv_indir, c.llm_max_seq);
-  count_launch(B > 0 ? 2 : 1);
-  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "mixed step failed");
-  for (int b = 0; b < B; ++b)
-    if (e->slot_group[b] >= 0) {
-      e->slot_len[b] += 1;
-      if (e->slot_grows[b]) e->slot_own[b] += 1;
-    }
-  for (int i = 0; i < n; ++i) {
-    const int s = rows.r[i];
-    e->slot_len[s] = fin.r[i] ? len.r[i] : 0;
-    e->slot_group[s] = fin.r[i] ? s : -1;
-    e->slot_kept[s] = fin.r[i] ? 0 : len.r[i];
-    e->slot_own[s] = fin.r[i] ? len.r[i] : 0;
-    e->slot_grows[s] = fin.r[i] ? 1 : 0;
-  }
-  if (n_out == 0) return EMU_OK;
-  // logits: the rows read, one final norm and one lm_head GEMM over them, then split to the two outputs
-  EMU_TRY(e->ensure(e->pf_last, (size_t)n_out * Hd * 2));
-  EMU_TRY(e->ensure(e->step_logits, (size_t)n_out * c.llm_vocab * sizeof(float)));
-  bf16* last = (bf16*)e->pf_last.p;
-  float* lg = (float*)e->step_logits.p;
-  gather_rows_kernel<<<n_out, 128, 0, st>>>((const bf16*)e->pf_h.p, Hd, d_idx + 4 * kLlmMaxRows, last);
-  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "logits row gather failed");
-  EMU_TRY(rmsnorm(last, e->final_norm, last, n_out, Hd, c.llm_rms_eps, 0, st));
-  GemmEpilogue el;
-  el.out_fp32 = 1;
-  el.C = lg; el.ldc = c.llm_vocab;
-  EMU_TRY(gemm_bf16(last, Hd, e->lm_head, Hd, n_out, e->Vl, Hd, el, st));
-  count_launch(3);
-  const size_t row_bytes = (size_t)c.llm_vocab * sizeof(float);
-  const int n_dec = logits ? B : 0;
-  if (n_dec > 0 && cudaMemcpyAsync(logits, lg, n_dec * row_bytes, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
-    return e->fail(EMU_ERR_CUDA, "decode logits copy failed");
-  if (logits_last && cudaMemcpyAsync(logits_last, lg + (size_t)n_dec * c.llm_vocab, n * row_bytes, cudaMemcpyDeviceToDevice, st) !=
-                         cudaSuccess)
-    return e->fail(EMU_ERR_CUDA, "segment logits copy failed");
-  return EMU_OK;
+  return slot_prefill(e, token_ids, beam_src_idx, B, logits, sg, embeds, 0, nullptr, logits_last, "mixed step", (cudaStream_t)stream);
 }

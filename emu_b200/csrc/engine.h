@@ -37,6 +37,26 @@ struct DevBuf {
   size_t bytes = 0;
 };
 
+// slot mode: the host mirror of one slot.  Live at length len, or free and keeping the first `kept` positions of its own row
+// (prefix caching; 0 = nothing).  own = how many leading positions of a live slot's table row are its own physical row: its
+// whole length while it was never re-parented (grows), the join length of a beam group's first slot, 0 for a forked slot.
+struct Slot {
+  int len = 0;     // host mirror of d_pos (0 = free)
+  int group = -1;  // first slot of its beam group, -1 = free
+  int kept = 0, own = 0;
+  bool grows = false;
+  bool live() const { return group >= 0; }
+  void set_live(int self, int L) { *this = Slot{L, self, 0, L, true}; }
+  void set_kept(int K) { *this = Slot{0, -1, K, 0, false}; }
+  void set_free() { set_kept(0); }
+  void set_fork(const Slot& src) { *this = Slot{src.len, src.group, 0, 0, false}; }  // its table row points into src's
+  void advance() {  // a decode step
+    if (!live()) return;
+    len += 1;
+    if (grows) own += 1;
+  }
+};
+
 struct UNetModel;  // unet.cu
 struct VaeModel;   // vae.cu
 struct CFormerModel;  // cformer.cu
@@ -85,21 +105,14 @@ struct EmuEngine {
   float *dec_logits_shard = nullptr, *dec_logits_gather = nullptr;
   // prefill workspaces (grown on demand)
   emu::DevBuf pf_h, pf_xn, pf_qkv, pf_attn, pf_act, pf_tmp, pf_last;
-  emu::DevBuf step_idx, step_logits;  // emu_llm_step: its slot lists and logits rows, and the logits of those rows
+  emu::DevBuf step_idx, step_logits;  // slot-mode prefill: its segment lists and logits rows, and the logits of those rows
   // slot mode (continuous batching, include/emu_b200_slots.h): every cache row is a slot holding its own sequence
   int n_slots = 0;               // > 0: slot mode with this many slots
-  std::vector<int> slot_len;     // host mirror of d_pos per slot (0 = free)
-  std::vector<int> slot_group;   // first slot of the slot's beam group, -1 = free
+  std::vector<emu::Slot> slots;  // [n_slots]
   int* d_active = nullptr;       // [kLlmMaxRows] 1 = live slot: the decode step advances its position
-  int* d_join_rows = nullptr;    // [kLlmMaxRows] cache rows of the sequences being joined
-  int *d_join_start = nullptr, *d_join_posoff = nullptr;  // [kLlmMaxRows] their left-pad starts / position offsets
-  // prefix caching (include/emu_b200_prefix.h): a slot may leave but keep the first slot_kept[s] positions of its own row.
-  // slot_own[s] = how many leading positions of a live slot's table row are its own physical row: the whole length of a
-  // slot that was never re-parented (slot_grows), the join length of a beam group's first slot, 0 for a forked slot.
-  std::vector<int> slot_kept, slot_own;
-  std::vector<char> slot_grows;
+  // [kLlmMaxRows] left-pad starts / position offsets of the segments being prefilled (join, extend, mixed step)
+  int *d_join_start = nullptr, *d_join_posoff = nullptr;
   int *d_kept_start = nullptr, *d_kept_posoff = nullptr;  // [kLlmMaxRows] a kept slot's real left-pad start / position offset
-  int* d_ext = nullptr;  // [3][kLlmMaxRows] emu_llm_extend's cache rows, prefix lengths and new-token counts
   // decode graphs keyed by the baked-in arguments (the last int: slot mode, whose step advances live rows only)
   typedef std::tuple<int, const void*, const void*, const void*, const void*, const void*, const void*, int, int> GraphKey;
   std::map<GraphKey, cudaGraphExec_t> graphs;

@@ -114,18 +114,17 @@ struct AttnArgs {
   int causal = 0;                 // query i attends keys j <= i + (Nk - Nq)
   const int* kv_start = nullptr;  // [B] first valid key (left padding) or null
   const float* bias = nullptr;    // [H, Nq, Nk] additive (T5 relative position bias) or null
-  // [B] batch index of k / v read by query batch b (a join prefills new sequences into chosen KV-cache rows), or null =
-  // b itself; kv_rows = how many batch entries the k / v views span (0 = B)
+  // [B] batch index of k / v read by query batch b (slot mode reads and writes chosen KV-cache rows), or null = b itself;
+  // kv_rows = how many batch entries the k / v views span (0 = B)
   const int* kv_row = nullptr;
   int kv_rows = 0;
-  // [B] causal attention with a per-batch query offset (prefix caching): query i of batch b sits at key position
-  // q_off[b] + i and sees keys [kv_start[b], q_off[b] + i]; null = the uniform offset Nk - Nq.  D of 64 or 128 only.
+  // Packed queries (slot mode), all three [B] or all null, causal, D of 64 or 128 only: batch b's queries are rows
+  // q_row0[b] .. q_row0[b] + q_len[b] - 1 of ONE [q_rows, H, D] view of q and of out (q_bs / o_bs unused; rows outside a
+  // batch are never stored).  Query i of batch b sits at key position q_off[b] + i and sees keys [kv_start[b], q_off[b] + i]
+  // (null: the uniform offset Nk - Nq).  Keys at or past q_off[b] + q_len[b] were not written by the caller: no query reads
+  // them and their V rows enter P·V as zeros.
   const int* q_off = nullptr;
-  // [B] with q_off: batch b's real query rows (right padding beyond them), or null = Nq.  Keys at or past q_off[b] + q_len[b]
-  // were not written by the caller: no query reads them and their V rows enter P·V as zeros.
   const int* q_len = nullptr;
-  // [B] with q_off and q_len, packed queries (chunked prefill): batch b's queries are rows q_row0[b] .. q_row0[b] + q_len[b]
-  // - 1 of ONE [q_rows, H, D] view of q and of out (q_bs / o_bs unused); rows outside a batch are never stored.
   const int* q_row0 = nullptr;
   int q_rows = 0;
 };
@@ -167,12 +166,7 @@ int rope_kv_write(bf16* qkv /*[B,N,3*H*D] pair-interleaved q,k*/, int B, int N, 
                   cudaStream_t st, const int* pos_dev = nullptr /*[B] device slot of the new token (N == 1), overrides pos0*/,
                   bf16* q_out = nullptr /*decode: the rotated q goes compact [B*N, H*D] here instead of in place*/,
                   const int* kv_row = nullptr /*[B] cache row of batch b (join into chosen rows), null = b*/);
-// prefix caching (emu_llm_extend): batch b's N tokens go to cache slots q0[b] + n of row kv_row[b] (null = b), rotated at
-// position slot - pos_off[b]; only n < n_new[b] are real (right padding): the rest are neither rotated nor written
-int rope_kv_write_rows(bf16* qkv, int B, int N, int H, int D, const bf16* cos, const bf16* sin, const int* pos_off /*[B]*/,
-                       const int* q0 /*[B]*/, const int* n_new /*[B]*/, bf16* k_cache, bf16* v_cache, int t_max,
-                       const int* kv_row, cudaStream_t st);
-// chunked prefill (emu_llm_step): one launch over the M packed rows of a mixed step (include/emu_b200_chunked.h,
+// slot mode (join, extend, mixed step): one launch over the M packed rows of a mixed step (include/emu_b200_chunked.h,
 // emu_op_rope_kv_write_packed); decode rows of slots with active[b] == 0 write no K/V
 int rope_kv_write_packed(bf16* qkv, int M, int B, int n, int H, int D, const bf16* cos, const bf16* sin, const int* pos,
                          const int* pos_off, const int* active, bf16* q_out, const int* seg_row, const int* seg_q0,

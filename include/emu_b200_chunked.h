@@ -34,12 +34,16 @@ extern "C" {
  * own.  embeds [sum(host_new), hidden] bf16 (device), the segments back to back.  host_final[i] = 1: the slot becomes live at
  * prefix + new (at most llm_max_seq), as after emu_llm_extend; 0: it is kept at prefix + new (at most llm_max_seq - 1).
  * logits_last [n, vocab] fp32: the logits of each segment's last token, or NULL.
- * The segments' slots are distinct and not live; they may lie below B. */
+ * The segments' slots are distinct and not live; they may lie below B.
+ * Logits rows (the decode rows and the segments' last tokens) take the prefill rule: the final norm fused into the lm_head
+ * GEMV at up to 8 rows, norm then GEMM above that.  emu_llm_join and emu_llm_extend are this call with B = 0 and every
+ * segment final. */
 int emu_llm_step(EmuEngine* e, const int32_t* token_ids, const int32_t* beam_src_idx, int B, float* logits,
                  const int32_t* host_slots, const int32_t* host_prefix, const int32_t* host_new, const int32_t* host_final, int n,
                  const void* embeds, float* logits_last, emu_stream_t s);
 
-/* ---- the kernels behind emu_llm_step as stand-alone operators (device pointers, B <= 32, n <= 32) ---- */
+/* ---- the kernels behind slot mode's prefill (emu_llm_join, emu_llm_extend and emu_llm_step all run it) as stand-alone
+ * operators (device pointers, B <= 32, n <= 32) ---- */
 
 /* RoPE + KV append of a packed mixed step: qkv [M, 3*H*D] bf16 (q / k pair-interleaved per head), M >= B + n.
  * Row b < B (decode): rotated at pos[b] - pos_off[b]; q goes compact to q_out [B, H*D]; its k / v go to slot pos[b] of cache

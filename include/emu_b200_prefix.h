@@ -34,7 +34,7 @@ int emu_llm_copy_prefix(EmuEngine* e, int src_slot, int dst_slot, int P, emu_str
 /* The free slots host_slots[0..n) become live: slot i continues at length host_prefix[i] (at most its kept length; 0 starts
  * from nothing), and host_new[i] (1 .. N) tokens, right-padded to N in inputs_embeds [n, N, hidden] bf16, are prefilled after
  * it with HF positions continuing the slot's own.  logits_last [n, vocab] fp32: the logits of each row's last real token, or
- * NULL.  One weight pass for all n rows. */
+ * NULL.  One weight pass for all n rows: the rows are compacted as they are staged, so no padding token is computed. */
 int emu_llm_extend(EmuEngine* e, const int32_t* host_slots, const int32_t* host_prefix, const int32_t* host_new, int n,
                    const void* inputs_embeds, int N, float* logits_last, emu_stream_t s);
 
@@ -42,24 +42,7 @@ int emu_llm_extend(EmuEngine* e, const int32_t* host_slots, const int32_t* host_
  * heads, llm_max_seq, head dim}.  The pointer stays valid until the engine is destroyed. */
 int emu_llm_kv_cache(EmuEngine* e, void** kv, int64_t* dims5);
 
-/* ---- the kernels behind emu_llm_extend and emu_llm_copy_prefix as stand-alone operators (device pointers, B <= 32) ---- */
-
-/* RoPE + KV append of right-padded rows: qkv [B, N, 3*H*D] bf16 (q / k pair-interleaved per head); batch b's first
- * n_new[b] tokens are rotated at cache slot q0[b] + n minus pos_off[b] (q in place) and their k / v written to slot
- * q0[b] + n of cache row kv_row[b] (NULL = b) of k_cache / v_cache [rows, H, t_max, D]; the padding is left untouched.
- * q0, n_new, pos_off, kv_row: device int32 [B].  D = 64 or 128. */
-int emu_op_rope_kv_write_rows(void* qkv, int B, int N, int H, int D, const void* rope_cos, const void* rope_sin,
-                              const int32_t* pos_off, const int32_t* q0, const int32_t* n_new, const int32_t* kv_row, void* k_cache,
-                              void* v_cache, int t_max, emu_stream_t s);
-
-/* Causal prefill attention with a per-batch query offset: query i of batch b sits at key position q_off[b] + i and sees keys
- * [kv_start[b], q_off[b] + i] (kv_start NULL = 0) of K/V batch kv_row[b] (NULL = b; kv_rows = batches the K/V views span).
- * q_len [B] (NULL = Nq): batch b's real query rows; keys at or past q_off[b] + q_len[b] are never read into any output, so
- * they may hold anything.  Views and strides as emu_op_attn_prefill (st12: q, k, v, out batch / token / head strides in
- * elements).  D = 64 or 128. */
-int emu_op_attn_prefill_offset(const void* q, const void* k, const void* v, void* out, int B, int H, int Nq, int Nk, int D,
-                               const int64_t* st12, float scale, const int32_t* q_off, const int32_t* q_len,
-                               const int32_t* kv_start, const int32_t* kv_row, int kv_rows, emu_stream_t s);
+/* ---- the kernel behind emu_llm_copy_prefix as a stand-alone operator (device pointers) ---- */
 
 /* Positions [0, P) of cache row src -> row dst in every plane of a bf16 cache [outer][rows][H][t_max][D]. */
 int emu_op_kv_prefix_copy(void* cache, int outer, int rows, int H, int D, int t_max, int src, int dst, int P, emu_stream_t s);

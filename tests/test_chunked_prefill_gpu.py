@@ -72,26 +72,32 @@ def _rot(x, c, s_):
     return torch.stack([lo, hi], -1).flatten(-2)
 
 
-@pytest.mark.parametrize("D", [64, 128])
-def test_packed_rope_kv_write_matches_a_torch_restatement(cuda, D):
+# B = 0: a join or an extend, segments only, each at its own cache row, first slot and position offset
+@pytest.mark.parametrize("D,B", [(64, 4), (128, 4), (64, 0), (128, 0)], ids=["64", "128", "segments64", "segments128"])
+def test_packed_rope_kv_write_matches_a_torch_restatement(cuda, D, B):
     """decode rows rotated at pos - pos_off, q compact, k / v written only for live rows; segment rows rotated at q0 + j -
     posoff, q in place, k / v at their slots; rows past the last segment and every other cache position untouched"""
     from emu_b200 import _lib
-    g = torch.Generator().manual_seed(D)
+    g = torch.Generator().manual_seed(D if B else D + 1)
     H, T, rows = 2, 64, 6
     half, max_pos = D // 2, T + 8
     ang = torch.arange(max_pos)[:, None].float() / (10000 ** (torch.arange(half).float() * 2 / D))
     cos, sin = ang.cos().to(torch.bfloat16), ang.sin().to(torch.bfloat16)
-    B, pos, pos_off, active = 4, [12, 30, 7, 20], [0, 3, 0, 5], [1, 0, 1, 0]     # rows 1 and 3 are not live
-    seg_row, seg_q0, seg_new, seg_posoff = [1, 5, 3], [30, 0, 20], [5, 1, 9], [3, 0, 2]
+    if B:
+        pos, pos_off, active = [12, 30, 7, 20], [0, 3, 0, 5], [1, 0, 1, 0]        # rows 1 and 3 are not live
+        seg_row, seg_q0, seg_new, seg_posoff = [1, 5, 3], [30, 0, 20], [5, 1, 9], [3, 0, 2]
+    else:
+        pos = pos_off = active = []
+        seg_row, seg_q0, seg_new, seg_posoff = [4, 1, 2], [10, 0, 40], [9, 1, 5], [2, 0, 7]
     M = B + sum(seg_new) + 2                                                      # two rows past the last segment
     qkv = torch.randn(M, 3 * H * D, generator=g).to(torch.bfloat16)
     kc = torch.randn(rows, H, T, D, generator=g).to(torch.bfloat16)
     vc = torch.randn(rows, H, T, D, generator=g).to(torch.bfloat16)
     q_out = torch.zeros(B, H * D, dtype=torch.bfloat16)
     got_q, got_k, got_v, got_o = qkv.cuda(), kc.cuda(), vc.cuda(), q_out.cuda()
-    _lib.op_rope_kv_write_packed(got_q, H, D, cos.cuda(), sin.cuda(), got_k, got_v, B, _i32(pos), _i32(pos_off), _i32(active),
-                                 got_o, _i32(seg_row), _i32(seg_q0), _i32(seg_new), _i32(seg_posoff))
+    dec = (_i32(pos), _i32(pos_off), _i32(active), got_o) if B else (None, None, None, None)
+    _lib.op_rope_kv_write_packed(got_q, H, D, cos.cuda(), sin.cuda(), got_k, got_v, B, *dec, _i32(seg_row), _i32(seg_q0),
+                                 _i32(seg_new), _i32(seg_posoff))
     want_q, want_k, want_v, want_o = qkv.clone(), kc.clone(), vc.clone(), q_out.clone()
     for b in range(B):
         p = pos[b]
@@ -125,11 +131,13 @@ def _attn_ref(q, k, v, q_off, kv_start, scale):
     return torch.einsum("hqk,khd->qhd", torch.softmax(s, -1).nan_to_num(), v.float())
 
 
-@pytest.mark.parametrize("lens", [(1, 7, 64), (129, 1, 7, 64)], ids=["mma", "wgmma"])
+# NqX: segments of X, X - 3 and X / 2 queries (a join or an extend's suffixes); below 128 queries the mma.sync kernel runs
+@pytest.mark.parametrize("lens", [(1, 7, 64), (129, 1, 7, 64), (7, 4, 3), (64, 61, 32), (129, 126, 64), (200, 197, 100)],
+                         ids=["mma", "wgmma", "Nq7", "Nq64", "Nq129", "Nq200"])
 @pytest.mark.parametrize("D", [64, 128])
 def test_packed_attention_matches_torch(cuda, lens, D):
-    """segments of 1 / 7 / 64 (and 129) queries packed with gaps between them into one q view; K/V read through kv_row with
-    NaN in every key at or past a segment's end; each segment's rows equal the reference, the gaps stay as they were"""
+    """segments packed with gaps between them into one q view at their own key offsets; K/V read through kv_row with NaN in
+    every key at or past a segment's end; each segment's rows equal the reference, the gaps stay as they were"""
     from emu_b200 import _lib
     g = torch.Generator().manual_seed(D + len(lens))
     H, rows = 4, 6

@@ -397,16 +397,10 @@ def test_prefix_header_symbols_are_bound_exported_and_disjoint(lib):
 def test_prefix_entry_points_refuse_null_arguments_without_a_gpu(lib):
     N = None
     one = (ctypes.c_int32 * 1)(0)
-    st = (ctypes.c_int64 * 12)(*([8] * 12))
     V = ctypes.c_void_p(16)
     for name, args in {"emu_llm_leave_keep": [(N, one, one, 1, N)],
                        "emu_llm_copy_prefix": [(N, 0, 1, 4, N)],
                        "emu_llm_extend": [(N, one, one, one, 1, V, 4, N, N)],
-                       "emu_op_rope_kv_write_rows": [(N, 1, 4, 2, 64, V, V, V, V, V, N, V, V, 16, N),
-                                                     (V, 1, 4, 2, 64, V, V, V, N, V, N, V, V, 16, N),
-                                                     (V, 1, 4, 2, 48, V, V, V, V, V, N, V, V, 16, N)],
-                       "emu_op_attn_prefill_offset": [(V, V, V, V, 1, 2, 4, 8, 64, st, ctypes.c_float(1.0), N, N, N, N, 0, N),
-                                                      (V, V, V, V, 1, 2, 4, 8, 96, st, ctypes.c_float(1.0), V, N, N, N, 0, N)],
                        "emu_op_kv_prefix_copy": [(N, 2, 4, 2, 64, 16, 0, 1, 4, N), (V, 2, 4, 2, 64, 16, 1, 1, 4, N),
                                                  (V, 2, 4, 2, 64, 16, 0, 1, 17, N),
                                                  (ctypes.c_void_p(24), 2, 4, 2, 64, 16, 0, 1, 4, N)],

@@ -3,7 +3,6 @@
 An extend from nothing must compute what a join computes; a join of a prefix plus an extend of the suffix must agree with the
 fp32 oracle on the whole prompt as closely as a bf16 run does; a kept prefix must not feel the decode steps of other slots;
 and the stand-alone kernels must match their torch restatements."""
-import math
 
 import pytest
 import torch
@@ -206,86 +205,6 @@ def test_prefix_copy_equals_a_slice_copy(cuda):
         want[:, dst, :, :P] = want[:, src, :, :P]
         _lib.op_kv_prefix_copy(cache, src, dst, P)
         assert torch.equal(cache, want)
-
-
-def _attn_ref(q, k, v, q_off, kv_start, scale):
-    B, Nq, H, D = q.shape
-    out = torch.empty(B, Nq, H, D)
-    for b in range(B):
-        kk, vv = k[b].float(), v[b].float()
-        s = torch.einsum("qhd,khd->hqk", q[b].float(), kk) * scale
-        i = torch.arange(Nq)[:, None] + int(q_off[b])
-        j = torch.arange(k.shape[1])[None, :]
-        s = s.masked_fill((j > i) | (j < int(kv_start[b])), float("-inf"))
-        out[b] = torch.einsum("hqk,khd->qhd", torch.softmax(s, -1).nan_to_num(), vv)
-    return out
-
-
-@pytest.mark.parametrize("Nq", [7, 64, 129, 200], ids=lambda n: "Nq%d" % n)
-@pytest.mark.parametrize("D", [64, 128])
-def test_offset_attention_matches_torch(cuda, Nq, D):
-    """query batches read K/V rows through kv_row (as the engine's extend does), with fewer real query rows than Nq; every
-    key at or past a row's end is NaN, and the real rows' outputs stay finite and equal to the reference"""
-    from emu_b200 import _lib
-    g = torch.Generator().manual_seed(Nq + D)
-    B, H, rows = 3, 4, 5
-    q_off = torch.tensor([0, 50, 131], dtype=torch.int32)
-    q_len = torch.tensor([Nq, max(1, Nq - 3), max(1, Nq // 2)], dtype=torch.int32)
-    kv_start = torch.tensor([0, 3, 17], dtype=torch.int32)
-    kv_row = torch.tensor([4, 0, 2], dtype=torch.int32)
-    Nk = int(q_off.max()) + Nq
-    q = torch.randn(B, Nq, H, D, generator=g).to(torch.bfloat16)
-    k = torch.randn(rows, Nk, H, D, generator=g).to(torch.bfloat16)
-    v = torch.randn(rows, Nk, H, D, generator=g).to(torch.bfloat16)
-    for b in range(B):
-        end = int(q_off[b] + q_len[b])
-        k[kv_row[b], end:] = float("nan")
-        v[kv_row[b], end:] = float("nan")
-    scale = 1 / math.sqrt(D)
-    got = _lib.op_attn_prefill_offset(q.cuda(), k.cuda(), v.cuda(), scale, q_off.cuda(), kv_start.cuda(), kv_row.cuda(),
-                                      q_len.cuda()).float().cpu()
-    # the reference sees zeros where the engine must not look (its own P·V would turn 0 · NaN into NaN)
-    want = _attn_ref(q, k[kv_row.long()].nan_to_num(0.0), v[kv_row.long()].nan_to_num(0.0), q_off, kv_start, scale)
-    for b in range(B):
-        n = int(q_len[b])
-        assert torch.isfinite(got[b, :n]).all(), b
-        err = (got[b, :n] - want[b, :n]).abs().max().item()
-        assert err < 2e-2, (b, err)
-
-
-def test_row_rope_kv_write_matches_a_torch_restatement(cuda):
-    """q / k pairs (2j, 2j + 1) rotated at cache slot q0[b] + n minus pos_off[b], each product rounded to bf16 before the sum
-    (HF's bf16 rotate-half); k / v written to row kv_row[b], nothing written or rotated past n_new[b]"""
-    from emu_b200 import _lib
-    g = torch.Generator().manual_seed(3)
-    B, N, H, D, T = 3, 9, 2, 128, 64
-    half, max_pos = D // 2, T + 8
-    ang = torch.arange(max_pos)[:, None].float() / (10000 ** (torch.arange(half).float() * 2 / D))
-    cos, sin = ang.cos().to(torch.bfloat16), ang.sin().to(torch.bfloat16)
-    qkv = torch.randn(B, N, 3 * H * D, generator=g).to(torch.bfloat16)
-    kc = torch.randn(5, H, T, D, generator=g).to(torch.bfloat16)
-    vc = torch.randn(5, H, T, D, generator=g).to(torch.bfloat16)
-    q0, n_new, pos_off, rows = [10, 0, 40], [9, 1, 5], [2, 0, 7], [4, 1, 2]
-    i32 = lambda x: torch.tensor(x, dtype=torch.int32, device="cuda")
-    got_q, got_k, got_v = qkv.cuda(), kc.cuda(), vc.cuda()
-    _lib.op_rope_kv_write_rows(got_q, H, D, cos.cuda(), sin.cuda(), got_k, got_v, i32(pos_off), i32(q0), i32(n_new), i32(rows))
-
-    def rot(x, c, s_):                       # x [..., D] pair-interleaved
-        a, b = x[..., 0::2].float(), x[..., 1::2].float()
-        r = lambda t: t.to(torch.bfloat16).float()
-        lo, hi = (r(a * c) + r(-b * s_)).to(torch.bfloat16), (r(b * c) + r(a * s_)).to(torch.bfloat16)
-        return torch.stack([lo, hi], -1).flatten(-2)
-    want_q, want_k, want_v = qkv.clone(), kc.clone(), vc.clone()
-    for b in range(B):
-        for n in range(n_new[b]):
-            p = q0[b] + n
-            c, s_ = cos[p - pos_off[b]].float(), sin[p - pos_off[b]].float()
-            t = qkv[b, n].view(3, H, D)
-            want_q[b, n, :H * D] = rot(t[0], c, s_).flatten()
-            want_k[rows[b], :, p] = rot(t[1], c, s_)
-            want_v[rows[b], :, p] = t[2]
-    assert torch.equal(got_k.cpu(), want_k) and torch.equal(got_v.cpu(), want_v)
-    assert torch.equal(got_q.cpu(), want_q)                     # the padding rows are left alone
 
 
 # ---- one real LLaMA-33B layer ----
