@@ -85,6 +85,8 @@ PREFIX_SYMBOLS = ["emu_llm_leave_keep", "emu_llm_slot_kept", "emu_llm_copy_prefi
                   "emu_op_kv_prefix_copy"]
 # ... and in include/emu_b200_chunked.h (chunked prefill: the mixed decode + prefill step and its kernels)
 CHUNKED_SYMBOLS = ["emu_llm_step", "emu_op_rope_kv_write_packed", "emu_op_attn_prefill_packed"]
+# ... and in include/emu_b200_regress.h (regression slots: Emu2-Gen's prompt encoding for every slot at once)
+REGRESS_SYMBOLS = ["emu_llm_regress_join", "emu_llm_regress_step"]
 # ... and in include/emu_b200_gen_slots.h (latent slots: continuous batching for image generation)
 GEN_SLOT_SYMBOLS = ["emu_denoise_step_slots", "emu_op_denoise_prepare", "emu_op_denoise_euler"]
 # ... and in include/emu_b200_diffusion_ops.h (the diffusion kernels as stand-alone operators)
@@ -350,6 +352,36 @@ class Engine:
                                     _ptr(logits) if B else None, hs, hp, hn, hf, cnt, _ptr(embeds), _ptr(last), _stream()),
               self.h)
         return last
+
+    # ---- regression slots (include/emu_b200_regress.h) ----
+    def _regress_out(self, name, out, rows):
+        # the C entry points take a bare pointer: a short buffer would be written past its end
+        if out.dtype != torch.bfloat16 or out.dim() != 3 or not out.is_contiguous() or out.shape[0] < rows \
+                or out.shape[2] != self.cfg.vit_width:
+            raise ValueError("%s: out must be a contiguous bf16 [>= %d, L, %d] tensor, got %s %s"
+                             % (name, rows, self.cfg.vit_width, tuple(out.shape), out.dtype))
+
+    def regress_join(self, slots, new, embeds, out):
+        """prefill len(slots) prompts into the free slots, packed back to back in embeds [sum(new), hidden] (prompt i has
+        new[i] tokens, no padding); each slot becomes a live regression slot with its embedding 0 in out[slot][0]
+        (out [n_slots, L, width] bf16, the other rows untouched)"""
+        if len(new) != len(slots):
+            raise ValueError("regress_join: %d token counts for %d slots" % (len(new), len(slots)))
+        embeds = embeds.to(torch.bfloat16).contiguous()
+        if embeds.dim() != 2 or embeds.shape[0] != sum(int(k) for k in new) or embeds.shape[1] != self.cfg.llm_hidden:
+            raise ValueError("regress_join: embeds must be [sum(new) = %d, %d], got %s"
+                             % (sum(int(k) for k in new), self.cfg.llm_hidden, tuple(embeds.shape)))
+        self._regress_out("regress_join", out, max(int(s) for s in slots) + 1 if slots else 0)
+        hs, cnt = self._host_slots(slots)
+        hn, _ = self._host_slots(new)
+        check(self.lib.emu_llm_regress_join(self.h, hs, hn, cnt, _ptr(embeds), _ptr(out), int(out.shape[1]), _stream()),
+              self.h)
+
+    def regress_step(self, B, out):
+        """one regression step of every live slot below B: its next embedding goes to out[slot][k] (out as in regress_join;
+        one CUDA graph per (B, out))"""
+        self._regress_out("regress_step", out, int(B))
+        check(self.lib.emu_llm_regress_step(self.h, int(B), _ptr(out), int(out.shape[1]), _stream()), self.h)
 
     def sample_tokens(self, logits, temperature=1.0, top_k=0, top_p=1.0, ban_id=-1, seed=0, offset=0):
         return op_sample_tokens(logits, temperature, top_k, top_p, -1 if ban_id is None else ban_id, seed, offset)

@@ -739,6 +739,9 @@ class ImageRequest:
         # set at admission
         self.slot = None
         self.step = 0
+        self.regressing = False     # encode_steps: its prompt is in its LLaMA regression slot (the slot index is the same)
+        self.n_regressed = 0        # ... its embeddings regressed so far
+        self.encoded = None         # the prompt embeddings [cond; uncond] (or [cond]) its latent slot was conditioned with
 
 
 class DenoiseSlotScheduler(_RequestQueue):
@@ -755,9 +758,19 @@ class DenoiseSlotScheduler(_RequestQueue):
     A request that fails answers with its own error and frees its slot; the others continue.  Each request's latents are the
     ones `denoise` gives it alone (bitwise while the UNet's row count 2B stays within the GEMV path of its small linears, 8).
     height / width are fixed per scheduler: the buffers, and the CUDA graph of each B, are made for one latent size.
-    Owns the pipeline's engine while it lives.  Single-threaded: `submit` may be called from any thread, `step` from one."""
+    Owns the pipeline's engine while it lives.  Single-threaded: `submit` may be called from any thread, `step` from one.
 
-    def __init__(self, pipeline, n_slots=4, height=1024, width=1024, n_tokens=None):
+    Regression slots (`encode_steps=R`, opt-in): a generation-mode request's prompt is encoded in the engine's LLaMA slot mode
+    (include/emu_b200_regress.h) instead of by one generate_image call while every live slot waits.  Its latent slot index is
+    also its LLaMA slot, so n_slots <= llm_max_batch, and every regression step runs at B = n_slots.  Admission runs the ViT
+    for the newcomers' pictures, embeds their prompts (EmuModel.image_prompt_ids / image_prompt_embeds, as generate_image) and
+    prefills all of them in ONE emu_llm_regress_join; then each step() runs up to R emu_llm_regress_step while any prompt is
+    regressing.  A request whose L embeddings are done leaves its LLaMA slot, is conditioned ([cond; cached uncond]) into its
+    latent slot and denoises from that step's UNet step on.  Requests with prompt_embeds and autoencoding-mode requests
+    (pictures only) are encoded at admission as before.  A request's embeddings are those of its prompt regressed alone in the
+    same slot of a pool of the same size, bit for bit, and its image is the one it gets from this scheduler alone."""
+
+    def __init__(self, pipeline, n_slots=4, height=1024, width=1024, n_tokens=None, encode_steps=None):
         super().__init__()
         self.pipe, self.engine = pipeline, pipeline.engine
         self.n_slots = int(n_slots)
@@ -786,9 +799,30 @@ class DenoiseSlotScheduler(_RequestQueue):
         self.owner = [None] * n
         self.steps = 0
         self.batch_sizes = collections.deque(maxlen=1024)   # B of the recent UNet steps (observability; the tests read it)
+        self.encode_steps = None if encode_steps is None else int(encode_steps)
+        self.regress_steps = 0                              # encode_steps: regression steps run, and the recent joins' sizes
+        self.join_sizes = collections.deque(maxlen=1024)
+        if self.encode_steps is not None:
+            self._begin_regression(n)
         # every workspace at its largest size now: a later growth would drop every captured graph
         with _on_device(dev):
             self._unet_step(n)
+
+    def _begin_regression(self, n):
+        if self.encode_steps < 1:
+            raise ValueError("encode_steps must be >= 1, got %d" % self.encode_steps)
+        enc, cfg = self.pipe.multimodal_encoder, self.engine.cfg
+        if n > cfg.llm_max_batch:
+            raise ValueError("encode_steps: the %d latent slots are LLaMA slots too, at most llm_max_batch = %d"
+                             % (n, cfg.llm_max_batch))
+        if self.L != enc.n_query:
+            raise ValueError("encode_steps: the encoder regresses %d embeddings, the slots hold %d" % (enc.n_query, self.L))
+        self.max_seq = int(cfg.llm_max_seq)
+        self.embeds = torch.zeros(n, self.L, self.ctx.shape[2], dtype=torch.bfloat16, device=self.device)
+        with _on_device(self.device):
+            # generate_image resets the LLM (it leaves slot mode): the unconditional branch is made first, once
+            self.uncond = self.pipe._unconditional("", lambda: enc.generate_image(text=[""]))
+            self.engine.slots_begin(n)
 
     # ---- producer side ----
     def submit(self, request: ImageRequest):
@@ -797,18 +831,38 @@ class DenoiseSlotScheduler(_RequestQueue):
         if (request.height, request.width) != (self.height, self.width):
             raise ValueError("this scheduler generates %dx%d images; a %dx%d request needs a scheduler of its own size"
                              % (self.width, self.height, request.width, request.height))
+        text = self._pool_text(request)
+        if text is not None:                                # the prompt and L - 1 regressed positions must fit a slot
+            n = self.pipe.multimodal_encoder.image_prompt_ids([text])[0].shape[1]
+            if n + self.L - 1 > self.max_seq:
+                raise ValueError("prompt of %d tokens and %d regressed embeddings exceed llm_max_seq = %d"
+                                 % (n, self.L, self.max_seq))
         return super().submit(request)
 
     def _live(self):
         return [r for r in self.owner if r is not None]
 
+    def _denoising(self):
+        return [r for r in self.owner if r is not None and not r.regressing]
+
+    def _pool_text(self, r):
+        """encode_steps: the text of r's generation-mode prompt, which regression slots encode; None for a request that is
+        encoded at admission (prompt_embeds, autoencoding mode, or encode_steps unset)"""
+        if self.encode_steps is None or r.prompt_embeds is not None:
+            return None
+        from .emu2.constants import DEFAULT_IMG_PLACEHOLDER
+        text, pictures, saw_text = self.pipe._prompt_text(r.inputs, DEFAULT_IMG_PLACEHOLDER)
+        return None if pictures and not saw_text else text
+
     # ---- one iteration ----
     @torch.no_grad()
     def step(self):
-        """admit -> step -> retire (class docstring); returns the requests finished in this step"""
+        """admit -> (regress) -> step -> retire (class docstring); returns the requests finished in this step"""
         with _on_device(self.device):
             self._admit()
-            live = self._live()
+            if self.encode_steps is not None:
+                self._regress()
+            live = self._denoising()
             if not live:
                 return []
             try:
@@ -828,24 +882,35 @@ class DenoiseSlotScheduler(_RequestQueue):
             return finished
 
     def _admit(self):
+        pool = []
         while True:
             with self._lock:
                 if not self.waiting or None not in self.owner:
-                    return
+                    break
                 r = self.waiting.popleft()
                 r.slot = self.owner.index(None)
                 self.owner[r.slot] = r
             try:
-                self._fill_slot(r)
+                text = self._pool_text(r)
+                if text is None:
+                    self._fill_slot(r)
+                else:
+                    pool.append((r, self._pool_prompt(r, text)))
             except Exception as ex:         # a prompt that cannot be encoded fails on its own
                 self._fail(r, ex)
+        if pool:
+            self._regress_join(pool)
 
     def _fill_slot(self, r):
-        pipe, s = self.pipe, r.slot
-        cfg = r.guidance > 1.0
         pe = r.prompt_embeds
         if pe is None:
-            pe = pipe._prepare_and_encode_inputs(r.inputs, cfg)
+            pe = self.pipe._prepare_and_encode_inputs(r.inputs, r.guidance > 1.0)
+        self._condition(r, pe)
+
+    def _condition(self, r, pe):
+        """r's latent slot from its prompt embeddings pe [2 or 1, L, Cc]: conditioning rows, schedule, initial latents"""
+        pipe, s = self.pipe, r.slot
+        cfg = r.guidance > 1.0
         pe = pe.to(self.device, torch.bfloat16)
         if pe.dim() != 3 or pe.shape[0] != (2 if cfg else 1) or tuple(pe.shape[1:]) != tuple(self.ctx.shape[1:]):
             raise ValueError("prompt embeddings of shape %s do not fit a slot: expected [%d, %d, %d]"
@@ -859,12 +924,80 @@ class DenoiseSlotScheduler(_RequestQueue):
         self.time_ids[2 * s], self.time_ids[2 * s + 1] = tid[0], tid[u]
         self.latents[s] = lat[0]
         r.timesteps, r.sigmas = [float(t) for t in ts], [float(v) for v in sig]
+        r.encoded = pe
+
+    # ---- regression slots (encode_steps) ----
+    def _pool_prompt(self, r, text):
+        """r's prompt as generate_image builds it: tokenised with [IMG] appended, its pictures through the ViT, spliced ->
+        embeddings [N, hidden]"""
+        from .emu2.constants import DEFAULT_IMG_PLACEHOLDER
+        enc = self.pipe.multimodal_encoder
+        _, pictures, _ = self.pipe._split_prompt(r.inputs, DEFAULT_IMG_PLACEHOLDER)
+        ids, mask, image_id = enc.image_prompt_ids([text])
+        return enc.image_prompt_embeds(ids, pictures, image_id)[0]
+
+    def _regress_join(self, items):
+        """ONE emu_llm_regress_join for the newcomers (two when some prompts are shorter than 128 tokens and some are not: the
+        prefill attention kernel is picked by a join's longest prompt, so each prompt joins with its own kind and keeps its
+        bits); if a join fails, its prompts join one by one, so that only the culprit fails"""
+        for group in ([it for it in items if it[1].shape[0] < 128], [it for it in items if it[1].shape[0] >= 128]):
+            if not group:
+                continue
+            try:
+                self._join(group)
+            except Exception as ex:
+                if len(group) == 1:
+                    self._fail(group[0][0], ex)
+                    continue
+                for item in group:
+                    try:
+                        self._join([item])
+                    except Exception as ex1:
+                        self._fail(item[0], ex1)
+
+    def _join(self, items):
+        self.engine.regress_join([r.slot for r, _ in items], [e.shape[0] for _, e in items], torch.cat([e for _, e in items]),
+                                 self.embeds)
+        self.join_sizes.append(len(items))
+        for r, _ in items:
+            r.regressing, r.n_regressed = True, 1
+        for r, _ in items:
+            if r.n_regressed == self.L:
+                self._regressed(r)
+
+    def _regress(self):
+        """up to encode_steps regression steps while any prompt is regressing; a finished prompt conditions its latent slot"""
+        for _ in range(self.encode_steps):
+            busy = [r for r in self.owner if r is not None and r.regressing]
+            if not busy:
+                return
+            try:
+                self.engine.regress_step(self.n_slots, self.embeds)
+            except Exception as ex:        # the prompts in the step fail, the scheduler stays usable
+                for r in busy:
+                    self._fail(r, ex)
+                return
+            self.regress_steps += 1
+            for r in busy:
+                r.n_regressed += 1
+                if r.n_regressed == self.L:
+                    self._regressed(r)
+
+    def _regressed(self, r):
+        """r's L embeddings are done: it leaves its LLaMA slot and its latent slot is conditioned"""
+        r.regressing = False
+        try:
+            self.engine.leave([r.slot])
+            cond = self.embeds[r.slot:r.slot + 1].clone()
+            self._condition(r, torch.cat([cond, self.uncond.to(self.device, torch.bfloat16)]) if r.guidance > 1.0 else cond)
+        except Exception as ex:
+            self._fail(r, ex)
 
     def _unet_step(self, B):
         if self._copied is not None:
             self._copied.synchronize()       # the staging buffer is rewritten only after its last copy has run
         self._stage.zero_()
-        for r in self._live():
+        for r in self._denoising():
             i = r.step
             self._stage_params[r.slot] = torch.tensor([r.sigmas[i], r.sigmas[i + 1], r.timesteps[i], r.guidance])
             self._stage_live[r.slot] = 1
@@ -888,3 +1021,9 @@ class DenoiseSlotScheduler(_RequestQueue):
     def _release(self, r):
         if r.slot is not None and self.owner[r.slot] is r:
             self.owner[r.slot] = None
+            if r.regressing:                 # its LLaMA slot is the same index
+                r.regressing = False
+                try:
+                    self.engine.leave([r.slot])
+                except Exception:
+                    pass

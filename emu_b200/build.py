@@ -28,7 +28,8 @@ def _digest():
     for f in sorted(os.listdir(CSRC)) + ["../../include/emu_b200.h", "../../include/emu_b200_safety.h",
                                         "../../include/emu_b200_slots.h", "../../include/emu_b200_ops.h",
                                         "../../include/emu_b200_gen_slots.h", "../../include/emu_b200_diffusion_ops.h",
-                                        "../../include/emu_b200_prefix.h", "../../include/emu_b200_chunked.h"]:
+                                        "../../include/emu_b200_prefix.h", "../../include/emu_b200_chunked.h",
+                                        "../../include/emu_b200_regress.h"]:
         p = os.path.join(CSRC, f)
         if os.path.isfile(p):
             h.update(f.encode())

@@ -8,6 +8,7 @@
 #include "engine.h"
 #include "../../include/emu_b200_chunked.h"
 #include "../../include/emu_b200_prefix.h"
+#include "../../include/emu_b200_regress.h"
 #include "../../include/emu_b200_slots.h"
 
 #include <dlfcn.h>
@@ -185,6 +186,33 @@ __global__ void gather_rows_kernel(const bf16* __restrict__ h, int Hd, const int
   const uint4* src = reinterpret_cast<const uint4*>(h + (long)idx[b] * Hd);
   uint4* dst = reinterpret_cast<uint4*>(out + (long)b * Hd);
   for (int i = threadIdx.x; i < Hd / 8; i += blockDim.x) dst[i] = src[i];
+}
+// regression join: the last packed row of segment b (rows row0[b] .. row0[b] + n_new[b] - 1 of h) -> row slot[b] of out
+__global__ void gather_last_to_slot_kernel(const bf16* __restrict__ h, int Hd, const int* __restrict__ slot,
+                                           const int* __restrict__ n_new, const int* __restrict__ row0, bf16* out) {
+  const int b = blockIdx.x;
+  const uint4* src = reinterpret_cast<const uint4*>(h + (long)(row0[b] + n_new[b] - 1) * Hd);
+  uint4* dst = reinterpret_cast<uint4*>(out + (long)slot[b] * Hd);
+  for (int i = threadIdx.x; i < Hd / 8; i += blockDim.x) dst[i] = src[i];
+}
+// regression slots: the projected row r[s] [w] of slot s becomes its feedback fb[s] and, while k[s] < L, its output row
+// out[s][k[s]]; then k[s] += 1 (at most L).  One CTA per slot: CTA b is slot join.r[b] starting from k = 0 (a join of n_join
+// slots), or, with n_join = 0, slot b if active[b] (a step; the rows of the other slots are dropped).  w % 8 == 0.
+__global__ void regress_emit_kernel(const bf16* __restrict__ r, bf16* fb, int* k, bf16* out, int L, int w, SlotList join,
+                                    int n_join, const int* __restrict__ active) {
+  const int s = n_join ? join.r[blockIdx.x] : blockIdx.x;
+  if (!n_join && !active[s]) return;
+  const int kk = n_join ? 0 : k[s];
+  const uint4* src = reinterpret_cast<const uint4*>(r + (long)s * w);
+  uint4* f = reinterpret_cast<uint4*>(fb + (long)s * w);
+  uint4* o = reinterpret_cast<uint4*>(out + ((long)s * L + kk) * w);
+  for (int i = threadIdx.x; i < w / 8; i += blockDim.x) {
+    const uint4 v = src[i];
+    f[i] = v;
+    if (kk < L) o[i] = v;
+  }
+  __syncthreads();  // every thread has read k[s]
+  if (threadIdx.x == 0) k[s] = kk < L ? kk + 1 : L;
 }
 __global__ void argmax_ban_kernel(float* logits, int cols, int ban) {
   if (ban >= 0 && ban < cols) logits[(long)blockIdx.x * cols + ban] = -INFINITY;
@@ -882,14 +910,12 @@ extern "C" int emu_llm_embed(EmuEngine* e, const int32_t* ids, int n, void* out,
   return embed_gather(e->embed, ids, (bf16*)out, n, e->cfg.llm_hidden, (cudaStream_t)s);
 }
 
-extern "C" int emu_project(EmuEngine* e, int which, const void* x, int M, void* y, emu_stream_t s) {
-  if (!e || !x || !y || M < 1) return EMU_ERR_INVALID;
+// y [M, out] = x [M, in] W^T of projection `which` (0 project_up, 1 project_down, 2 the student head; its weight loaded):
+// the GEMV up to 8 rows, the GEMM above
+static int project_rows(EmuEngine* e, int which, const void* x, int M, void* y, cudaStream_t st) {
   const bf16* W = which == 0 ? e->proj_up : (which == 1 ? e->proj_down : e->stu_head);
   const int in = which == 0 ? e->proj_up_in : (which == 1 ? e->proj_down_in : e->stu_in);
   const int out = which == 0 ? e->proj_up_out : (which == 1 ? e->proj_down_out : e->stu_out);
-  if (!W) return e->fail(EMU_ERR_STATE, "projection weight missing");
-  cudaStream_t st = (cudaStream_t)s;
-  count_launch();
   if (M <= 8 && in % 32 == 0) {
     GemvArgs a;
     a.W = W; a.N = out; a.K = in; a.x = (const bf16*)x; a.ldx = in; a.B = M; a.y = y; a.ldy = out;
@@ -898,6 +924,14 @@ extern "C" int emu_project(EmuEngine* e, int which, const void* x, int M, void* 
   GemmEpilogue ep;
   ep.C = y; ep.ldc = out;
   return gemm_bf16((const bf16*)x, in, W, in, M, out, in, ep, st);
+}
+
+extern "C" int emu_project(EmuEngine* e, int which, const void* x, int M, void* y, emu_stream_t s) {
+  if (!e || !x || !y || M < 1) return EMU_ERR_INVALID;
+  if (!(which == 0 ? e->proj_up : (which == 1 ? e->proj_down : e->stu_head)))
+    return e->fail(EMU_ERR_STATE, "projection weight missing");
+  count_launch();
+  return project_rows(e, which, x, M, y, (cudaStream_t)s);
 }
 
 // prefill workspaces for M prompt tokens; the embeddings go to pf_h (null: the caller stages them)
@@ -1368,6 +1402,52 @@ static int check_decode_rows(EmuEngine* e, int B, const std::string& none_live) 
   return EMU_OK;
 }
 
+// launch body(stream, &n_launches) — a fixed launch sequence — on st as the CUDA graph cached under key (captured on first use),
+// or eagerly with EMU_NO_GRAPH=1 (debugging / parity switch) or without graphs
+template <class Body>
+static int run_graphed(EmuEngine* e, const EmuEngine::GraphKey& key, cudaStream_t st, Body body) {
+  int nl = 0;
+  const char* no_graph = getenv("EMU_NO_GRAPH");
+  const bool graphable = e->use_graphs && !(no_graph && no_graph[0] == '1');  // NCCL collectives are graph-capturable
+  if (!graphable) {
+    EMU_TRY(body(st, &nl));
+    count_launch(nl);
+    return EMU_OK;
+  }
+  auto it = e->graphs.find(key);
+  if (it == e->graphs.end()) {
+    if (e->graphs.size() > 64) {
+      for (auto& g : e->graphs) cudaGraphExecDestroy(g.second);
+      e->graphs.clear();
+      e->graph_nodes.clear();
+    }
+    // capture on an engine-owned stream: the caller's stream may be the legacy default stream, which cannot
+    // be captured; the instantiated graph is then launched on the caller's stream
+    if (!e->cap_stream && cudaStreamCreateWithFlags(&e->cap_stream, cudaStreamNonBlocking) != cudaSuccess)
+      return e->fail(EMU_ERR_CUDA, "capture stream create failed");
+    if (cudaStreamBeginCapture(e->cap_stream, cudaStreamCaptureModeRelaxed) != cudaSuccess)
+      return e->fail(EMU_ERR_CUDA, std::string("graph capture begin failed: ") + cudaGetErrorString(cudaGetLastError()));
+    int rc = body(e->cap_stream, &nl);
+    cudaGraph_t graph = nullptr;
+    cudaError_t ce = cudaStreamEndCapture(e->cap_stream, &graph);
+    if (rc != EMU_OK || ce != cudaSuccess || !graph) {
+      if (graph) cudaGraphDestroy(graph);
+      cudaGetLastError();
+      return rc != EMU_OK ? rc : e->fail(EMU_ERR_CUDA, std::string("graph capture failed: ") + cudaGetErrorString(ce));
+    }
+    cudaGraphExec_t exec = nullptr;
+    ce = cudaGraphInstantiate(&exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (ce != cudaSuccess) return e->fail(EMU_ERR_CUDA, std::string("graph instantiate failed: ") + cudaGetErrorString(ce));
+    e->graphs[key] = exec;
+    e->graph_nodes[key] = nl;
+    it = e->graphs.find(key);
+  }
+  if (cudaGraphLaunch(it->second, st) != cudaSuccess) return e->fail(EMU_ERR_CUDA, "graph launch failed");
+  count_launch(e->graph_nodes[key]);
+  return EMU_OK;
+}
+
 extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void* embeds, const int32_t* beam_src_idx,
                               int B, float* logits, void* hidden, int32_t* next_ids, int ban_id, emu_stream_t stream) {
   if (!e || B < 1 || ((token_ids == nullptr) == (embeds == nullptr))) return EMU_ERR_INVALID;
@@ -1385,46 +1465,11 @@ extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void
     EMU_TRY(kv_reparent(e, beam_src_idx, B, st));
     count_launch();
   }
-  int nl = 0;
-  const char* no_graph = getenv("EMU_NO_GRAPH");  // debugging / parity switch: launch the step eagerly
-  const bool graphable = e->use_graphs && !(no_graph && no_graph[0] == '1');  // NCCL collectives are graph-capturable
-  if (!graphable) {
-    EMU_TRY(decode_step_body(e, token_ids, embeds, B, logits, hidden, next_ids, ban_id, st, &nl));
-    count_launch(nl);
-  } else {
-    EmuEngine::GraphKey key(B, token_ids, embeds, logits, hidden, next_ids, (const void*)st, ban_id, e->n_slots > 0 ? 1 : 0);
-    auto it = e->graphs.find(key);
-    if (it == e->graphs.end()) {
-      if (e->graphs.size() > 64) {
-        for (auto& g : e->graphs) cudaGraphExecDestroy(g.second);
-        e->graphs.clear();
-        e->graph_nodes.clear();
-      }
-      // capture on an engine-owned stream: the caller's stream may be the legacy default stream, which cannot
-      // be captured; the instantiated graph is then launched on the caller's stream
-      if (!e->cap_stream && cudaStreamCreateWithFlags(&e->cap_stream, cudaStreamNonBlocking) != cudaSuccess)
-        return e->fail(EMU_ERR_CUDA, "capture stream create failed");
-      if (cudaStreamBeginCapture(e->cap_stream, cudaStreamCaptureModeRelaxed) != cudaSuccess)
-        return e->fail(EMU_ERR_CUDA, std::string("graph capture begin failed: ") + cudaGetErrorString(cudaGetLastError()));
-      int rc = decode_step_body(e, token_ids, embeds, B, logits, hidden, next_ids, ban_id, e->cap_stream, &nl);
-      cudaGraph_t graph = nullptr;
-      cudaError_t ce = cudaStreamEndCapture(e->cap_stream, &graph);
-      if (rc != EMU_OK || ce != cudaSuccess || !graph) {
-        if (graph) cudaGraphDestroy(graph);
-        cudaGetLastError();
-        return rc != EMU_OK ? rc : e->fail(EMU_ERR_CUDA, std::string("graph capture failed: ") + cudaGetErrorString(ce));
-      }
-      cudaGraphExec_t exec = nullptr;
-      ce = cudaGraphInstantiate(&exec, graph, 0);
-      cudaGraphDestroy(graph);
-      if (ce != cudaSuccess) return e->fail(EMU_ERR_CUDA, std::string("graph instantiate failed: ") + cudaGetErrorString(ce));
-      e->graphs[key] = exec;
-      e->graph_nodes[key] = nl;
-      it = e->graphs.find(key);
-    }
-    if (cudaGraphLaunch(it->second, st) != cudaSuccess) return e->fail(EMU_ERR_CUDA, "graph launch failed");
-    count_launch(e->graph_nodes[key]);
-  }
+  EmuEngine::GraphKey key(B, token_ids, embeds, logits, hidden, next_ids, (const void*)st, ban_id, e->n_slots > 0 ? 1 : 0);
+  auto body = [&](cudaStream_t cs, int* nl) {
+    return decode_step_body(e, token_ids, embeds, B, logits, hidden, next_ids, ban_id, cs, nl);
+  };
+  EMU_TRY(run_graphed(e, key, st, body));
   if (e->n_slots > 0) {
     for (int b = 0; b < B; ++b) e->slots[b].advance();
   } else {
@@ -1486,9 +1531,11 @@ struct Segments {
 // Segment i's embeddings are rows [i * ld, i * ld + n_new[i]) of embeds (ld = 0: already packed).  mask [n, N], every segment
 // starting from nothing with N tokens: the left-pad starts and HF position offsets.  logits [B, vocab] of the decode rows
 // and logits_last [n, vocab] of each segment's last token, either may be null.  `what` names the call in a CUDA failure.
+// hidden_rows [n_slots, hidden] (or null): each segment's last row after the final norm, at row slot.r[i] (the rows of the
+// other slots are scratch: they are normed in place too).
 static int slot_prefill(EmuEngine* e, const int32_t* token_ids, const int32_t* beam_src_idx, int B, float* logits,
                         const Segments& sg, const void* embeds, int ld, const int32_t* mask, float* logits_last,
-                        const char* what, cudaStream_t st) {
+                        const char* what, cudaStream_t st, bf16* hidden_rows = nullptr) {
   const EmuConfig& c = e->cfg;
   const int Hd = c.llm_hidden, n = sg.n, K = kLlmMaxRows;
   int host_idx[6 * K];  // cache rows, prefixes, token counts, first packed rows, then the rows whose logits are read
@@ -1552,6 +1599,13 @@ static int slot_prefill(EmuEngine* e, const int32_t* token_ids, const int32_t* b
     Slot& s = e->slots[sg.slot.r[i]];
     if (sg.final_.r[i]) s.set_live(sg.slot.r[i], len.r[i]);
     else s.set_kept(len.r[i]);
+  }
+  if (hidden_rows) {  // row by row, as the prefill's last_hidden: a row's bits do not depend on the others
+    gather_last_to_slot_kernel<<<n, 128, 0, st>>>(h, Hd, m.seg_row, m.seg_new, m.seg_row0, hidden_rows);
+    count_launch();
+    if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, std::string(what) + ": last-row gather failed");
+    EMU_TRY(rmsnorm(hidden_rows, e->final_norm, hidden_rows, e->n_slots, Hd, c.llm_rms_eps, 0, st));
+    count_launch();
   }
   if (n_out == 0) return EMU_OK;
   // the rows' logits in one pass over lm_head, written straight to the one output asked for, or split to both
@@ -1768,4 +1822,95 @@ extern "C" int emu_llm_step(EmuEngine* e, const int32_t* token_ids, const int32_
     sg.final_.r[i] = f;
   }
   return slot_prefill(e, token_ids, beam_src_idx, B, logits, sg, embeds, 0, nullptr, logits_last, "mixed step", (cudaStream_t)stream);
+}
+
+// ================================================================================================
+// regression slots: Emu2-Gen's prompt encoding in slot mode (include/emu_b200_regress.h)
+// ================================================================================================
+// project_down and project_up chain hidden -> width -> hidden
+static int regress_ready(EmuEngine* e) {
+  const int Hd = e->cfg.llm_hidden;
+  if (!e->proj_up || !e->proj_down) return e->fail(EMU_ERR_STATE, "regression slots need the project_up and project_down weights");
+  if (e->proj_down_in != Hd || e->proj_up_out != Hd || e->proj_up_in != e->proj_down_out)
+    return e->fail(EMU_ERR_STATE, "project_down [" + std::to_string(e->proj_down_out) + ", " + std::to_string(e->proj_down_in) +
+                                      "] and project_up [" + std::to_string(e->proj_up_out) + ", " + std::to_string(e->proj_up_in) +
+                                      "] do not chain through hidden " + std::to_string(Hd));
+  if (e->proj_down_out % 8)
+    return e->fail(EMU_ERR_UNSUPPORTED, "regression width " + std::to_string(e->proj_down_out) + " is not a multiple of 8");
+  return EMU_OK;
+}
+
+// the regression buffers, allocated once at kLlmMaxRows rows so the pointers the step graphs bake in never change; zeroed
+static int regress_alloc(EmuEngine* e, cudaStream_t st) {
+  if (e->rg_fb) return EMU_OK;
+  const size_t K = kLlmMaxRows, wb = K * e->proj_down_out * 2, hb = K * e->cfg.llm_hidden * 2;
+  bf16 *fb = (bf16*)e->dmalloc(wb), *r = (bf16*)e->dmalloc(wb), *x = (bf16*)e->dmalloc(hb), *h = (bf16*)e->dmalloc(hb);
+  int* k = (int*)e->dmalloc(K * sizeof(int));
+  if (!fb || !r || !x || !h || !k) return e->fail(EMU_ERR_NOMEM, "regression buffers");
+  if (cudaMemsetAsync(fb, 0, wb, st) != cudaSuccess || cudaMemsetAsync(r, 0, wb, st) != cudaSuccess ||
+      cudaMemsetAsync(x, 0, hb, st) != cudaSuccess || cudaMemsetAsync(h, 0, hb, st) != cudaSuccess ||
+      cudaMemsetAsync(k, 0, K * sizeof(int), st) != cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "regression buffers reset failed");
+  e->rg_fb = fb; e->rg_r = r; e->rg_x = x; e->rg_h = h; e->rg_k = k;
+  return EMU_OK;
+}
+
+extern "C" int emu_llm_regress_join(EmuEngine* e, const int32_t* host_slots, const int32_t* host_new, int n, const void* embeds,
+                                    void* out, int L, emu_stream_t stream) {
+  if (!e || !host_slots || !host_new || !embeds || !out || n < 1 || n > kLlmMaxRows || L < 1) return EMU_ERR_INVALID;
+  for (int i = 0; i < n; ++i)
+    if (host_slots[i] < 0 || host_slots[i] >= kLlmMaxRows || host_new[i] < 1) return EMU_ERR_INVALID;
+  if (e->kv_copy) return e->fail(EMU_ERR_UNSUPPORTED, "regression slots with EMU_KV_COPY=1 (no slot mode)");
+  EMU_TRY(slot_mode_ok(e));
+  EMU_TRY(llm_ready(e));
+  EMU_TRY(regress_ready(e));
+  const EmuConfig& c = e->cfg;
+  Segments sg;
+  sg.n = n;
+  EMU_TRY(check_slots(e, host_slots, n, true, &sg.slot));
+  for (int i = 0; i < n; ++i) {
+    if (host_new[i] > c.llm_max_seq)
+      return e->fail(EMU_ERR_INVALID, "slot " + std::to_string(sg.slot.r[i]) + ": prompt of " + std::to_string(host_new[i]) +
+                                          " tokens exceeds llm_max_seq = " + std::to_string(c.llm_max_seq));
+    sg.prefix.r[i] = 0;
+    sg.n_new.r[i] = host_new[i];
+    sg.final_.r[i] = 1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  EMU_TRY(regress_alloc(e, st));
+  EMU_TRY(slot_prefill(e, nullptr, nullptr, 0, nullptr, sg, embeds, 0, nullptr, nullptr, "regression join", st, e->rg_h));
+  // always n_slots rows: a segment's projection is the same bits however many joined with it
+  EMU_TRY(project_rows(e, 1, e->rg_h, e->n_slots, e->rg_r, st));
+  regress_emit_kernel<<<n, 128, 0, st>>>(e->rg_r, e->rg_fb, e->rg_k, (bf16*)out, L, e->proj_down_out, sg.slot, n, e->d_active);
+  count_launch(2);
+  if (cudaGetLastError() != cudaSuccess) return e->fail(EMU_ERR_CUDA, "regression join failed");
+  for (int i = 0; i < n; ++i) e->slots[sg.slot.r[i]].regress = true;
+  return EMU_OK;
+}
+
+extern "C" int emu_llm_regress_step(EmuEngine* e, int B, void* out, int L, emu_stream_t stream) {
+  if (!e || !out || B < 1 || B > kLlmMaxRows || L < 1) return EMU_ERR_INVALID;
+  if (e->kv_copy) return e->fail(EMU_ERR_UNSUPPORTED, "regression slots with EMU_KV_COPY=1 (no slot mode)");
+  EMU_TRY(slot_mode_ok(e));
+  EMU_TRY(llm_ready(e));
+  EMU_TRY(regress_ready(e));
+  EMU_TRY(check_decode_rows(e, B, "regression step with no live slot"));
+  for (int b = 0; b < B; ++b)
+    if (e->slots[b].live() && !e->slots[b].regress)
+      return e->fail(EMU_ERR_STATE, "slot " + std::to_string(b) + " is live but did not join through emu_llm_regress_join");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int w = e->proj_down_out;
+  auto body = [&](cudaStream_t cs, int* nl) {
+    int n_dec = 0;
+    EMU_TRY(project_rows(e, 0, e->rg_fb, B, e->rg_x, cs));
+    EMU_TRY(decode_step_body(e, nullptr, e->rg_x, B, nullptr, e->rg_h, nullptr, -1, cs, &n_dec));
+    EMU_TRY(project_rows(e, 1, e->rg_h, B, e->rg_r, cs));
+    regress_emit_kernel<<<B, 128, 0, cs>>>(e->rg_r, e->rg_fb, e->rg_k, (bf16*)out, L, w, SlotList{}, 0, e->d_active);
+    *nl = n_dec + 3;
+    return cudaGetLastError() == cudaSuccess ? EMU_OK : e->fail(EMU_ERR_CUDA, "regression step failed");
+  };
+  EmuEngine::GraphKey key(B, nullptr, e->rg_x, nullptr, out, nullptr, (const void*)st, L, 2);
+  EMU_TRY(run_graphed(e, key, st, body));
+  for (int b = 0; b < B; ++b) e->slots[b].advance();
+  return EMU_OK;
 }

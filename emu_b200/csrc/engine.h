@@ -45,6 +45,7 @@ struct Slot {
   int group = -1;  // first slot of its beam group, -1 = free
   int kept = 0, own = 0;
   bool grows = false;
+  bool regress = false;  // a regression slot (include/emu_b200_regress.h): joined through emu_llm_regress_join
   bool live() const { return group >= 0; }
   void set_live(int self, int L) { *this = Slot{L, self, 0, L, true}; }
   void set_kept(int K) { *this = Slot{0, -1, K, 0, false}; }
@@ -113,7 +114,13 @@ struct EmuEngine {
   // [kLlmMaxRows] left-pad starts / position offsets of the segments being prefilled (join, extend, mixed step)
   int *d_join_start = nullptr, *d_join_posoff = nullptr;
   int *d_kept_start = nullptr, *d_kept_posoff = nullptr;  // [kLlmMaxRows] a kept slot's real left-pad start / position offset
-  // decode graphs keyed by the baked-in arguments (the last int: slot mode, whose step advances live rows only)
+  // regression slots (include/emu_b200_regress.h), allocated by the first regression join: per slot its feedback
+  // [kLlmMaxRows, width] and next output row [kLlmMaxRows]; the projected rows [kLlmMaxRows, width], and the step's decoder
+  // inputs / final-normed hidden rows [kLlmMaxRows, hidden]
+  emu::bf16 *rg_fb = nullptr, *rg_r = nullptr, *rg_x = nullptr, *rg_h = nullptr;
+  int* rg_k = nullptr;
+  // decode graphs keyed by the baked-in arguments (the last int: 1 = slot mode, whose step advances live rows only;
+  // 2 = a regression step, keyed by (B, embeds = its decoder inputs, hidden = out, ban_id = L))
   typedef std::tuple<int, const void*, const void*, const void*, const void*, const void*, const void*, int, int> GraphKey;
   std::map<GraphKey, cudaGraphExec_t> graphs;
   std::map<GraphKey, int> graph_nodes;

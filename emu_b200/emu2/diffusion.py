@@ -255,8 +255,10 @@ class EmuVisualGeneration:
         return (latents.to(torch.bfloat16).float() * init_noise_sigma).contiguous()
 
     # ---- boundary: Emu2/emu/diffusion.py:168-212 (same inputs, same two modes, same cache keys) ----
-    def _split_prompt(self, inputs, placeholder):
-        """interleaved [str | PIL.Image] -> (text with one placeholder per picture, stacked pictures or None, saw any text)"""
+    @staticmethod
+    def _prompt_text(inputs, placeholder):
+        """interleaved [str | PIL.Image] -> (text with one placeholder per picture, the pictures as given, saw any text);
+        without the picture transform, so a scheduler can size and route a prompt before it is encoded"""
         pieces, pictures, saw_text = [], [], False
         for item in inputs:
             if isinstance(item, str):
@@ -264,9 +266,15 @@ class EmuVisualGeneration:
                 saw_text = True
             else:
                 pieces.append(placeholder)
-                pictures.append(self.transform(item, self.device_))
+                pictures.append(item)
+        return "".join(pieces), pictures, saw_text
+
+    def _split_prompt(self, inputs, placeholder):
+        """interleaved [str | PIL.Image] -> (text with one placeholder per picture, stacked pictures or None, saw any text)"""
+        text, pictures, saw_text = self._prompt_text(inputs, placeholder)
+        pictures = [self.transform(p, self.device_) for p in pictures]
         stacked = torch.stack(pictures).to(self.device_, torch.bfloat16) if pictures else None
-        return "".join(pieces), stacked, saw_text
+        return text, stacked, saw_text
 
     def _unconditional(self, key, make):
         """The classifier-free-guidance branch does not depend on the request: made once per mode, kept in

@@ -217,12 +217,25 @@ class EmuModel:
     @torch.no_grad()
     def generate_image(self, text: List[str], image: Optional[torch.Tensor] = None,
                        placeholder: str = DEFAULT_IMG_PLACEHOLDER):
+        input_ids, attention_mask, IMAGE = self.image_prompt_ids(text, placeholder)
+        return self.generate_image_from_ids(input_ids, attention_mask, image=image, image_token_id=IMAGE)
+
+    def image_prompt_ids(self, text: List[str], placeholder: str = DEFAULT_IMG_PLACEHOLDER):
+        """generate_image's prompts tokenised (left padded): picture placeholders expanded to the query slots and [IMG]
+        appended -> (input_ids, attention_mask, <image> token id).  The regression slots of the continuous image scheduler
+        take their prompts from here too."""
         tok = self.decoder.tokenizer
         IMAGE = tok.convert_tokens_to_ids([DEFAULT_IMAGE_TOKEN])[0]
         text = [t.replace(placeholder, self.image_placeholder) for t in text]
         text = [f"{t}{DEFAULT_IMG_TOKEN}" for t in text]          # iteration 0 of the reference loop (:110-111)
         input_ids, attention_mask = self._tokenize(text)
-        return self.generate_image_from_ids(input_ids, attention_mask, image=image, image_token_id=IMAGE)
+        return input_ids, attention_mask, IMAGE
+
+    @torch.no_grad()
+    def image_prompt_embeds(self, input_ids, image=None, image_token_id=32003):
+        """generate_image's prompt embeddings [B, N, hidden]: the token embeddings with the projected ViT tokens of the
+        pictures spliced into every <image> slot (each is a prompt slot at iteration 0)"""
+        return self.embed_prompt(input_ids.to(self.device_), image, None, image_token_id)
 
     @torch.no_grad()
     def generate_image_from_ids(self, input_ids, attention_mask, image=None, image_token_id=32003):
@@ -230,14 +243,9 @@ class EmuModel:
         (emu.py:109-147).  Causal masking makes that identical to one prefill of `text + [IMG]` followed by
         n_query-1 single-position steps fed with project_up(project_down(h_last)) (SURVEY.md §8a' item 2);
         positions are arange including pads (lm.model is called without position_ids, emu.py:133-138)."""
-        input_ids = input_ids.to(self.device_)
         attention_mask = attention_mask.to(self.device_)
-        B = input_ids.shape[0]
-        embeds = self.engine.llm_embed(input_ids)
-        if image is not None:
-            e = self.encode_image(image)
-            e = self._project_up(e.reshape(-1, e.shape[-1]))
-            embeds[input_ids == image_token_id] = e  # every <image> in the prompt is a prompt slot at iteration 0
+        embeds = self.image_prompt_embeds(input_ids, image, image_token_id)
+        B = embeds.shape[0]
         self.engine.llm_reset()
         hidden, _ = self.engine.llm_prefill(embeds, attention_mask, hf_positions=False, want_hidden=True,
                                             want_logits=False)

@@ -22,7 +22,9 @@ Opt-in continuous batching for chat (`EmuServer(chat_scheduler="continuous")`, `
 runs the pipeline's model under emu_b200/batching.py's SlotScheduler instead — requests join the decode batch between two
 steps and leave it as soon as they are finished, each with its own knobs.  Single GPU only.  The same for image generation
 (`EmuServer(generate_scheduler="continuous")`, `--continuous-generation`): a ContinuousWorker drives a DenoiseSlotScheduler,
-whose latent slots join and leave between UNet steps, each request with its own step count and guidance.
+whose latent slots join and leave between UNet steps, each request with its own step count and guidance.  With
+`generate_encode_steps=R` (`--generate-encode-steps R`) the newcomers' prompts are encoded together in LLaMA regression slots,
+at most R regression steps between two UNet steps, instead of one whole generate_image per newcomer while the live slots wait.
 
 With tensor parallelism (launched under torchrun, one process per GPU) rank 0 serves HTTP and broadcasts every admitted batch;
 the other ranks run `follow()` and execute the same calls, which is what the engine's collectives need.
@@ -192,10 +194,15 @@ def chat_prefix_request(pipeline, inputs, knobs):
     return chat_request(pipeline, inputs, prefix_keys=True, **knobs)
 
 
-def generate_scheduler_for(pipeline, n_slots):
+def generate_scheduler_for(pipeline, n_slots, encode_steps=None):
     """latent slots at the size the demo form always gets: forward's default 1024x1024"""
     from .batching import DenoiseSlotScheduler
-    return DenoiseSlotScheduler(pipeline, n_slots or 4)
+    return DenoiseSlotScheduler(pipeline, n_slots or 4, encode_steps=encode_steps)
+
+
+def encoding_generate_scheduler(encode_steps):
+    """a make_scheduler for image generation whose prompts are encoded in regression slots, encode_steps per UNet step"""
+    return lambda pipeline, n_slots: generate_scheduler_for(pipeline, n_slots, encode_steps=encode_steps)
 
 
 def generate_slot_request(pipeline, inputs, knobs):
@@ -345,11 +352,13 @@ class EmuServer:
     """HTTP front + one worker per pipeline.  `chat` / `generate`: a pipeline or a list of pipelines (the reference's
     --chat-concurrency / --generate-concurrency instances); requests go to the worker with the shortest queue.
     `chat_scheduler` / `generate_scheduler`: "batching" (BatchingWorker, the default) or "continuous" (ContinuousWorker; for
-    generation with max_images_per_batch latent slots)."""
+    generation with max_images_per_batch latent slots).  `generate_encode_steps`: with continuous generation, encode the
+    newcomers' prompts in regression slots, at most this many regression steps between two UNet steps."""
 
     def __init__(self, chat=None, generate=None, host="0.0.0.0", port=9000, max_wait_ms=0.0, max_images_per_batch=4,
                  cache_dir=None, announce=None, max_body_bytes=256 << 20, chat_scheduler="batching",
-                 generate_scheduler="batching", chat_prefix_cache=False, chat_prefill_chunk=None):
+                 generate_scheduler="batching", chat_prefix_cache=False, chat_prefill_chunk=None,
+                 generate_encode_steps=None):
         self.cache_dir = cache_dir
         self.chat_prefix_cache = bool(chat_prefix_cache)
         if self.chat_prefix_cache and chat_scheduler != "continuous":
@@ -360,6 +369,12 @@ class EmuServer:
                              "chat_scheduler='continuous'")
         if self.chat_prefill_chunk is not None and self.chat_prefill_chunk < 1:
             raise ValueError("chat_prefill_chunk must be >= 1, got %d" % self.chat_prefill_chunk)
+        self.generate_encode_steps = None if generate_encode_steps is None else int(generate_encode_steps)
+        if self.generate_encode_steps is not None and generate_scheduler != "continuous":
+            raise ValueError("generate_encode_steps interleaves prompt encoding with the UNet steps of live requests: it needs "
+                             "generate_scheduler='continuous'")
+        if self.generate_encode_steps is not None and self.generate_encode_steps < 1:
+            raise ValueError("generate_encode_steps must be >= 1, got %d" % self.generate_encode_steps)
         self.max_body_bytes = int(max_body_bytes)
         if cache_dir:
             os.makedirs(cache_dir, exist_ok=True)
@@ -386,8 +401,10 @@ class EmuServer:
             raise ValueError("chat_scheduler must be 'batching' or 'continuous', got %r" % (chat_scheduler,))
         # (no announce for generation: the UNet is not tensor parallel, follower ranks hold no generation pipeline)
         if generate_scheduler == "continuous":
+            make_gen = (generate_scheduler_for if self.generate_encode_steps is None
+                        else encoding_generate_scheduler(self.generate_encode_steps))
             self.gen_workers = [ContinuousWorker(p, max_images_per_batch, "emu-gen-%d" % i, generate_slot_request,
-                                                 generate_scheduler_for, "generate")
+                                                 make_gen, "generate")
                                 for i, p in enumerate(as_list(generate))]
         elif generate_scheduler == "batching":
             self.gen_workers = [BatchingWorker(p, "generate", (lambda knobs: max_images_per_batch)
@@ -551,6 +568,9 @@ def main(argv=None):
     ap.add_argument("--prefill-chunk", type=int, default=None, metavar="C",
                     help="with --continuous-batching: a newcomer's prompt is prefilled in chunks of at most C tokens, each in "
                          "the same weight pass as the live requests' next token, so no live request waits for a whole prompt")
+    ap.add_argument("--generate-encode-steps", type=int, default=None, metavar="R",
+                    help="with --continuous-generation: newcomers' prompts are encoded together in LLaMA regression slots, "
+                         "at most R regression steps between two UNet steps, so live requests never wait for a whole encode")
     ap.add_argument("--cache-dir", type=str, default="", help="keep request pictures / results here (the reference always does)")
     ap.add_argument("--safety-checker", action="store_true",
                     help="run the built-in NSFW safety checker (the checkpoint's safety_checker.* weights) on every generated "
@@ -562,6 +582,11 @@ def main(argv=None):
         ap.error("--prefill-chunk prefills newcomers inside the live requests' decode steps: it needs --continuous-batching")
     if args.prefill_chunk is not None and args.prefill_chunk < 1:
         ap.error("--prefill-chunk must be >= 1")
+    if args.generate_encode_steps is not None and not args.continuous_generation:
+        ap.error("--generate-encode-steps interleaves prompt encoding with live requests' UNet steps: it needs "
+                 "--continuous-generation")
+    if args.generate_encode_steps is not None and args.generate_encode_steps < 1:
+        ap.error("--generate-encode-steps must be >= 1")
     logging.basicConfig(level=logging.INFO, format="%(asctime)s %(name)s %(levelname)s %(message)s")
     import torch
     import torch.distributed as dist
@@ -616,7 +641,8 @@ def main(argv=None):
                     announce=make_announce() if world > 1 else None,
                     chat_scheduler="continuous" if args.continuous_batching else "batching",
                     generate_scheduler="continuous" if args.continuous_generation else "batching",
-                    chat_prefix_cache=args.prefix_cache, chat_prefill_chunk=args.prefill_chunk)
+                    chat_prefix_cache=args.prefix_cache, chat_prefill_chunk=args.prefill_chunk,
+                    generate_encode_steps=args.generate_encode_steps)
     log.info("serving on %s:%d (chat x%d, generate x%d)", args.host, srv.port, len(chat), len(gen))
     try:
         srv.serve_forever()
