@@ -87,6 +87,8 @@ PREFIX_SYMBOLS = ["emu_llm_leave_keep", "emu_llm_slot_kept", "emu_llm_copy_prefi
 CHUNKED_SYMBOLS = ["emu_llm_step", "emu_op_rope_kv_write_packed", "emu_op_attn_prefill_packed"]
 # ... and in include/emu_b200_regress.h (regression slots: Emu2-Gen's prompt encoding for every slot at once)
 REGRESS_SYMBOLS = ["emu_llm_regress_join", "emu_llm_regress_step"]
+# ... and in include/emu_b200_spec.h (prompt-lookup speculative decoding: verify / commit, the draft and acceptance kernels)
+SPEC_SYMBOLS = ["emu_llm_verify", "emu_llm_commit", "emu_spec_draft", "emu_spec_accept", "emu_op_attn_verify"]
 # ... and in include/emu_b200_gen_slots.h (latent slots: continuous batching for image generation)
 GEN_SLOT_SYMBOLS = ["emu_denoise_step_slots", "emu_op_denoise_prepare", "emu_op_denoise_euler"]
 # ... and in include/emu_b200_diffusion_ops.h (the diffusion kernels as stand-alone operators)
@@ -382,6 +384,40 @@ class Engine:
         one CUDA graph per (B, out))"""
         self._regress_out("regress_step", out, int(B))
         check(self.lib.emu_llm_regress_step(self.h, int(B), _ptr(out), int(out.shape[1]), _stream()), self.h)
+
+    # ---- speculative decoding (include/emu_b200_spec.h) ----
+    def llm_verify(self, tokens, n, logits=None, next_ids=None, ban_id=-1, ban_rows=0):
+        """one weight pass over tokens[:n] (int32, row 0 the last committed token, then the drafts) at positions L .. L + n - 1
+        of the batch-1 cache: logits [n, vocab] fp32 and / or next_ids [n] int32 (rows < ban_rows without ban_id); the cache
+        length stays L until llm_commit"""
+        c = self.cfg
+        for name, t, need, dt in (("tokens", tokens, n, torch.int32), ("logits", logits, n * c.llm_vocab, torch.float32),
+                                  ("next_ids", next_ids, n, torch.int32)):
+            if t is not None and (t.dtype != dt or t.numel() < need or not t.is_contiguous()):
+                raise ValueError(f"llm_verify: {name} must be a contiguous {dt} tensor of at least {need} elements, got "
+                                 f"{tuple(t.shape)} {t.dtype}")
+        check(self.lib.emu_llm_verify(self.h, _ptr(tokens), int(n), _ptr(logits), _ptr(next_ids), int(ban_id), int(ban_rows),
+                                      _stream()), self.h)
+
+    def llm_commit(self, m):
+        """keep the first m positions the last verify wrote"""
+        check(self.lib.emu_llm_commit(self.h, int(m), _stream()), self.h)
+
+    def spec_draft(self, hist, hist_len, k, max_ngram, max_length, eos_token_id, out, out_len):
+        """the prompt-lookup draft of hist[:hist_len] (device int32 scalars / buffers): out[0] = the last token, out[1:1 + d]
+        the draft, out_len = d"""
+        if out.numel() < 1 + k or hist.dtype != torch.int32 or out.dtype != torch.int32:
+            raise ValueError("spec_draft: int32 buffers, out of at least 1 + k = %d entries" % (1 + k))
+        check(self.lib.emu_spec_draft(_ptr(hist), _ptr(hist_len), int(k), int(max_ngram), int(max_length), int(eos_token_id),
+                                      _ptr(out), _ptr(out_len), _stream()))
+
+    def spec_accept(self, hist, hist_len, tokens, next_ids, n, eos_token_id, max_len, stats):
+        """append the accepted drafts of a verify over tokens[:n] and the token after them to hist; stats[:2] = (tokens
+        appended, finished)"""
+        if hist.numel() < max_len or hist.dtype != torch.int32:
+            raise ValueError("spec_accept: hist must be int32 with room for max_len = %d tokens" % max_len)
+        check(self.lib.emu_spec_accept(_ptr(hist), _ptr(hist_len), _ptr(tokens), _ptr(next_ids), int(n), int(eos_token_id),
+                                       int(max_len), _ptr(stats), _stream()))
 
     def sample_tokens(self, logits, temperature=1.0, top_k=0, top_p=1.0, ban_id=-1, seed=0, offset=0):
         return op_sample_tokens(logits, temperature, top_k, top_p, -1 if ban_id is None else ban_id, seed, offset)
@@ -824,6 +860,18 @@ def op_attn_prefill_rows(q, k, v, scale, causal=False, kv_start=None, kv_row=Non
 
 
 # ---- chunked prefill kernels (include/emu_b200_chunked.h) ----
+def op_attn_verify(q, k_cache, v_cache, pos, scale, row=0, start=None, indir=None, n=None):
+    """the verify attention: q [n, >= H*D] bf16 (head h of row j at [j, h*D:(h+1)*D]), one layer's cache [rows, H, t_max, D];
+    query j sees positions start[0] .. pos[0] + j of cache row `row` (through indir [t_max] if given) -> [n, H*D] bf16"""
+    _, H, t_max, D = k_cache.shape
+    n = q.shape[0] if n is None else n
+    out = torch.empty(n, H * D, dtype=torch.bfloat16, device=q.device)
+    check(load().emu_op_attn_verify(_ptr(q), C.c_long(q.stride(0)), _ptr(k_cache), _ptr(v_cache), int(n), int(H), int(D),
+                                    int(t_max), int(row), _i32(pos, "pos"), _i32(start, "start"), _i32(indir, "indir"),
+                                    C.c_float(scale), _ptr(out), _stream()))
+    return out
+
+
 def op_rope_kv_write_packed(qkv, H, D, rope_cos, rope_sin, k_cache, v_cache, B=0, pos=None, pos_off=None, active=None,
                             q_out=None, seg_row=None, seg_q0=None, seg_new=None, seg_posoff=None):
     """qkv [M, 3*H*D] packed: rows [0, B) decode rows (q -> q_out [B, H*D], k / v at slot pos[b] of row b if active[b]), then

@@ -29,7 +29,7 @@ def _digest():
                                         "../../include/emu_b200_slots.h", "../../include/emu_b200_ops.h",
                                         "../../include/emu_b200_gen_slots.h", "../../include/emu_b200_diffusion_ops.h",
                                         "../../include/emu_b200_prefix.h", "../../include/emu_b200_chunked.h",
-                                        "../../include/emu_b200_regress.h"]:
+                                        "../../include/emu_b200_regress.h", "../../include/emu_b200_spec.h"]:
         p = os.path.join(CSRC, f)
         if os.path.isfile(p):
             h.update(f.encode())

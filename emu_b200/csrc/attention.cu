@@ -243,6 +243,278 @@ int attn_decode(const bf16* q, const bf16* k_cache, const bf16* v_cache, int B, 
 }
 
 // ================================================================================================
+// verify (speculative decoding): NQ <= 8 consecutive queries of ONE sequence, query j at position L + j = pos[0] + j sees
+// keys [start[0], L + j].  Split-KV CTAs (head, split) read every K / V element of their key range once for all NQ queries;
+// the causal limit only touches the last NQ keys.  The splits are combined by the last CTA of a head in split order, so the
+// result does not depend on which CTA finishes last.  Keys at or past L + NQ are never loaded.
+// ================================================================================================
+constexpr int kVerThreads = 128;
+constexpr int kVerMaxSplit = 32;
+
+template <int D, int NQ>
+__global__ void __launch_bounds__(kVerThreads) attn_verify_kernel(
+    const bf16* __restrict__ q, long q_ts, const bf16* __restrict__ k_cache, const bf16* __restrict__ v_cache, int H,
+    int t_max, int row, const int* __restrict__ pos, const int* __restrict__ start, float scale, bf16* out, float* ws_o,
+    float* ws_ml, int* counters, int nsplit, int per_cap, const int* __restrict__ indir) {
+  constexpr int EPL = D / 8;     // K elements per lane in the score phase (8 lanes per key)
+  constexpr int VPL = EPL / 8;   // uint4 per lane
+  constexpr int DV = 4;          // V elements per thread in the P·V phase
+  constexpr int TPR = D / DV;    // threads per V row
+  constexpr int TL = kVerThreads / TPR;  // V rows in flight per CTA pass
+  extern __shared__ __align__(16) float sc[];  // scores / probabilities [NQ][per_cap]
+  __shared__ __align__(16) float qs[NQ][D];
+  __shared__ float red[NQ][kVerThreads / 32];
+  __shared__ float s_m[NQ], s_l[NQ];
+  __shared__ float opart[TL][NQ][D];
+  __shared__ int s_last;
+
+  const int h = blockIdx.x, sp = blockIdx.y;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int L = pos[0];
+  const int t_end = L + NQ;
+  const int t_begin = start ? start[0] : 0;
+  const int per = (t_end - t_begin + nsplit - 1) / nsplit;
+  const int t0 = t_begin + sp * per;
+  const int t1 = min(t0 + per, t_end);
+
+  for (int i = tid; i < NQ * D; i += kVerThreads)
+    qs[i / D][i % D] = __bfloat162float(q[(long)(i / D) * q_ts + (long)h * D + i % D]) * scale;
+  __syncthreads();
+
+  const long row_stride = (long)H * t_max * D;
+  const bf16* kb = k_cache + (long)h * t_max * D;
+  const bf16* vb = v_cache + (long)h * t_max * D;
+
+  // ---- phase 1: scores.  Lane `part` of a key's 8 lanes holds elements (v * 8 + part) * 8 .. + 8: each v is one coalesced
+  // 128-byte row segment, and the float4 reads of qs by the 8 parts fall in distinct banks.
+  const int part = lane & 7, tig = lane >> 3;
+  for (int tb = t0 + warp * 4; tb < t1; tb += 32) {  // warp-uniform trip count; two key groups in flight per trip
+    int tk[2] = {tb + tig, tb + 16 + tig};
+    uint4 kr[2][VPL];
+#pragma unroll
+    for (int g = 0; g < 2; ++g) {
+      if (tk[g] < t1) {
+        const int r = indir ? __ldg(indir + tk[g]) : row;
+        const uint4* p = reinterpret_cast<const uint4*>(kb + r * row_stride + (long)tk[g] * D);
+#pragma unroll
+        for (int v = 0; v < VPL; ++v) kr[g][v] = ldg_stream(p + v * 8 + part);
+      }
+    }
+#pragma unroll
+    for (int g = 0; g < 2; ++g) {
+      float s[NQ];
+#pragma unroll
+      for (int j = 0; j < NQ; ++j) s[j] = 0.f;
+      if (tk[g] < t1) {
+#pragma unroll
+        for (int v = 0; v < VPL; ++v) {
+          const uint32_t k4[4] = {kr[g][v].x, kr[g][v].y, kr[g][v].z, kr[g][v].w};
+          float kf[8];
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            kf[2 * c] = bf16_lo(k4[c]);
+            kf[2 * c + 1] = bf16_hi(k4[c]);
+          }
+          const int e0 = (v * 8 + part) * 8;
+#pragma unroll
+          for (int j = 0; j < NQ; ++j) {
+            const float4 a = *reinterpret_cast<const float4*>(&qs[j][e0]);
+            const float4 b = *reinterpret_cast<const float4*>(&qs[j][e0 + 4]);
+            s[j] += kf[0] * a.x + kf[1] * a.y + kf[2] * a.z + kf[3] * a.w + kf[4] * b.x + kf[5] * b.y + kf[6] * b.z +
+                    kf[7] * b.w;
+          }
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < NQ; ++j) {
+        s[j] += __shfl_xor_sync(0xffffffffu, s[j], 4);
+        s[j] += __shfl_xor_sync(0xffffffffu, s[j], 2);
+        s[j] += __shfl_xor_sync(0xffffffffu, s[j], 1);
+      }
+      if (tk[g] < t1 && part == 0) {
+#pragma unroll
+        for (int j = 0; j < NQ; ++j) sc[j * per_cap + tk[g] - t0] = tk[g] <= L + j ? s[j] : -INFINITY;
+      }
+    }
+  }
+  __syncthreads();
+
+  // ---- phase 2: per-query max, exp, sum ----
+  const int nk = t1 > t0 ? t1 - t0 : 0;
+  float mx[NQ];
+#pragma unroll
+  for (int j = 0; j < NQ; ++j) mx[j] = -INFINITY;
+  for (int i = tid; i < nk; i += kVerThreads)
+#pragma unroll
+    for (int j = 0; j < NQ; ++j) mx[j] = fmaxf(mx[j], sc[j * per_cap + i]);
+#pragma unroll
+  for (int j = 0; j < NQ; ++j) {
+    mx[j] = warp_max(mx[j]);
+    if (lane == 0) red[j][warp] = mx[j];
+  }
+  __syncthreads();
+  if (tid < NQ) {
+    float m = red[tid][0];
+    for (int w = 1; w < kVerThreads / 32; ++w) m = fmaxf(m, red[tid][w]);
+    s_m[tid] = m;
+  }
+  __syncthreads();
+  float ls[NQ];
+#pragma unroll
+  for (int j = 0; j < NQ; ++j) ls[j] = 0.f;
+  for (int i = tid; i < nk; i += kVerThreads) {
+#pragma unroll
+    for (int j = 0; j < NQ; ++j) {
+      const float m = s_m[j];
+      const float p = m == -INFINITY ? 0.f : __expf(sc[j * per_cap + i] - m);
+      sc[j * per_cap + i] = p;
+      ls[j] += p;
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < NQ; ++j) {
+    ls[j] = warp_sum(ls[j]);
+    if (lane == 0) red[j][warp] = ls[j];
+  }
+  __syncthreads();
+  if (tid < NQ) {
+    float l = 0.f;
+    for (int w = 0; w < kVerThreads / 32; ++w) l += red[tid][w];
+    s_l[tid] = l;
+  }
+
+  // ---- phase 3: P·V, each V row loaded once for all NQ queries ----
+  const int dq = tid % TPR, tl = tid / TPR;
+  float acc[NQ][DV];
+#pragma unroll
+  for (int j = 0; j < NQ; ++j)
+#pragma unroll
+    for (int c = 0; c < DV; ++c) acc[j][c] = 0.f;
+#pragma unroll 2
+  for (int t = t0 + tl; t < t1; t += TL) {
+    const int r = indir ? __ldg(indir + t) : row;
+    const uint2 vv = __ldg(reinterpret_cast<const uint2*>(vb + r * row_stride + (long)t * D + dq * DV));
+    const float vf[4] = {bf16_lo(vv.x), bf16_hi(vv.x), bf16_lo(vv.y), bf16_hi(vv.y)};
+#pragma unroll
+    for (int j = 0; j < NQ; ++j) {
+      const float p = sc[j * per_cap + t - t0];
+#pragma unroll
+      for (int c = 0; c < DV; ++c) acc[j][c] += p * vf[c];
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < NQ; ++j)
+#pragma unroll
+    for (int c = 0; c < DV; ++c) opart[tl][j][dq * DV + c] = acc[j][c];
+  __syncthreads();
+
+  const long hs = (long)h * nsplit + sp;
+  for (int i = tid; i < NQ * D; i += kVerThreads) {
+    const int j = i / D, d = i % D;
+    float o = 0.f;
+#pragma unroll
+    for (int w = 0; w < TL; ++w) o += opart[w][j][d];
+    if (nsplit == 1) {
+      const float l = s_l[j];
+      out[(long)j * H * D + (long)h * D + d] = __float2bfloat16_rn(l > 0.f ? o / l : 0.f);
+    } else {
+      ws_o[(hs * NQ + j) * D + d] = o;
+    }
+  }
+  if (nsplit == 1) return;
+  if (tid < NQ) {
+    ws_ml[(hs * NQ + tid) * 2] = s_m[tid];
+    ws_ml[(hs * NQ + tid) * 2 + 1] = s_l[tid];
+  }
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) {
+    const int prev = atomicAdd(&counters[h], 1);
+    s_last = (prev == nsplit - 1);
+    if (s_last) counters[h] = 0;  // self-reset for the next launch / graph replay
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  for (int i = tid; i < NQ * D; i += kVerThreads) {
+    const int j = i / D, d = i % D;
+    const long base = (long)h * nsplit;
+    float M = -INFINITY;
+    for (int s = 0; s < nsplit; ++s) M = fmaxf(M, __ldcg(&ws_ml[((base + s) * NQ + j) * 2]));
+    float Ls = 0.f, O = 0.f;
+    for (int s = 0; s < nsplit; ++s) {
+      const float mi = __ldcg(&ws_ml[((base + s) * NQ + j) * 2]), li = __ldcg(&ws_ml[((base + s) * NQ + j) * 2 + 1]);
+      const float w = li > 0.f ? __expf(mi - M) : 0.f;
+      Ls += li * w;
+      O += __ldcg(&ws_o[((base + s) * NQ + j) * D + d]) * w;
+    }
+    out[(long)j * H * D + (long)h * D + d] = __float2bfloat16_rn(Ls > 0.f ? O / Ls : 0.f);
+  }
+}
+
+size_t attn_verify_workspace_bytes(int H, int D) { return (size_t)H * kVerMaxSplit * 8 * (D + 2) * sizeof(float); }
+
+template <int D, int NQ>
+static int launch_verify(const bf16* q, long q_ts, const bf16* k_cache, const bf16* v_cache, int H, int t_max, int row,
+                         const int* pos, const int* start, float scale, bf16* out, float* ws, int* counters, int nsplit,
+                         int per_cap, cudaStream_t st, const int* indir) {
+  const size_t smem = (size_t)NQ * per_cap * sizeof(float);
+  static size_t mx = 0;
+  if (smem > mx) {
+    if (cudaFuncSetAttribute(attn_verify_kernel<D, NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+      return EMU_ERR_CUDA;
+    mx = smem;
+  }
+  float* ws_o = ws;
+  float* ws_ml = ws + (size_t)H * kVerMaxSplit * 8 * D;
+  attn_verify_kernel<D, NQ><<<dim3(H, nsplit), kVerThreads, smem, st>>>(q, q_ts, k_cache, v_cache, H, t_max, row, pos, start,
+                                                                        scale, out, ws_o, ws_ml, counters, nsplit, per_cap,
+                                                                        indir);
+  return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
+}
+
+template <int D>
+static int verify_dispatch(int n, const bf16* q, long q_ts, const bf16* k_cache, const bf16* v_cache, int H, int t_max, int row,
+                           const int* pos, const int* start, float scale, bf16* out, float* ws, int* counters, int nsplit,
+                           int per_cap, cudaStream_t st, const int* indir) {
+#define EMU_VERIFY_CASE(N)                                                                                              \
+  case N:                                                                                                               \
+    return launch_verify<D, N>(q, q_ts, k_cache, v_cache, H, t_max, row, pos, start, scale, out, ws, counters, nsplit, \
+                               per_cap, st, indir);
+  switch (n) {
+    EMU_VERIFY_CASE(1)
+    EMU_VERIFY_CASE(2)
+    EMU_VERIFY_CASE(3)
+    EMU_VERIFY_CASE(4)
+    EMU_VERIFY_CASE(5)
+    EMU_VERIFY_CASE(6)
+    EMU_VERIFY_CASE(7)
+    EMU_VERIFY_CASE(8)
+  }
+#undef EMU_VERIFY_CASE
+  return EMU_ERR_INVALID;
+}
+
+int attn_verify(const bf16* q, long q_ts, const bf16* k_cache, const bf16* v_cache, int n, int H, int D, int t_max, int row,
+                const int* pos, const int* start, float scale, bf16* out, float* workspace, int* counters, int max_len_hint,
+                cudaStream_t st, const int* indir) {
+  if (D != 64 && D != 128) return EMU_ERR_UNSUPPORTED;
+  if (n < 1 || n > 8 || H < 1 || max_len_hint < 1 || (q_ts % 8)) return EMU_ERR_INVALID;
+  // about 8 CTAs per SM over the heads, and at least 32 keys per split
+  int nsplit = (8 * kNumSMs + H - 1) / H;
+  if (nsplit > max_len_hint / 32) nsplit = max_len_hint / 32;
+  if (nsplit > kVerMaxSplit) nsplit = kVerMaxSplit;
+  if (nsplit < 1) nsplit = 1;
+  const int per_cap = (max_len_hint + nsplit - 1) / nsplit;
+  if ((size_t)8 * per_cap * sizeof(float) > 160 * 1024) return EMU_ERR_UNSUPPORTED;
+  if (D == 128)
+    return verify_dispatch<128>(n, q, q_ts, k_cache, v_cache, H, t_max, row, pos, start, scale, out, workspace, counters,
+                                nsplit, per_cap, st, indir);
+  return verify_dispatch<64>(n, q, q_ts, k_cache, v_cache, H, t_max, row, pos, start, scale, out, workspace, counters, nsplit,
+                             per_cap, st, indir);
+}
+
+// ================================================================================================
 // prefill / encoder flash attention (mma.sync m16n8k16, 4 warps x 16 query rows, 64-key blocks)
 // ================================================================================================
 constexpr int kFaThreads = 128;

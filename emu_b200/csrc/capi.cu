@@ -7,6 +7,7 @@
 #include "../../include/emu_b200_chunked.h"
 #include "../../include/emu_b200_gen_slots.h"
 #include "../../include/emu_b200_diffusion_ops.h"
+#include "../../include/emu_b200_spec.h"
 #include "diffusion_common.h"
 
 using namespace emu;
@@ -197,6 +198,33 @@ extern "C" int emu_op_kv_reorder(void* cache, int Bcap, const int32_t* src_idx, 
   if (n_used_tokens < 1 || n_used_tokens > t_max) return EMU_ERR_INVALID;
   count_launch();
   return kv_reorder((bf16*)cache, Bcap, src_idx, B, outer, n_used_tokens, H, D, t_max, (cudaStream_t)s);
+}
+
+// the verify attention of speculative decoding (include/emu_b200_spec.h), with its own workspace as above
+extern "C" int emu_op_attn_verify(const void* q, long q_ts, const void* k_cache, const void* v_cache, int n, int H, int D,
+                                  int t_max, int row, const int32_t* pos, const int32_t* start, const int32_t* indir,
+                                  float scale, void* out, emu_stream_t s) {
+  if (!q || !k_cache || !v_cache || !pos || !out) return EMU_ERR_INVALID;
+  if (n < 1 || n > 8 || H < 1 || !llm_head_dim_ok(D) || t_max < 1 || row < 0 || q_ts < (long)H * D) return EMU_ERR_INVALID;
+  static float* ws = nullptr;
+  static int* counters = nullptr;
+  static int cap_h = 0, cap_d = 0;
+  if (H > cap_h || D > cap_d) {
+    const int h = H > cap_h ? H : cap_h, d = D > cap_d ? D : cap_d;
+    if (ws) cudaFree(ws);
+    if (counters) cudaFree(counters);
+    ws = nullptr;
+    counters = nullptr;
+    cap_h = cap_d = 0;
+    if (cudaMalloc((void**)&ws, attn_verify_workspace_bytes(h, d)) != cudaSuccess) return EMU_ERR_NOMEM;
+    if (cudaMalloc((void**)&counters, (size_t)h * sizeof(int)) != cudaSuccess) return EMU_ERR_NOMEM;
+    if (cudaMemset(counters, 0, (size_t)h * sizeof(int)) != cudaSuccess) return EMU_ERR_CUDA;
+    cap_h = h;
+    cap_d = d;
+  }
+  count_launch();
+  return attn_verify((const bf16*)q, q_ts, (const bf16*)k_cache, (const bf16*)v_cache, n, H, D, t_max, row, pos, start, scale,
+                     (bf16*)out, ws, counters, t_max, (cudaStream_t)s, indir);
 }
 
 extern "C" int emu_op_argmax_rows(const float* logits, int rows, int cols, int32_t* out, emu_stream_t s) {

@@ -10,6 +10,7 @@
 #include "../../include/emu_b200_prefix.h"
 #include "../../include/emu_b200_regress.h"
 #include "../../include/emu_b200_slots.h"
+#include "../../include/emu_b200_spec.h"
 
 #include <dlfcn.h>
 #include <math.h>
@@ -849,6 +850,7 @@ extern "C" int emu_llm_reset(EmuEngine* e, emu_stream_t s) {
   if (!e) return EMU_ERR_INVALID;
   e->cur_len = 0;
   e->cache_B = 0;
+  e->spec_n = 0;
   e->n_slots = 0;
   e->slots.clear();
   if (e->d_pos && cudaMemsetAsync(e->d_pos, 0, 3 * kLlmMaxRows * sizeof(int), (cudaStream_t)s) != cudaSuccess) return EMU_ERR_CUDA;
@@ -1476,6 +1478,128 @@ extern "C" int emu_llm_decode(EmuEngine* e, const int32_t* token_ids, const void
     e->cur_len += 1;
   }
   return EMU_OK;
+}
+
+// ================================================================================================
+// speculative decoding: verify n consecutive tokens of the batch-1 sequence in one weight pass (include/emu_b200_spec.h)
+// ================================================================================================
+static int spec_alloc(EmuEngine* e) {
+  if (e->sp_idx) return EMU_OK;
+  const EmuConfig& c = e->cfg;
+  bf16* qkv = (bf16*)e->dmalloc((size_t)8 * 3 * e->Hl * c.llm_head_dim * 2);
+  float* ws = (float*)e->dmalloc(attn_verify_workspace_bytes(e->Hl, c.llm_head_dim));
+  int* counters = (int*)e->dmalloc((size_t)e->Hl * sizeof(int));
+  int* idx = (int*)e->dmalloc(16 * sizeof(int));
+  if (!qkv || !ws || !counters || !idx) return e->fail(EMU_ERR_NOMEM, "speculative decoding buffers");
+  int iota[16];
+  for (int i = 0; i < 16; ++i) iota[i] = i;
+  if (cudaMemset(counters, 0, (size_t)e->Hl * sizeof(int)) != cudaSuccess ||
+      cudaMemcpy(idx, iota, sizeof(iota), cudaMemcpyHostToDevice) != cudaSuccess)
+    return e->fail(EMU_ERR_CUDA, "speculative decoding buffers init failed");
+  e->sp_qkv = qkv; e->sp_ws = ws; e->sp_counters = counters; e->sp_idx = idx;
+  return EMU_OK;
+}
+
+// the kernels of one verify (captured into a CUDA graph by emu_llm_verify): the decode step's GEMVs at B = n, the packed
+// RoPE / KV append of one segment (cache row 0, positions d_pos[0] ..), the verify attention, and the lm_head of every row
+static int verify_body(EmuEngine* e, const int32_t* tokens, int n, float* logits, int32_t* next_ids, int ban_id, int ban_rows,
+                       cudaStream_t st, int* n_launch) {
+  const EmuConfig& c = e->cfg;
+  const int Hd = c.llm_hidden, D = c.llm_head_dim, Hl = e->Hl, Fl = e->Fl;
+  const float scale = 1.0f / sqrtf((float)D);
+  const int pdl = 1;
+  int nl = 1;
+  bf16* h = e->dec_h;
+  EMU_TRY(embed_gather(e->embed, tokens, h, n, Hd, st));
+  for (int l = 0; l < c.llm_layers; ++l) {
+    const LlmLayer& L = e->layers[l];
+    bf16* kc = kv_layer(e, l, 0);
+    bf16* vc = kv_layer(e, l, 1);
+    GemvArgs q;
+    q.W = L.wqkv; q.N = 3 * Hl * D; q.K = Hd; q.x = h; q.ldx = Hd; q.B = n;
+    q.norm_w = L.ln1; q.norm_eps = c.llm_rms_eps; q.y = e->sp_qkv; q.ldy = 3 * Hl * D; q.pdl = pdl;
+    EMU_TRY(gemv_bf16(q, st));
+    EMU_TRY(rope_kv_write_packed(e->sp_qkv, n, 0, 1, Hl, D, e->rope_cos, e->rope_sin, nullptr, nullptr, nullptr, nullptr,
+                                 e->sp_idx, e->d_pos, e->sp_idx + n, e->d_posoff, kc, vc, c.llm_max_seq, st));
+    EMU_TRY(attn_verify(e->sp_qkv, 3L * Hl * D, kc, vc, n, Hl, D, c.llm_max_seq, 0, e->d_pos, e->d_start, scale, e->dec_attn,
+                        e->sp_ws, e->sp_counters, c.llm_max_seq, st, e->kv_indir));
+    GemvArgs o;
+    o.W = L.wo; o.N = Hd; o.K = Hl * D; o.x = e->dec_attn; o.ldx = Hl * D; o.B = n; o.pdl = pdl;
+    o.residual = h; o.ldr = Hd; o.y = h; o.ldy = Hd;
+    EMU_TRY(gemv_bf16(o, st));
+    GemvArgs g;
+    g.W = L.wgu; g.N = 2 * Fl; g.K = Hd; g.x = h; g.ldx = Hd; g.B = n;
+    g.norm_w = L.ln2; g.norm_eps = c.llm_rms_eps; g.mode = EPI_SWIGLU; g.y = e->dec_act; g.ldy = Fl; g.pdl = pdl;
+    EMU_TRY(gemv_bf16(g, st));
+    GemvArgs d;
+    d.W = L.wdown; d.N = Hd; d.K = Fl; d.x = e->dec_act; d.ldx = Fl; d.B = n; d.pdl = pdl;
+    d.residual = h; d.ldr = Hd; d.y = h; d.ldy = Hd;
+    EMU_TRY(gemv_bf16(d, st));
+    nl += 6;
+  }
+  if (logits || next_ids) {
+    float* lg = logits ? logits : e->dec_logits_local;
+    GemvArgs g;
+    g.W = e->lm_head; g.N = e->Vl; g.K = Hd; g.x = h; g.ldx = Hd; g.B = n;
+    g.norm_w = e->final_norm; g.norm_eps = c.llm_rms_eps;
+    g.out_fp32 = 1; g.pdl = pdl; g.y = lg; g.ldy = c.llm_vocab;
+    EMU_TRY(gemv_bf16(g, st));
+    ++nl;
+    if (next_ids) {
+      if (ban_id >= 0 && ban_rows > 0) {
+        argmax_ban_kernel<<<ban_rows, 1, 0, st>>>(lg, c.llm_vocab, ban_id);
+        ++nl;
+      }
+      EMU_TRY(argmax_rows(lg, n, c.llm_vocab, next_ids, st));
+      ++nl;
+    }
+  }
+  *n_launch = nl;
+  return cudaGetLastError() == cudaSuccess ? EMU_OK : e->fail(EMU_ERR_CUDA, "verify launch failed");
+}
+
+extern "C" int emu_llm_verify(EmuEngine* e, const int32_t* tokens, int n, float* logits, int32_t* next_ids, int ban_id,
+                              int ban_rows, emu_stream_t stream) {
+  if (!e) return EMU_ERR_INVALID;
+  if (!tokens) return e->fail(EMU_ERR_INVALID, "verify: tokens is null");
+  EMU_TRY(llm_ready(e));
+  const EmuConfig& c = e->cfg;
+  if (e->n_slots > 0) return e->fail(EMU_ERR_STATE, "verify in slot mode (emu_llm_reset leaves it)");
+  if (e->tp_size > 1) return e->fail(EMU_ERR_UNSUPPORTED, "verify under tensor parallelism");
+  if (c.llm_head_dim != 64 && c.llm_head_dim != 128)
+    return e->fail(EMU_ERR_UNSUPPORTED, "verify needs head_dim 64 or 128");
+  if (e->cur_len < 1) return e->fail(EMU_ERR_STATE, "verify before prefill");
+  if (e->cache_B != 1) return e->fail(EMU_ERR_INVALID, "verify needs batch 1, the cache holds " + std::to_string(e->cache_B));
+  const int n_max = c.llm_max_batch < 8 ? c.llm_max_batch : 8;
+  if (n < 1 || n > n_max)
+    return e->fail(EMU_ERR_INVALID, "verify: n = " + std::to_string(n) + " outside [1, min(8, llm_max_batch) = " +
+                                        std::to_string(n_max) + "]");
+  if (ban_rows < 0 || ban_rows > n) return e->fail(EMU_ERR_INVALID, "verify: ban_rows outside [0, n]");
+  if (e->cur_len + n > c.llm_max_seq)
+    return e->fail(EMU_ERR_INVALID, "KV cache full: verify of " + std::to_string(n) + " rows at length " +
+                                        std::to_string(e->cur_len) + " exceeds llm_max_seq " + std::to_string(c.llm_max_seq));
+  EMU_TRY(spec_alloc(e));
+  cudaStream_t st = (cudaStream_t)stream;
+  PdlScope pdl_chain(1);
+  EmuEngine::GraphKey key(n, tokens, nullptr, logits, nullptr, next_ids, (const void*)st, ban_id, 16 + ban_rows);
+  auto body = [&](cudaStream_t cs, int* nl) { return verify_body(e, tokens, n, logits, next_ids, ban_id, ban_rows, cs, nl); };
+  EMU_TRY(run_graphed(e, key, st, body));
+  e->spec_n = n;
+  e->spec_len = e->cur_len;
+  return EMU_OK;
+}
+
+extern "C" int emu_llm_commit(EmuEngine* e, int m, emu_stream_t stream) {
+  if (!e) return EMU_ERR_INVALID;
+  if (e->spec_n < 1 || e->n_slots > 0 || e->spec_len != e->cur_len)
+    return e->fail(EMU_ERR_STATE, "commit without a verify since the cache last changed");
+  if (m < 1 || m > e->spec_n)
+    return e->fail(EMU_ERR_INVALID, "commit: m = " + std::to_string(m) + " outside [1, " + std::to_string(e->spec_n) + "]");
+  e->cur_len += m;
+  e->spec_n = 0;
+  set_int_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(e->d_pos, kLlmMaxRows, e->cur_len);
+  count_launch();
+  return cudaGetLastError() == cudaSuccess ? EMU_OK : e->fail(EMU_ERR_CUDA, "commit failed");
 }
 
 // ================================================================================================

@@ -119,8 +119,15 @@ struct EmuEngine {
   // inputs / final-normed hidden rows [kLlmMaxRows, hidden]
   emu::bf16 *rg_fb = nullptr, *rg_r = nullptr, *rg_x = nullptr, *rg_h = nullptr;
   int* rg_k = nullptr;
+  // speculative decoding (include/emu_b200_spec.h), allocated by the first verify: the verify rows' q|k|v [8, 3 * Hl * D], the
+  // verify attention's split workspace and per-head counters, and sp_idx[i] = i (i <= 8: the one segment's cache row 0 and
+  // row count n for the packed RoPE / KV append).  spec_n = rows of the last verify at cache length spec_len (0: none).
+  emu::bf16* sp_qkv = nullptr;
+  float* sp_ws = nullptr;
+  int *sp_counters = nullptr, *sp_idx = nullptr;
+  int spec_n = 0, spec_len = 0;
   // decode graphs keyed by the baked-in arguments (the last int: 1 = slot mode, whose step advances live rows only;
-  // 2 = a regression step, keyed by (B, embeds = its decoder inputs, hidden = out, ban_id = L))
+  // 2 = a regression step, keyed by (B, embeds = its decoder inputs, hidden = out, ban_id = L); 16 + ban_rows = a verify)
   typedef std::tuple<int, const void*, const void*, const void*, const void*, const void*, const void*, int, int> GraphKey;
   std::map<GraphKey, cudaGraphExec_t> graphs;
   std::map<GraphKey, int> graph_nodes;

@@ -10,6 +10,7 @@
 #include "common.cuh"
 #include "engine.h"
 #include "ops.h"
+#include "../../include/emu_b200_spec.h"
 
 namespace emu {
 
@@ -551,9 +552,91 @@ __global__ void __launch_bounds__(1024) sample_kernel(const float* __restrict__ 
   }
 }
 
+// ---- prompt-lookup speculative decoding (include/emu_b200_spec.h) ----
+// PromptLookupCandidateGenerator.get_candidates (transformers 5.5): n-gram sizes min(max_ngram, len - 1) .. 1; for each, the
+// leftmost window equal to the history's last n-gram whose continuation [idx + g, min(idx + g + k, len, max_length)) is
+// non-empty; the first size with such a window wins; the draft is cut before its first EOS.  No draft when
+// max_length == len + 1.  out[0] = the last history token (row 0 of the next verify), out[1 .. 1 + d) = the draft.
+__global__ void __launch_bounds__(256) spec_draft_kernel(const int* __restrict__ hist, const int* __restrict__ hist_len, int k,
+                                                         int max_ngram, int max_length, int eos_id, int* out, int* out_len) {
+  __shared__ int s_best;
+  const int len = *hist_len;
+  int src = 0, d = 0;
+  if (max_length != len + 1) {
+    for (int g = min(max_ngram, len - 1); g >= 1; --g) {
+      if (threadIdx.x == 0) s_best = INT_MAX;
+      __syncthreads();
+      const int* ng = hist + len - g;
+      for (int idx = threadIdx.x; idx <= len - g; idx += blockDim.x) {
+        const int s = idx + g, e = min(min(s + k, len), max_length);
+        if (s >= e) continue;
+        bool match = true;
+        for (int i = 0; i < g && match; ++i) match = hist[idx + i] == ng[i];
+        if (match) atomicMin(&s_best, idx);
+      }
+      __syncthreads();
+      const int best = s_best;
+      __syncthreads();  // s_best is rewritten by the next size
+      if (best != INT_MAX) {
+        src = best + g;
+        d = min(min(src + k, len), max_length) - src;
+        break;
+      }
+    }
+  }
+  if (threadIdx.x == 0) {
+    int n = 0;
+    while (n < d && hist[src + n] != eos_id) {
+      out[1 + n] = hist[src + n];
+      ++n;
+    }
+    out[0] = hist[len - 1];
+    *out_len = n;
+  }
+}
+
+// accept: a = the leading drafts tokens[1 ..] equal to the verify arg-max next_ids; next_ids[0 .. a] (a accepted drafts and the
+// token after them) are appended to the history, stopping after an EOS and at max_len entries.  stats[0] = m, the tokens
+// appended (the cache positions to commit), stats[1] = 1 when generation has finished.
+__global__ void spec_accept_kernel(int* hist, int* hist_len, const int* __restrict__ tokens, const int* __restrict__ next_ids,
+                                   int n, int eos_id, int max_len, int* stats) {
+  const int len = *hist_len;
+  int a = 0;
+  while (a < n - 1 && tokens[1 + a] == next_ids[a]) ++a;
+  int m = 0, done = 0;
+  for (int i = 0; i <= a && len + m < max_len; ++i) {
+    const int t = next_ids[i];
+    hist[len + m++] = t;
+    if (t == eos_id) {
+      done = 1;
+      break;
+    }
+  }
+  if (len + m >= max_len) done = 1;
+  *hist_len = len + m;
+  stats[0] = m;
+  stats[1] = done;
+}
+
 }  // namespace emu
 
 using namespace emu;
+
+extern "C" int emu_spec_draft(const int32_t* hist, int32_t* hist_len, int k, int max_ngram, int max_length, int eos_id,
+                              int32_t* out, int32_t* out_len, emu_stream_t stream) {
+  if (!hist || !hist_len || !out || !out_len || k < 1 || max_ngram < 1) return EMU_ERR_INVALID;
+  spec_draft_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(hist, hist_len, k, max_ngram, max_length, eos_id, out, out_len);
+  count_launch();
+  return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
+}
+
+extern "C" int emu_spec_accept(int32_t* hist, int32_t* hist_len, const int32_t* tokens, const int32_t* next_ids, int n,
+                               int eos_id, int max_len, int32_t* stats, emu_stream_t stream) {
+  if (!hist || !hist_len || !tokens || !next_ids || !stats || n < 1 || n > 8 || max_len < 1) return EMU_ERR_INVALID;
+  spec_accept_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(hist, hist_len, tokens, next_ids, n, eos_id, max_len, stats);
+  count_launch();
+  return cudaGetLastError() == cudaSuccess ? EMU_OK : EMU_ERR_CUDA;
+}
 
 extern "C" int emu_sample_tokens(const float* logits, int rows, int vocab, float temperature, int top_k, float top_p,
                                  int ban_id, uint64_t seed, uint64_t offset, int32_t* out_ids, emu_stream_t stream) {

@@ -102,6 +102,14 @@ int attn_decode(const bf16* q /*[B, H*D] pair-interleaved like k*/, const bf16* 
                 float* workspace, int* counters, int max_len_hint, int pdl, cudaStream_t st,
                 const int* indir = nullptr /*[rows][t_max] cache row holding token t of sequence b; null = own row*/);
 size_t attn_decode_workspace_bytes(int B, int H, int D);
+// verify (speculative decoding): n <= 8 consecutive queries of one sequence, rows j of q [n, q_ts] (head h at h * D), query j at
+// cache slot pos[0] + j seeing slots [start[0], pos[0] + j] of cache row `row` (through indir [t_max], that row's table, if
+// given); out [n, H*D].  max_len_hint >= pos[0] + n - start[0] sizes the splits.  workspace attn_verify_workspace_bytes(H, D),
+// counters [H] zeroed once (the kernel resets what it uses).
+int attn_verify(const bf16* q, long q_ts, const bf16* k_cache, const bf16* v_cache, int n, int H, int D, int t_max, int row,
+                const int* pos, const int* start, float scale, bf16* out, float* workspace, int* counters, int max_len_hint,
+                cudaStream_t st, const int* indir = nullptr);
+size_t attn_verify_workspace_bytes(int H, int D);
 // prefill / encoder attention (flash style, mma.sync): q,k,v given as strided [B, N, H, D] views
 struct AttnArgs {
   const bf16* q = nullptr; const bf16* k = nullptr; const bf16* v = nullptr;

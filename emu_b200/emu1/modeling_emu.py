@@ -147,7 +147,9 @@ class Emu:
                                    prefix_allowed_tokens_fn=prefix_allowed_tokens_fn,
                                    num_return_sequences=num_return_sequences,
                                    early_stopping=kwargs.get("early_stopping", False), generator=kwargs.get("generator"),
-                                   check_every=kwargs.get("check_every"))
+                                   check_every=kwargs.get("check_every"),
+                                   prompt_lookup_num_tokens=kwargs.get("prompt_lookup_num_tokens"),
+                                   max_matching_ngram_size=kwargs.get("max_matching_ngram_size", 2), prompt_ids=input_ids)
 
     @torch.no_grad()
     def generate_image(self, text: List[str], image: Optional[torch.Tensor] = None,

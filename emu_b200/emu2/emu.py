@@ -211,7 +211,9 @@ class EmuModel:
                                    prefix_allowed_tokens_fn=kwargs.get("prefix_allowed_tokens_fn"),
                                    num_return_sequences=kwargs.get("num_return_sequences", 1),
                                    early_stopping=kwargs.get("early_stopping", False), generator=kwargs.get("generator"),
-                                   check_every=kwargs.get("check_every"))
+                                   check_every=kwargs.get("check_every"),
+                                   prompt_lookup_num_tokens=kwargs.get("prompt_lookup_num_tokens"),
+                                   max_matching_ngram_size=kwargs.get("max_matching_ngram_size", 2), prompt_ids=input_ids)
 
     # ---- Emu2/emu/emu.py:92-153 ----
     @torch.no_grad()

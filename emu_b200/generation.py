@@ -16,6 +16,8 @@ Strategies (the combinations `lm.generate` picks from do_sample / num_beams / pe
   beam_search          num_beams>1 (reference default 5)   every default call; do_sample=True -> HF beam-sample (what the demo
                                                            runs when "do_sample" is ticked with its default num_beams=5)
   contrastive_search   penalty_alpha>0, top_k>1, 1 beam    Emu2/emu/emu.py:166,222 / Emu1 modeling_emu.py:110 forward the knob
+  speculative_greedy_  prompt_lookup_num_tokens=k, greedy, HF prompt-lookup assisted generation (lm.generate's **kwargs): the
+    search             batch 1                             greedy ids, several drafted tokens checked per weight pass
 `num_return_sequences` (Emu1 `num_captions`, modeling_emu.py:113,177) is honoured by beam search (n best hypotheses per prompt) and
 sampling (n independent draws per prompt, one prefill).
 
@@ -423,14 +425,86 @@ def contrastive_search(engine, inputs_embeds, attention_mask, max_new_tokens, eo
     return _finish_rows(prev[:, :n_done].to(torch.int64), eos_token_id, pad_token_id)
 
 
+@torch.no_grad()
+def speculative_greedy_search(engine, inputs_embeds, attention_mask, max_new_tokens, eos_token_id, pad_token_id, k,
+                              max_matching_ngram_size=2, prompt_ids=None, min_length=0):
+    """Greedy search at batch 1 with prompt-lookup speculative decoding (HF assisted generation with
+    `prompt_lookup_num_tokens=k`): the same ids as greedy_search, in fewer passes over the weights.
+
+    The history is prompt_ids (the prompt's token ids, picture positions holding their placeholder ids; may be None) followed
+    by the generated tokens, on the device.  After the prefill every step runs emu_llm_verify over the last committed token
+    and up to k drafted tokens (n = d + 1 rows, one weight pass), emu_spec_accept (the drafts equal to the arg-max before them,
+    then the arg-max after the last of them), emu_spec_draft for the next step, ONE read-back of {tokens appended, finished,
+    next draft length}, and emu_llm_commit of the appended positions.  A draft only changes how many tokens a pass yields:
+    every kept token is the arg-max of the verify row that produced it."""
+    dev = inputs_embeds.device
+    N = inputs_embeds.shape[1]
+    i32 = dict(dtype=torch.int32, device=dev)
+    P = 0 if prompt_ids is None else int(prompt_ids.shape[-1])
+    cap = P + max_new_tokens
+    hist = torch.zeros(cap, **i32)
+    if P:
+        hist[:P].copy_(prompt_ids.reshape(-1))
+    logits = _prefill(engine, inputs_embeds, attention_mask, 1)
+    if min_length > 0:
+        logits[:, eos_token_id] = float("-inf")
+    hist[P:P + 1].copy_(logits.argmax(-1))
+    hist_len = torch.full((1,), P + 1, **i32)
+    # fixed addresses: the verify's CUDA graphs are keyed by their arguments
+    tokens = torch.zeros(k + 1, **i32)      # the verify's rows: the last committed token, then the draft
+    next_ids = torch.zeros(k + 1, **i32)
+    stats = torch.zeros(3, **i32)           # tokens appended, finished, next draft length
+    stats[1:2].copy_((hist[P:P + 1] == eos_token_id) | (max_new_tokens <= 1))
+    engine.spec_draft(hist, hist_len, k, max_matching_ngram_size, cap, eos_token_id, tokens, stats[2:])
+    _, done, d = stats.tolist()
+    n_gen, max_seq = 1, engine.cfg.llm_max_seq
+    while not done:
+        # the cache holds the prompt and every generated token but the last; no row past max_new_tokens or llm_max_seq
+        L = N + n_gen - 1
+        n = 1 + max(0, min(d, max_new_tokens - n_gen - 1, max_seq - L - 1))
+        engine.llm_verify(tokens, n, next_ids=next_ids, ban_id=eos_token_id, ban_rows=max(0, min(n, min_length - n_gen)))
+        engine.spec_accept(hist, hist_len, tokens, next_ids, n, eos_token_id, cap, stats)
+        engine.spec_draft(hist, hist_len, k, max_matching_ngram_size, cap, eos_token_id, tokens, stats[2:])
+        m, done, d = stats.tolist()
+        n_gen += m
+        if not done:
+            engine.llm_commit(m)
+    return _finish_rows(hist[None, P:P + n_gen].to(torch.int64), eos_token_id, pad_token_id)
+
+
+def _speculative_knobs(engine, batch, k, max_matching_ngram_size, do_sample, num_beams, penalty_alpha, top_k, rp, ngram,
+                       prefix_allowed_tokens_fn):
+    """the refusals of prompt-lookup decoding, as HF's assisted generation makes them where it has them: (k, n-gram size)"""
+    if do_sample or num_beams != 1 or batch != 1:
+        raise ValueError("prompt_lookup_num_tokens needs greedy search at batch 1 (no sampling, num_beams = 1), got "
+                         "do_sample=%s, num_beams=%d, batch=%d" % (bool(do_sample), num_beams, batch))
+    if penalty_alpha is not None and penalty_alpha > 0 and top_k is not None and top_k > 1:
+        raise ValueError("prompt_lookup_num_tokens cannot be combined with contrastive search (penalty_alpha)")
+    if rp != 1.0 or ngram or prefix_allowed_tokens_fn is not None:
+        raise NotImplementedError("prompt_lookup_num_tokens with logits processors (repetition_penalty, "
+                                  "no_repeat_ngram_size, prefix_allowed_tokens_fn)")
+    k = int(k)
+    limit = min(7, int(engine.cfg.llm_max_batch) - 1)
+    if k < 1 or k > limit:
+        raise ValueError("prompt_lookup_num_tokens = %d outside [1, %d]: a verify checks at most min(8, llm_max_batch = %d) "
+                         "rows, the last token and k drafts" % (k, limit, engine.cfg.llm_max_batch))
+    g = 2 if max_matching_ngram_size is None else int(max_matching_ngram_size)
+    if g < 1:
+        raise ValueError("max_matching_ngram_size has to be >= 1, got %d" % g)
+    return k, g
+
+
 def generate(engine, inputs_embeds, attention_mask, max_new_tokens, eos_token_id, pad_token_id, do_sample=False, num_beams=1,
              min_length=0, length_penalty=1.0, repetition_penalty=1.0, penalty_alpha=None, top_k=None, top_p=None,
              temperature=None, no_repeat_ngram_size=0, prefix_allowed_tokens_fn=None, num_return_sequences=1,
-             early_stopping=False, generator=None, check_every=None):
+             early_stopping=False, generator=None, check_every=None, prompt_lookup_num_tokens=None, max_matching_ngram_size=2,
+             prompt_ids=None):
     """`lm.generate(inputs_embeds=...)` as the reference calls it (Emu2/emu/emu.py:213-229, Emu1/models/modeling_emu.py:162-179):
     picks the decoding strategy from the knobs the way GenerationMixin (transformers 4.31, the pinned version) does
 
         num_beams == 1, no sampling, penalty_alpha > 0 and top_k > 1   -> contrastive search
+        num_beams == 1, no sampling, prompt_lookup_num_tokens = k      -> speculative greedy search (batch 1; prompt_ids,
+                                                                          the prompt's token ids, are drafted from too)
         num_beams == 1, no sampling                                    -> greedy search
         num_beams == 1, do_sample                                      -> multinomial sampling
         num_beams  > 1                                                 -> beam search / beam-sample (do_sample)
@@ -438,6 +512,13 @@ def generate(engine, inputs_embeds, attention_mask, max_new_tokens, eos_token_id
     and returns the new token ids [B * num_return_sequences, T]."""
     num_beams, rp, ngram, n_ret = decoding_knobs(num_beams, repetition_penalty, no_repeat_ngram_size, num_return_sequences)
     ce = {} if check_every is None else {"check_every": check_every}
+    if prompt_lookup_num_tokens is not None:
+        k, g = _speculative_knobs(engine, inputs_embeds.shape[0], prompt_lookup_num_tokens, max_matching_ngram_size, do_sample,
+                                  num_beams, penalty_alpha, top_k, rp, ngram, prefix_allowed_tokens_fn)
+        if n_ret != 1:
+            raise ValueError("num_return_sequences has to be 1 when doing greedy / contrastive search, got %d" % n_ret)
+        return speculative_greedy_search(engine, inputs_embeds, attention_mask, max_new_tokens, eos_token_id, pad_token_id, k,
+                                         max_matching_ngram_size=g, prompt_ids=prompt_ids, min_length=min_length)
     if num_beams == 1 and not do_sample:
         if n_ret != 1:
             raise ValueError("num_return_sequences has to be 1 when doing greedy / contrastive search, got %d" % n_ret)
